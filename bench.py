@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — NVILA-8B single-image request (BASELINE.json configs[1]) on B200, plus the blocks the
+"""bench.py — NVILA-8B single-image request (BASELINE.json configs[1]) on H100, plus the blocks the
 other BASELINE configs need (all in ONE JSON line, printed by rank 0).
 
 One "step" = one request through the hot path: 1 x 448^2 synthetic image -> SigLIP tower ->
@@ -24,14 +24,18 @@ mm_projector -> text/media splice -> Qwen2-7B prefill (S = 257 visual + 22 text 
   sp_prefill      BASELINE configs[4]: LongVILA 256 frames (S = 65,814), sequence-parallel over ALL
                   ranks of this launch through LlavaLlamaModel.generate(max_new_tokens=1) with
                   vila_b200.sp enabled; first-token id + last-token logits top-5 / checksum so runs at
-                  N = 1/2/4/8 can be compared from the driver's SCALE file alone (strong scaling)
+                  N = 1/2/4/8 can be compared from their JSON lines alone (strong scaling)
   cpu_baseline    the oracle (PyTorch port of the reference's modules) on the host cores: the FULL
                   26-layer tower + projector + 28-layer prefill once, then a bounded number of decode
                   tokens through all 28 layers (no extrapolation); thread count swept and stated
 
 `--impl reference`      the same CPU port as its own arm (rank 0 only).
 `--impl reference_gpu`  informational: HF transformers (SigLIP + Qwen2, sdpa, bf16, eager) on the same
-                        B200 for the same request — the library path the reference would run.
+                        GPU for the same request — the library path the reference would run.
+`--dump-outputs DIR`    after the timed steps, write what the last timed request returned (generated ids,
+                        last prefill hidden state, first-token logits, spliced input embeddings) as
+                        DIR/<name>.npy (float32 / float64).  Inputs are seeded, so two builds run with the
+                        same arguments can be compared output for output.
 Launch with torchrun for N > 1: the decode request does not shard at bs=1 ("replicas only",
 SURVEY §8e): every rank serves its own replica, value = all ranks' tokens / max-over-ranks time; the
 sp_prefill block is the part that really shards.
@@ -66,8 +70,8 @@ def read_peaks():
         return {"hbm_gbs": float(d["hbm_gbs"]), "bf16_tflops": float(d["bf16_tflops"]),
                 "bf16_tflops_sustained": float(d.get("bf16_tflops_sustained", d["bf16_tflops"])),
                 "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0,
-            "source": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0,
+            "source": "H100 SXM data sheet (700 W, dense bf16), not measured"}
 
 
 class ClockSampler:
@@ -134,9 +138,28 @@ def llm_weight_bytes(lc):
     return 2 * (lc.num_hidden_layers * layer_w + lc.vocab_size * lc.hidden_size)
 
 
+def dump_outputs(out_dir, llm, last):
+    """The last timed request's results as DIR/<name>.npy: generated ids (float64), the last prefill
+    hidden state, the first-token logits computed from it and the spliced input embeddings (float32);
+    about 5 MB in all."""
+    import numpy as np
+    import torch
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    hidden = last["hidden"]
+    arrays = {
+        "generated_ids": last["dec"].hist[:NEW_TOKENS].to(torch.float64),
+        "prefill_last_hidden": hidden.float(),
+        "first_token_logits": llm.logits_from_hidden(hidden[None])[0].float(),
+        "input_embeds": last["emb"][0].float(),
+    }
+    for name, t in arrays.items():
+        np.save(d / f"{name}.npy", t.cpu().numpy())
+
+
 def decode_kernel_ledger(model, peaks, ctx=280):
     """Every kernel of one decode step, timed live with CUDA events: each kernel is launched back to
-    back over ALL layers' weights (7.6 GB of gate/up weights etc. >> the 126 MB L2, so every launch
+    back over ALL layers' weights (7.6 GB of gate/up weights etc. >> the 50 MB L2, so every launch
     streams from HBM; PDL lets launch i+1 prefetch under launch i exactly as in the decode graph)."""
     import torch
 
@@ -473,6 +496,7 @@ def run_ours(args):
     ev = lambda: torch.cuda.Event(enable_timing=True)
 
     vision_ms = []
+    last = {}  # what the most recent request_device() computed (for --dump-outputs)
 
     def request_device():
         """inputs resident in HBM; returns (t_ttft_ms, t_decode_ms)."""
@@ -488,6 +512,7 @@ def run_ours(args):
         dec.run(NEW_TOKENS)
         e2.record()
         torch.cuda.synchronize()
+        last.update(emb=emb, hidden=hid[-1], dec=dec)
         vision_ms.append(e0.elapsed_time(ea))  # SigLIP tower + projector + splice
         return e0.elapsed_time(e1), e1.elapsed_time(e2), emb.shape[1]
 
@@ -527,6 +552,8 @@ def run_ours(args):
         barrier()
         t_wall = time.perf_counter() - t_wall0
         launches_timed = _lib.LAUNCHES - launches0
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, llm, last)
         # e2e through the public API (host buffers)
         e2e_full, e2e_first = [], []
         for _ in range(args.steps):
@@ -603,13 +630,6 @@ def run_ours(args):
     weight_bytes_token = llm_weight_bytes(lc)
     gu = next(r for r in ledger if r["kernel"].startswith("gemv gate/up"))
     gemv_bytes, gemv_ms, achieved = gu["algorithmic_bytes"], gu["us"] / 1e3, gu["gbs"]
-    ncu_file = ROOT / "profiles" / "ncu_dominant_kernel.json"
-    traffic = None
-    if ncu_file.exists():
-        try:
-            traffic = json.loads(ncu_file.read_text()).get("dram_bytes_per_launch")
-        except Exception:
-            traffic = None
     vis_avg = sum(vision_ms[:args.steps]) / max(1, min(len(vision_ms), args.steps))
     # TTFT floor: tower (26 evaluated layers) + projector on the tensor pipe, prefill at the ridge
     vit_flops, proj_flops = 936e9 + 1.39e9, 15.0e9
@@ -643,7 +663,7 @@ def run_ours(args):
                    "vision": "SigLIP-so400m/14-448 (26 of 27 layers evaluated: hidden_states[-2])",
                    "projector": cfg.mm_projector_type, "llm": "Qwen2.5-7B architecture",
                    "parallelism": "replicas x%d (decode does not shard at bs=1); sp_prefill block: sp%d" % (world, world),
-                   "l2_policy": "no flush needed: each decode step streams %.2f GB of weights (>> 126 MB L2)"
+                   "l2_policy": "no flush needed: each decode step streams %.2f GB of weights (>> 50 MB L2)"
                                 % (weight_bytes_token / 1e9)},
         "e2e": {"value": round(e2e_decode_tok_s, 2), "unit": "tok/s",
                 "ttft_ms": round(ms_e2e_first, 3), "request_ms": round(ms_e2e_full, 3),
@@ -662,7 +682,7 @@ def run_ours(args):
         "roofline": {"kernel": "gemv_tma_kernel (gate/up SwiGLU GEMV, N=%d K=%d, fused RMSNorm prologue)"
                                % (2 * lc.intermediate_size, lc.hidden_size),
                      "bound": "hbm", "achieved": round(achieved, 1), "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                     "frac": round(achieved / peaks["hbm_gbs"], 4), "traffic": traffic,
+                     "frac": round(achieved / peaks["hbm_gbs"], 4),
                      "peak_source": peaks["source"], "algorithmic_bytes_per_launch": gemv_bytes,
                      "launch_ms": round(gemv_ms, 5)},
         "decode_kernels": ledger,
@@ -784,8 +804,7 @@ class CpuReference:
 
 def pick_threads(ref, candidates=None):
     """CPU decode is a memory-bound GEMV chain: more threads than memory channels need only adds
-    synchronisation cost (128 threads on the 128-CPU B200 host: 26 s per token; 16 threads: 0.18 s).
-    Sweep thread counts upwards on one decode token each, keep the fastest, and stop as soon as a count
+    synchronisation cost.  Sweep thread counts upwards on one decode token each, keep the fastest, and stop as soon as a count
     is more than 2x slower than the best so far (so the sweep itself stays cheap)."""
     import torch
     n = os.cpu_count() or 1
@@ -864,9 +883,9 @@ def run_reference(args):
 
 def run_reference_gpu(args):
     """Informational arm: the library path the reference runs (HF transformers SigLIP + Qwen2, torch
-    sdpa attention, cuBLAS GEMMs, eager launches) on the same B200 for the same request.  The
-    reference's own vendored SigLIP lives under /root/reference (absent on the GPU box); transformers'
-    SiglipVisionModel is the same architecture.  Random-init weights on the device."""
+    sdpa attention, cuBLAS GEMMs, eager launches) on the same GPU for the same request.  The
+    reference's own vendored SigLIP is not part of this project; transformers' SiglipVisionModel is the
+    same architecture.  Random-init weights on the device."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
@@ -960,8 +979,10 @@ def main():
     ap.add_argument("--cpu-budget", type=float, default=25.0)
     ap.add_argument("--frames", type=int, default=256, help="frames of the sp_prefill block")
     ap.add_argument("--sp-steps", type=int, default=10)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed request's outputs to DIR/<name>.npy")
     ap.add_argument("--profile", action="store_true",
-                    help="profiling aid (ncu): 1 warm-up, 8 new tokens, no extra blocks; NOT a valid bench number")
+                    help="profiling aid: 1 warm-up, 8 new tokens, no extra blocks; NOT a valid bench number")
     args = ap.parse_args()
     if args.profile:
         global NEW_TOKENS

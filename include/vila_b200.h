@@ -1,5 +1,5 @@
 /*
- * vila_b200 — C-ABI of the B200-native (sm_100a) VILA multimodal forward hot path.
+ * vila_b200 — C-ABI of the H100-native (sm_90a) VILA multimodal forward hot path.
  *
  * The reference (NVlabs/VILA) has no FFI on this path: every GPU op is a library call made from
  * Python (flash_attn, cuBLAS through nn.Linear, cuDNN through nn.Conv2d, ATen elementwise).  This
@@ -14,7 +14,7 @@
  *     row-major, 16-byte aligned; leading dimensions are in ELEMENTS;
  *   - `stream` is a cudaStream_t passed as void* (NULL = legacy default stream);
  *   - every function returns 0 on success; non-zero on error, message via vila_last_error()
- *     (thread-local). Nothing falls back to the CPU: without an sm_100a device calls fail.
+ *     (thread-local). Nothing falls back to the CPU: without an sm_90a device calls fail.
  *   - no hidden state beyond (a) the per-device stream-K scratch registered with vila_set_workspace and
  *     (b) per-device "function attributes set" flags: KV pool, page tables, workspaces and counters
  *     are caller-allocated.
@@ -56,7 +56,7 @@ int vila_set_workspace(void* ptr, uint64_t bytes);
 int vila_device_info(int* sm_count, int* cc_major, int* cc_minor);
 
 /* ---------------------------------------------------------------------------------------------
- * vila_linear — out[M,N] = epilogue(x[M,K] · w[N,K]^T)        (tcgen05 / TMEM / TMA GEMM)
+ * vila_linear — out[M,N] = epilogue(x[M,K] · w[N,K]^T)        (wgmma / TMA GEMM)
  *   epilogue: (+bias[N]) -> act -> (+residual[row % res_row_mod or row, :])   or SwiGLU:
  *   flags & VILA_FLAG_SWIGLU: w rows are interleaved (gate_0, up_0, gate_1, up_1, ...) and out is
  *   [M, N/2] = silu(gate) * up.
@@ -72,9 +72,9 @@ int vila_linear(const void* x, int64_t ldx, const void* w, int64_t ldw, const vo
                 int M, int N, int K, int act, int flags, void* stream);
 /* test hook: same, forcing the kernel configuration instead of the size heuristic:
  *   64 / 128 / 256   single-CTA tiles 128 x block_n (+1000: deterministic stream-K, +2000: stream-K off)
- *   4128 / 4256      CTA-pair tiles 256 x {128,256} (tcgen05 cta_group::2)
- *   5128             split-K CTA pairs on 128 x 128 tiles (needs <= #SM/2 tiles, K > 64)
- *   3000 / 3001      swap-AB skinny kernel (M <= 512), one CTA / CTA pair per weight block */
+ *   4128 / 4256      CTA-pair tiles 256 x {128,256} (2-CTA cluster, W tile multicast to both CTAs)
+ *   5128             split-K CTA pairs on 128 x 128 tiles, one tile per pair (K > 64)
+ *   3000 / 3001      small-M path (M <= 512): 128 x 128 tiles, single CTAs / CTA pairs (W multicast) */
 int vila_linear_cfg(int block_n, const void* x, int64_t ldx, const void* w, int64_t ldw,
                     const void* bias, const void* residual, int64_t ld_res, int res_row_mod,
                     void* out, int64_t ldo, int M, int N, int K, int act, int flags, void* stream);
@@ -87,7 +87,7 @@ int vila_rmsnorm(void* x_inout, const void* residual_add, const void* weight, vo
                  int cols, float eps, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * vila_fmha — flash attention forward, tcgen05 QK^T / PV with TMEM accumulators.
+ * vila_fmha — flash attention forward, wgmma QK^T / PV with register accumulators.
  *   q/o element (token t, head h, dim d) at  base + t*tok_stride + h*head_stride + d
  *   k/v: if kv_page_stride != 0 the KV cache is paged (128 tokens per page):
  *          element (page p, row r, head h, d) at base + p*kv_page_stride + r*kv_tok_stride + h*kv_head_stride + d
@@ -111,10 +111,9 @@ typedef struct vila_fmha_params {
   float scale;
 } vila_fmha_params;
 int vila_fmha(const vila_fmha_params* p, void* stream);
-/* test hook (like vila_linear_cfg): same, forcing the kernel flavour instead of the size heuristic:
- *   0 heuristic; 1 one query tile per CTA (fmha_fwd_kernel); 2 two query tiles per CTA with ping-pong
- *   softmax warpgroups and the O accumulator in TMEM (fmha2_fwd_kernel; needs Sq > 128, D in 72..96 or 128);
- *   3 / 4: as 2 with every 4th / every 2nd exponential as an FMA-pipe polynomial (measured slower) */
+/* test hook (like vila_linear_cfg): same, forcing the kernel flavour instead of the default:
+ *   0 default; 1 / 2 the wgmma kernel (one 128-row query tile per CTA, two consumer warpgroups);
+ *   3 / 4: as 1 with every 4th / every 2nd exponential as an FMA-pipe polynomial */
 int vila_fmha_cfg(int variant, const vila_fmha_params* p, void* stream);
 
 /* im2col for Conv2d(3,1152,k=14,s=14) (modeling_siglip.py:269-275): pixels [B,C,H,W] ->
@@ -163,10 +162,11 @@ int vila_rope_kv_append(void* qkv, const int32_t* positions, int S, int Hq, int 
 int vila_rope_kv_append_table(void* qkv, const void* rope_table, int S, int Hq, int Hkv, int D,
                               void* k_pool, void* v_pool, const int32_t* page_table, int cache_pos0,
                               void* stream);
-/* Fused q/k/v projection for a short prefill chunk (M <= 384 tokens, head_dim 128):
+/* q/k/v projection for a short prefill chunk (M <= 384 tokens, head_dim 128):
  * qkv = x @ w^T + bias; RoPE on the q and k heads; q heads -> qkv_out[:, :Hq*128]; k / v heads ->
- * the paged pools (k_pool NULL: they stay in qkv_out) — vila_linear followed by vila_rope_kv_append
- * in ONE kernel, bit-identical to the two calls (rope_table: vila_rope_table of the chunk's positions).  Replaces Qwen2Attention's q_proj/k_proj/v_proj +
+ * the paged pools (k_pool NULL: they stay in qkv_out).  Runs the GEMM and then the table-driven
+ * RoPE + KV-append kernel, bit-identical to vila_linear followed by vila_rope_kv_append
+ * (rope_table: vila_rope_table of the chunk's positions).  Replaces Qwen2Attention's q_proj/k_proj/v_proj +
  * apply_rotary_pos_emb + past_key_value.update (modeling_qwen2.py:223-226,99-160,262-266 of the
  * in-tree copy).  Returns 3 (and sets vila_last_error) when the shape is not covered: the caller
  * then issues the two separate calls. */
@@ -227,7 +227,7 @@ int vila_decode_attention_batch(const vila_decode_attn_params* p, int batch, int
                                 int out_stride, int pt_stride, int max_pages, void* stream);
 
 /* Long-context decode attention (video: 16K-66K cached tokens = 34-135 MB of K/V per layer): RoPE +
- * KV append for the new token, then the tcgen05 FMHA kernel in split-KV mode (the G query heads of a
+ * KV append for the new token, then the wgmma FMHA kernel in split-KV mode (the G query heads of a
  * KV group are the query rows of its 128-row tile; K/V pages stream through TMA on
  * Hkv * num_splits CTAs), then a deterministic combine.  split j covers tokens
  * [j*split_tokens, (j+1)*split_tokens) (multiple of 128; num_splits*split_tokens >= max context).

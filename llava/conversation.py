@@ -1,5 +1,5 @@
 """llava/conversation.py — only what `llava.cli.infer` touches: the conversation-mode registry.  The
-sm_100a path tokenises through the tokenizer's chat template (SeparatorStyle.AUTO in the reference,
+sm_90a path tokenises through the tokenizer's chat template (SeparatorStyle.AUTO in the reference,
 llava/utils/tokenizer.py:83-115), so a mode is just a name here."""
 from types import SimpleNamespace
 

@@ -14,5 +14,5 @@ def load(model_path: str, model_base: Optional[str] = None, devices: Optional[Li
         model_path = os.path.join(model_path, "model")
     if devices is not None:
         assert "max_memory" not in kwargs, "`max_memory` should not be set when `devices` is set"
-        kwargs["device"] = f"cuda:{devices[0]}"  # one model replica per GPU: the 8B weights fit one B200
+        kwargs["device"] = f"cuda:{devices[0]}"  # one model replica per GPU: the 8B weights fit one H100
     return load_pretrained_model(model_path, model_name, model_base, **kwargs)[1]

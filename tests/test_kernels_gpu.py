@@ -114,7 +114,7 @@ def test_linear_streamk_epilogues_and_workspace_is_clean(cuda):
 
 @pytest.mark.parametrize("M", [1, 33, 279, 384])
 def test_linear_qkv_rope_fused_equals_two_kernels(cuda, M):
-    """q/k/v projection with RoPE + paged KV append fused into the GEMM epilogue must be bit-identical
+    """vila_linear_qkv_rope (q/k/v projection with RoPE + paged KV append) must be bit-identical
     to vila_linear followed by vila_rope_kv_append (same rounding points), including the pool scatter
     through a permuted page table and a non-zero cache offset."""
     ops = _ops()
@@ -130,7 +130,7 @@ def test_linear_qkv_rope_fused_equals_two_kernels(cuda, M):
     n_pages = (p0 + M + 127) // 128 + 2
     table = torch.randperm(n_pages, generator=torch.Generator().manual_seed(1)).to(torch.int32).to(cuda)
     pools = [torch.zeros(n_pages, 128, Hkv, D, dtype=torch.bfloat16, device=cuda) for _ in range(4)]
-    ref = ops.linear(x, w, b, block_n=3000)  # the same swap-AB GEMM, plain epilogue
+    ref = ops.linear(x, w, b, block_n=3000)  # the same small-M GEMM, plain epilogue
     ops.rope_kv_append(ref, pos, Hq, Hkv, D, inv_freq, pools[0], pools[1], table, p0)
     tab = ops.rope_table(pos, D, inv_freq)
     got = ops.linear_qkv_rope(x, w, b, tab, Hq, Hkv, D, pools[2], pools[3], table, p0)
@@ -311,8 +311,7 @@ def test_fmha_paged(cuda):
     assert rel_err(out, ref) < 1.5e-2
 
 
-# ---- the two-tile kernel (fmha2_fwd_kernel: ping-pong softmax warpgroups, O in TMEM with lazy rescale)
-# forced through vila_fmha_cfg(variant=2); the heuristic only picks it once 256-row CTAs fill 148 SMs --
+# ---- the attention kernel pinned through vila_fmha_cfg(variant=1) and the default dispatch --
 @pytest.mark.parametrize("B", [1, 8, 64])
 def test_fmha2_noncausal_siglip(cuda, B):
     from tests.helpers import report_rel
@@ -322,12 +321,10 @@ def test_fmha2_noncausal_siglip(cuda, B):
     qkv = bf(torch.randn(B * S, 3, H, D, device=cuda, generator=g))
     q, k, v = qkv[:, 0], qkv[:, 1], qkv[:, 2]
     ref = ref_attention(q.view(B, S, H, D), k.view(B, S, H, D), v.view(B, S, H, D), False, D ** -0.5)
-    out2 = ops.fmha(q, k, v, B=B, Sq=S, Sk=S, causal=False, scale=D ** -0.5, variant=2)
     out1 = ops.fmha(q, k, v, B=B, Sq=S, Sk=S, causal=False, scale=D ** -0.5, variant=1)
-    report_rel(f"fmha2 noncausal d=72 B={B}", out2.view(B, S, H, D), ref, 1.5e-2)
     report_rel(f"fmha1 noncausal d=72 B={B}", out1.view(B, S, H, D), ref, 1.5e-2)
     auto = ops.fmha(q, k, v, B=B, Sq=S, Sk=S, causal=False, scale=D ** -0.5)
-    assert torch.equal(auto, out2 if B * H * 4 >= 148 else out1)  # the dispatcher's choice, bit-exact
+    assert torch.equal(auto, out1)  # the default dispatch runs the same kernel, bit-exact
 
 
 @pytest.mark.parametrize("Sq,Sk", [(4096, 4096), (16448, 16448), (2048, 6000), (129, 129), (300, 812)])
@@ -352,18 +349,14 @@ def test_fmha2_causal_gqa_paged(cuda, Sq, Sk):
     k_pool[perm[:n_blk].long()] = kp.view(n_blk, 128, Hkv, D)
     v_pool[perm[:n_blk].long()] = vp.view(n_blk, 128, Hkv, D)
     ref = ref_attention(q[None], k[None], v[None], True, D ** -0.5)[0]
-    out2 = ops.fmha(q, k_pool, v_pool, B=1, Sq=Sq, Sk=Sk, causal=True, scale=D ** -0.5,
-                    page_table=perm, variant=2)
-    report_rel(f"fmha2 causal GQA paged Sq={Sq} Sk={Sk}", out2, ref, 1.5e-2)
     out1 = ops.fmha(q, k_pool, v_pool, B=1, Sq=Sq, Sk=Sk, causal=True, scale=D ** -0.5,
                     page_table=perm, variant=1)
     report_rel(f"fmha1 causal GQA paged Sq={Sq} Sk={Sk}", out1, ref, 1.5e-2)
 
 
 def test_fmha2_lazy_rescale_growing_maxima(cuda):
-    """Scores that keep growing along the KV axis: every KV block raises the row maxima, some by more
-    than the lazy-rescale threshold (2^8 in the exp2 domain) and some by less -> both the deferred and
-    the forced TMEM-O rescale paths run; d=72 and d=128."""
+    """Scores that keep growing along the KV axis: every KV block raises the row maxima, some by a
+    lot and some by little, so the O rescale runs with factors far from and close to 1; d=72 and d=128."""
     from tests.helpers import report_rel
     ops = _ops()
     for (D, H, Hkv, S, causal) in [(128, 8, 2, 2048, True), (72, 16, 16, 1024, False)]:
@@ -373,7 +366,7 @@ def test_fmha2_lazy_rescale_growing_maxima(cuda):
         k = bf(torch.randn(S, Hkv, D, device=cuda, generator=g) * ramp)
         v = bf(torch.randn(S, Hkv, D, device=cuda, generator=g))
         ref = ref_attention(q[None], k[None], v[None], causal, D ** -0.5)[0]
-        for variant in (1, 2, 3, 4):  # 3 / 4: two-tile kernel with every 4th / 2nd exp2 as a polynomial
+        for variant in (1, 3, 4):  # 3 / 4: every 4th / 2nd exp2 as a polynomial
             out = ops.fmha(q, k, v, B=1, Sq=S, Sk=S, causal=causal, scale=D ** -0.5, variant=variant)
             assert torch.isfinite(out.float()).all()
             report_rel(f"fmha{variant} growing maxima d={D}", out, ref, 1.5e-2)
@@ -631,7 +624,7 @@ def test_preprocess_tiles_bit_exact_vs_pil(cuda, w, h, mode):
 @pytest.mark.parametrize("ctx,splits,split_tokens", [(130, 2, 128), (3000, 12, 256), (16448, 33, 512),
                                                      (65814, 37, 1792), (65814, 64, 1152), (1000, 37, 512)])
 def test_decode_attention_split_long_context(cuda, ctx, splits, split_tokens):
-    """vila_decode_attention_split (RoPE + append, tcgen05 FMHA in split-KV mode, combine) vs fp32
+    """vila_decode_attention_split (RoPE + append, wgmma FMHA in split-KV mode, combine) vs fp32
     attention over the whole context; (1000, 37, 512): most splits are empty."""
     from tests.helpers import report_rel
     ops = _ops()

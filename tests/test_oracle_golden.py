@@ -1,5 +1,5 @@
 """CPU: the oracle restatement against the committed golden fixtures, which were produced by the
-REFERENCE's own modules (oracle/gen_golden.py).  No GPU, no /root/reference needed."""
+REFERENCE's own modules (oracle/gen_golden.py).  No GPU, no reference checkout needed."""
 from pathlib import Path
 
 import torch

@@ -138,10 +138,10 @@ def test_sp_public_api_generate_and_forward(world, n_frames):
         assert n_same >= 1, (got_ids, ref_ids)
 
 
-def _cfg5_worker(rank, world, port, ret):
-    """BASELINE configs[4] at its NAMED size on one GPU: 256 frames -> S = 65,814 tokens through the
-    sequence-parallel prefill code path (world 1: two zigzag chunks, zigzag page order) against the oracle
-    evaluated on the device (fp32 = truth, bf16 = the reference's own numerics)."""
+def _cfg5_worker(rank, world, port, n_frames, ret):
+    """BASELINE configs[4] on one GPU: n_frames frames (256 -> S = 65,814 tokens, the named size) through
+    the sequence-parallel prefill code path (world 1: two zigzag chunks, zigzag page order) against the
+    oracle evaluated on the device (fp32 = truth, bf16 = the reference's own numerics)."""
     import torch.distributed as dist
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
@@ -158,8 +158,8 @@ def _cfg5_worker(rank, world, port, ret):
         model = LlavaLlamaModel(cfg, device="cuda").init_random(0, device_rng=True)
         llm = model.llm
         g = torch.Generator(device="cuda").manual_seed(11)
-        frames = torch.randn(256, 3, 448, 448, device="cuda", generator=g).to(torch.bfloat16)
-        vid = model.encoders["video"]([frames], {})[0]                      # [256*257, hidden] bf16
+        frames = torch.randn(n_frames, 3, 448, 448, device="cuda", generator=g).to(torch.bfloat16)
+        vid = model.encoders["video"]([frames], {})[0]                      # [n_frames*257, hidden] bf16
         text = llm.model.embed_tokens.weight[torch.arange(100, 122, device="cuda")]
         seq = torch.cat([text[:14], vid, text[14:]], 0)
         S = seq.shape[0]
@@ -195,15 +195,16 @@ def test_cfg5_named_size_matches_oracle():
     if not torch.cuda.is_available():
         pytest.skip("needs a GPU")
     free, total = torch.cuda.mem_get_info()
-    if total < 150 * 2 ** 30:
-        pytest.skip("needs a 180 GB B200 (fp32 oracle of the 8B model at S = 65.8K)")
+    # the fp32 oracle of the 8B model needs ~150 GB at the named 256 frames; an 80 GB H100 runs the
+    # same path at 128 frames (S = 32,918)
+    n_frames = 256 if total >= 150 * 2 ** 30 else 128
     import torch.multiprocessing as mp
     from tests.helpers import check_close
     ret = mp.Manager().dict()
-    mp.spawn(_cfg5_worker, args=(1, _free_port(), ret), nprocs=1, join=True)
+    mp.spawn(_cfg5_worker, args=(1, _free_port(), n_frames, ret), nprocs=1, join=True)
     S, logits, l32, l16 = ret[0]
-    assert S == 256 * 257 + 22
-    check_close("cfg5 SP prefill last-token logits (S = 65,814, 28 layers)", logits, l32, l16, factor=1.3)
+    assert S == n_frames * 257 + 22
+    check_close("cfg5 SP prefill last-token logits (S = %d, 28 layers)" % S, logits, l32, l16, factor=1.3)
     top2 = torch.topk(l32[0], 2).values
     if float(top2[0] - top2[1]) > 3 * 2 ** -8 * float(l32.abs().max()):
         assert int(torch.argmax(logits[0])) == int(torch.argmax(l32[0]))

@@ -1,4 +1,4 @@
-"""vila_b200 — B200-native (sm_100a) implementation of the VILA multimodal forward hot path.
+"""vila_b200 — H100-native (sm_90a) implementation of the VILA multimodal forward hot path.
 
 `vila_b200.model.LlavaLlamaModel` keeps the reference's `llava.model` API; every GPU op goes through
 the C-ABI in include/vila_b200.h (libvila_b200.so, built in-tree by `python -m vila_b200.build`).

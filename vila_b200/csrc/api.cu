@@ -12,7 +12,7 @@ static inline const bf* cb(const void* p) { return static_cast<const bf*>(p); }
 static inline bf* mb(void* p) { return static_cast<bf*>(p); }
 static inline cudaStream_t st(void* s) { return static_cast<cudaStream_t>(s); }
 
-static int require_sm100() {
+static int require_sm90() {
   static int ok = -1;
   if (ok < 0) {
     int dev = 0, major = 0, minor = 0;
@@ -23,20 +23,20 @@ static int require_sm100() {
       cudaGetLastError();
       return 1;
     }
-    ok = (major == 10) ? 1 : 0;
+    ok = (major == 9 && minor == 0) ? 1 : 0;
     if (!ok) {
-      vb::set_last_error("vila_b200: built for sm_100a only, device is sm_%d%d", major, minor);
+      vb::set_last_error("vila_b200: built for sm_90a only, device is sm_%d%d", major, minor);
     }
   }
   if (ok != 1) {
-    if (ok == 0) vb::set_last_error("vila_b200: built for sm_100a only (no fallback path)");
+    if (ok == 0) vb::set_last_error("vila_b200: built for sm_90a only (no fallback path)");
     return 1;
   }
   return 0;
 }
 #define VB_REQUIRE_DEVICE() \
   do {                      \
-    if (require_sm100()) return 3; \
+    if (require_sm90()) return 3; \
   } while (0)
 
 extern "C" {

@@ -1,7 +1,7 @@
-// vila_b200 — sm_100a PTX helper layer (mbarrier / TMA / tcgen05 / TMEM).
-// Everything in this file is hand-written inline PTX for Blackwell (B200, sm_100a).
-// No CUTLASS / CuTe / Triton. Bit layouts of the UMMA descriptors follow the PTX ISA
-// "tcgen05 matrix descriptor" / "instruction descriptor" tables.
+// vila_b200 — sm_90a PTX helper layer (mbarrier / TMA / clusters / wgmma descriptors).
+// Everything in this file is hand-written inline PTX for Hopper (H100, sm_90a).
+// No CUTLASS / CuTe / Triton. Bit layouts of the matrix descriptors follow the PTX ISA
+// "wgmma matrix descriptor" table.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -127,7 +127,7 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-// make generic-proxy smem writes visible to the async proxy (TMA / UMMA)
+// make generic-proxy smem writes visible to the async proxy (TMA / wgmma)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -195,49 +195,20 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// TMA multicast and thread-block clusters
 // ----------------------------------------------------------------------------------------------
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-  static_assert(kCols == 32 || kCols == 64 || kCols == 128 || kCols == 256 || kCols == 512, "");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// all previously issued tcgen05.mma of this thread arrive (once) on `bar` when they complete
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers bf16/fp16 inputs with fp32 accumulate
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                         uint32_t idesc, uint32_t accumulate) {
+// 2D TMA load delivered to the same shared-memory offset in every CTA of `cta_mask` (this cluster);
+// each destination CTA's mbarrier at the offset of `bar` receives the complete_tx of its copy
+__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* m, uint64_t* bar,
+                                                      int32_t c0, int32_t c1, uint16_t cta_mask) {
   asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;"
       :
-      : "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
+      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0),
+        "r"(c1), "h"(cta_mask)
       : "memory");
 }
-
-// ---- CTA pair (cta_group::2): two SMs of one cluster execute one 256-row UMMA ----
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -253,152 +224,39 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t smem_addr, uint32_t rank) 
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
   return r;
 }
-__device__ __forceinline__ float ld_dsmem_f32(uint32_t cluster_addr) {
-  float v;
-  asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(cluster_addr));
+__device__ __forceinline__ float2 ld_dsmem_v2f(uint32_t cluster_addr) {
+  float2 v;
+  asm volatile("ld.shared::cluster.v2.f32 {%0,%1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(cluster_addr));
   return v;
-}
-__device__ __forceinline__ float4 ld_dsmem_v4f(uint32_t cluster_addr) {
-  float4 v;
-  asm volatile("ld.shared::cluster.v4.f32 {%0,%1,%2,%3}, [%4];"
-               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
-               : "r"(cluster_addr));
-  return v;
-}
-__device__ __forceinline__ void st_dsmem_u32(uint32_t cluster_addr, uint32_t v) {
-  asm volatile("st.shared::cluster.b32 [%0], %1;" ::"r"(cluster_addr), "r"(v) : "memory");
 }
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr)
                : "memory");
 }
-// TMA load into THIS CTA's shared memory whose completion is signalled on an mbarrier that may live
-// in the peer CTA of the pair (bar_cluster_addr is a shared::cluster address, see mapa_u32)
-__device__ __forceinline__ void tma_load_2d_pair(void* smem_dst, const CUtensorMap* m,
-                                                 uint32_t bar_cluster_addr, int32_t c0, int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
-      :
-      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0),
-        "r"(c1)
-      : "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-               : "memory");
-}
-// the leader's previously issued pair-MMAs arrive on the barrier at this offset in BOTH CTAs
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::
-          "r"(smem_u32(bar)),
-      "h"(static_cast<uint16_t>(3))
-      : "memory");
-}
-// D (256 rows: 128 TMEM lanes in each CTA) (+)= A (128 rows from each CTA's smem) * B (N/2 rows from each)
-__device__ __forceinline__ void umma_f16_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                              uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      :
-      : "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
 
-// Instruction descriptor, kind::f16: bf16 x bf16 -> fp32.
-//   [4,6) c_format=1 (F32)  [7,10) a_format=1 (BF16)  [10,13) b_format=1 (BF16)
-//   [15] a_major (0=K,1=MN)  [16] b_major  [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn_major,
-                                                       uint32_t b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | (b_mn_major << 16) |
-         ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor (64-bit):
+// ----------------------------------------------------------------------------------------------
+// wgmma shared-memory matrix descriptor (sm_90a), 64-bit:
 //   [0,14) start_address>>4  [16,30) leading_byte_offset>>4  [32,46) stride_byte_offset>>4
-//   [46,48) version=1 (sm_100)  [49,52) base_offset  [61,64) layout (0 none, 2 SW128, 4 SW64, 6 SW32)
-enum : uint32_t { kLayoutNone = 0, kLayoutSW128 = 2, kLayoutSW64 = 4, kLayoutSW32 = 6 };
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes,
-                                                   uint32_t sbo_bytes, uint32_t layout) {
+//   [49,52) base_offset (0: every swizzle atom here is 1024-byte aligned)  [62,64) layout
+// K-major swizzled operands: SBO = pitch of 8-row groups, LBO unused; a k-step inside the swizzle
+// row advances the start address.  MN-major: LBO = pitch of swizzle-width column blocks along MN,
+// SBO = pitch of 8-row groups along K.
+// ----------------------------------------------------------------------------------------------
+enum : uint32_t { kWgmmaSW128 = 1, kWgmmaSW64 = 2, kWgmmaSW32 = 3 };
+__device__ __forceinline__ uint64_t make_wgmma_desc(uint32_t smem_addr, uint32_t lbo_bytes,
+                                                    uint32_t sbo_bytes, uint32_t layout) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3ffffu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3fffu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3fffu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(layout) << 61;
+  d |= static_cast<uint64_t>(layout) << 62;
   return d;
 }
+// named barrier over `count` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 
-// TMEM -> registers: 32 lanes x 32-bit, N consecutive columns per thread (lane = TMEM datapath row)
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x8(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x8(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-               :
-               : "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-// registers -> TMEM (same shape as tmem_ld_32x32b_x32)
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-      "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-      :
-      : "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]),
-        "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]),
-        "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]),
-        "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]),
-        "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 
 // ----------------------------------------------------------------------------------------------
 // host: TMA descriptor encoding through the driver entry point (no link-time libcuda dependency)

@@ -92,7 +92,7 @@ struct S2Args {
   int out_bh, out_bw;
 };
 // I = index type: uint32_t whenever the item count fits (always for real images) — the 64-bit divisions
-// of the generic version made the kernel instruction-issue bound (ncu r02: 76 % issue active, 0.19 of HBM)
+// of the generic version made the kernel instruction-issue bound
 template <typename I>
 __global__ void s2_merge_kernel(const __nv_bfloat16* __restrict__ tiles,
                                 __nv_bfloat16* __restrict__ out, S2Args a) {
@@ -192,7 +192,7 @@ __global__ void tsp_pool_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat
 }
 
 // the same pooling, 8 channels per thread (16-byte loads / stores, 32-bit index math): the scalar version
-// above moves 2 bytes per load and sat at 0.19 of HBM.  Same order of roundings per channel.
+// above moves 2 bytes per load, too few to keep HBM busy.  Same order of roundings per channel.
 __global__ void tsp_pool_v8_kernel(const uint4* __restrict__ x, uint4* __restrict__ out, int T, int h,
                                    int w, int Cv, int pt, int ph, int pw) {
   griddep_launch_dependents();

@@ -674,12 +674,12 @@ decode_attn_head_kernel(DecodeAttnBatchArgs args) {
 
 // ------------------------------------------------------------------------------------------------
 // long-context decode attention: combine of the split-KV partials written by fmha_decode_split
-// (tcgen05 FMHA kernel in split mode).  out[h, :] = sum_s w_s * O_s[h, :], w_s = 2^(lse_s - max) / sum.
+// (wgmma FMHA kernel in split mode).  out[h, :] = sum_s w_s * O_s[h, :], w_s = 2^(lse_s - max) / sum.
 // Splits are summed in index order (deterministic).
 // ------------------------------------------------------------------------------------------------
 // The split weights are computed once per CTA from lse values fetched in parallel, and the partial rows are
-// fetched 16 at a time: the first version walked the splits three times with one dependent load per step
-// (ncu r02: 23 us for 0.5 MB, a chain of 3 x 33 DRAM latencies).  Same summation order -> same result.
+// fetched 16 at a time, instead of walking the splits three times with one dependent load per step (a
+// chain of DRAM latencies).  Same summation order -> same result.
 constexpr int kCombineMaxSplits = 256;
 __global__ void decode_combine_kernel(const float* __restrict__ o_partial, const float* __restrict__ lse,
                                       __nv_bfloat16* __restrict__ out, int Hq, int D, int splits) {
@@ -797,7 +797,7 @@ int decode_attention(const DecodeAttnParams& p, cudaStream_t stream) {
 // Long-context decode attention in two launches (three without `counters`; all PDL, graph-capturable,
 // position on the device):
 //   1. rope_kv_append on the one new token: RoPE(q, k_new) in place, k/v appended at slot = position
-//   2. fmha_decode_split: the tcgen05 FMHA kernel with the G query heads of a KV group as its query
+//   2. fmha_decode_split: the wgmma FMHA kernel with the G query heads of a KV group as its query
 //      rows and the KV splits as blockIdx.z: K/V pages stream through TMA into the warp-specialised
 //      producer / MMA / softmax pipeline on every SM
 //   3. the combine: by the last split CTA of every KV head inside (2) when `counters` is given, else

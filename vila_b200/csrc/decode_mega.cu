@@ -1,9 +1,8 @@
-// Persistent decode "mega-kernel" for sm_100a: ALL layers of n_tokens greedy decode steps in ONE launch.
+// Persistent decode "mega-kernel" for sm_90a: ALL layers of n_tokens greedy decode steps in ONE launch.
 //
 // Why: at batch 1 the decode step is pure weight streaming (15.2 GB / token).  As separate kernels
-// (5 per layer) every kernel boundary drains the HBM pipe for ~5-7 us (tail, launch, x staging,
-// first-byte latency): measured 3.03 ms / token against 2.3 ms of pure transfer
-// (profiles/r01_gemv_variants.md).  Here one CTA per SM stays resident; each of its 8 warps owns a
+// (5 per layer) every kernel boundary drains the HBM pipe for a few microseconds (tail, launch,
+// x staging, first-byte latency).  Here one CTA per SM stays resident; each of its 8 warps owns a
 // shared-memory ring that its lane 0 keeps filled with cp.async.bulk (1-D TMA) copies of weight-row
 // chunks, and that ring runs AHEAD ACROSS PHASE AND TOKEN BOUNDARIES (weights never depend on
 // activations), so while a CTA waits at a grid barrier or stages the next activation vector its next

@@ -1,4 +1,4 @@
-// Weight-streaming GEMV with TMA bulk copies into per-warp shared-memory rings (sm_100a).
+// Weight-streaming GEMV with TMA bulk copies into per-warp shared-memory rings (sm_90a).
 //
 //   y = W x  (M == 1 decode):  every byte of W is read exactly once from HBM, so the kernel is a pure
 //   bandwidth problem.  Instead of register-staged LDG (in-flight bytes limited by registers) each of
@@ -114,8 +114,7 @@ gemv_tma_kernel(GemvParams p, int rows_per_block, int ksplit, TmaGemvLayout L) {
   }
   griddep_wait();
   // ---- prologue: x arrives as ONE bulk copy (a register-staged loop of dependent LDG -> STS round
-  // trips cost ~0.6 us per 4 KB slice: 6 us for the down projection's 38 KB activation vector, during
-  // which the full weight rings stalled the HBM stream) ----
+  // trips per slice would stall the full weight rings, and with them the HBM stream) ----
   if (lane == 0) {
     if (warp == 0) {
       mbar_arrive_expect_tx(&x_bar[0], x_bytes);
@@ -251,10 +250,9 @@ int gemv_tma_bf16(const GemvParams& p, cudaStream_t stream) {
   int rows_per_block = (p.N + sms - 1) / sms;
   if ((p.flags & 1) && (rows_per_block & 1)) rows_per_block += 1;
   const int grid = (p.N + rows_per_block - 1) / rows_per_block;
-  // Shared-memory budget: (almost) the whole SM.  Measured on B200: under a saturated HBM pipe the
-  // load latency is ~2.5 us, so ~110+ KB must be in flight per SM to sustain the full rate; halving
-  // the rings to let the next kernel's CTA co-reside (PDL) dropped the gate/up GEMV from 97 % to
-  // 76 % of the measured HBM peak (profiles/r01_gemv_variants.md).
+  // Shared-memory budget: (almost) the whole SM (227 KB per block on H100).  Under a saturated HBM
+  // pipe the load latency is a few microseconds, so ~100+ KB must be in flight per SM to sustain the
+  // full rate; the rings are not halved to let the next kernel's CTA co-reside.
   constexpr int kSmemBudget = 220 * 1024;
   // x and the norm weight arrive by bulk copy: 16-byte aligned sources (else: register-staged kernel)
   if ((reinterpret_cast<uintptr_t>(p.x) & 15) || (p.norm_w && (reinterpret_cast<uintptr_t>(p.norm_w) & 15)))

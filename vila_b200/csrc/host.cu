@@ -36,7 +36,7 @@ int num_sms() {
   if (cached[dev] == 0) {
     int n = 0;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    cached[dev] = n > 0 ? n : 148;
+    cached[dev] = n > 0 ? n : 132;
   }
   return cached[dev];
 }

@@ -22,9 +22,9 @@ struct GemmEpilogue {
   float* splitk_ws = nullptr;
   int* splitk_counters = nullptr;
   int split_k = 1;
-  // fused q/k/v projection epilogue (skinny kernel only, head_dim == 128): RoPE on the q and k heads
-  // and the KV-cache append, i.e. what rope_kv_append() does as a separate kernel.  Enabled when
-  // rope_table != nullptr.  N = (rope_hq + 2 rope_hkv) * 128; q heads go to C, k/v heads to the pools.
+  // q/k/v projection + RoPE (gemm_qkv_rope_bf16 only, head_dim == 128): RoPE on the q and k heads
+  // and the KV-cache append after the GEMM.  N = (rope_hq + 2 rope_hkv) * 128; q heads stay in C,
+  // k/v heads go to the pools (or stay in C when the pools are null).
   const __nv_bfloat16* rope_table = nullptr;  // [M, 128]: cos[0..64) | sin[0..64) per token (rope_table())
   __nv_bfloat16* k_pool = nullptr;         // paged pools [pages, 128, Hkv, 128] (nullptr: k/v stay in C)
   __nv_bfloat16* v_pool = nullptr;
@@ -35,8 +35,6 @@ struct GemmEpilogue {
 
 int set_workspace(void* ptr, size_t bytes);
 void get_workspace(void** ptr, size_t* bytes);
-int gemm_skinny_bf16(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int ldw, __nv_bfloat16* C,
-                     int ldc, int M, int N, int K, const GemmEpilogue& epi, int pair, cudaStream_t stream);  // -1: not handled
 int gemm_bf16(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int ldw, __nv_bfloat16* C,
               int ldc, int M, int N, int K, const GemmEpilogue& epi, cudaStream_t stream);
 int gemm_qkv_rope_bf16(const __nv_bfloat16* A, int lda, const __nv_bfloat16* W, int ldw, __nv_bfloat16* C,
@@ -65,10 +63,9 @@ struct FmhaParams {
   float scale;      // softmax scale (1/sqrt(D))
 };
 int fmha_prefill(const FmhaParams& p, cudaStream_t stream);
-int fmha_prefill_cfg(int variant, const FmhaParams& p, cudaStream_t stream);  // 0 auto, 1 one-tile, 2 two-tile
-// poly_every: every n-th exponential on the FMA pipe (0 = none, the default; 4; 2) — test/bench hook
-int fmha_prefill_v2(const FmhaParams& p, cudaStream_t stream, int poly_every = 0);  // -1: shape not handled
-// split-KV mode of the one-tile kernel for decode at long context (see fmha_tcgen05.cu)
+// variant: 0 default, 1 / 2 the wgmma kernel, 3 / 4 with every 4th / 2nd exp2 on the FMA pipe
+int fmha_prefill_cfg(int variant, const FmhaParams& p, cudaStream_t stream);
+// split-KV mode of the attention kernel for decode at long context (see fmha_wgmma.cu)
 // counters != nullptr ([Hq] ints, zero-initialised once): the last split CTA of a head combines into p.o
 int fmha_decode_split(const FmhaParams& p, const int32_t* n_tok_minus_1, int split_tokens,
                       float* o_partial, float* lse, int* counters, cudaStream_t stream);

@@ -132,7 +132,7 @@ rmsnorm_kernel(__nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ 
 
 // ---- warp-per-row variants for LARGE row counts (batched video frames, long prefill) --------------
 // One CTA per row keeps only rows_per_SM * row_bytes = 8 * 2.3 KB = 18 KB of loads in flight per SM
-// for SigLIP's 1152-wide rows (ncu, 65536 rows: 2.0 TB/s = 0.31 of the HBM peak).  Here a warp owns a
+// for SigLIP's 1152-wide rows, too little to cover the HBM latency.  Here a warp owns a
 // row, holds it in registers (no shared memory, no block barrier), and 64 resident warps per SM keep
 // ~150 KB in flight.  Same arithmetic as the CTA-per-row kernels (two-pass variance in fp32).
 constexpr int kWarpRowThreads = 256;
@@ -286,8 +286,7 @@ int rmsnorm_bf16(__nv_bfloat16* x_inout, const __nv_bfloat16* residual_add,
   VB_CHECK(cols * 2 <= 96 * 1024, "rmsnorm: row too long (%d)", cols);
   if (rows == 0) return 0;
   // rows of up to 2048 elements only: at 3584 (Qwen2-7B) the 14 vectors per lane cost 128 registers,
-  // i.e. fewer resident warps, and the warp-per-row form measured SLOWER than one CTA per row
-  // (ncu, 16470 x 3584: 84 vs 57 us)
+  // i.e. fewer resident warps than one CTA per row keeps busy
   if (rows >= kWarpRowMinRows && cols <= 8 * 256) {
     VB_CUDA(launch_pdl(rmsnorm_warp_kernel<8>, dim3((rows + 7) / 8), dim3(kWarpRowThreads), 0, stream,
                        x_inout, residual_add, w, out, rows, cols, eps));

@@ -1,4 +1,4 @@
-"""LlavaLlamaModel — drop-in mirror of the reference VLM wrapper on the sm_100a kernels.
+"""LlavaLlamaModel — drop-in mirror of the reference VLM wrapper on the sm_90a kernels.
 
 Reference surface kept (SURVEY.md §8b):
   class LlavaLlamaModel                       llava/model/language_model/llava_llama.py:41-163
@@ -184,11 +184,11 @@ class LlavaLlamaModel(nn.Module):
                  tokenizer=None):
         super().__init__()
         if not torch.cuda.is_available():
-            raise RuntimeError("vila_b200.LlavaLlamaModel needs a CUDA (sm_100a) device: the hot path "
+            raise RuntimeError("vila_b200.LlavaLlamaModel needs a CUDA (sm_90a) device: the hot path "
                                "has no CPU / eager fallback")
         from .. import _lib
         _lib.load()  # fail loudly if the extension is not built
-        ops.ensure_workspace(device)  # stream-K scratch for the skinny prefill / ViT GEMMs
+        ops.ensure_workspace(device)  # stream-K scratch for the under-filled long-K GEMMs
         self.config = config
         dtype = torch.bfloat16
         self.llm = Qwen2ForCausalLM(config.llm_cfg, device, dtype)

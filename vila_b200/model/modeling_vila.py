@@ -5,7 +5,7 @@ extra `pixel_values` argument), `generate` (:1089-1125: returns `input_ids ++ ou
 `return_output_ids_only`), `generate_content` (:1128-1244), `default_generation_config` (:1246-1258:
 eos_token_id is the tokenizer's single id here, not `stop_token_ids`).  Released NVILA checkpoints
 load through this class (`AutoModel.from_pretrained(..., trust_remote_code=True)`); here it is the
-same module tree and the same sm_100a ops as LlavaLlamaModel, with the remote-code call semantics.
+same module tree and the same sm_90a ops as LlavaLlamaModel, with the remote-code call semantics.
 """
 from __future__ import annotations
 

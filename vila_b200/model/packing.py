@@ -7,7 +7,7 @@ The reference packs a padded batch into ONE row, appends a dummy token (attentio
 flash-attention wrapper takes its unpad path, and lets the patched `_get_unpad_data` hand flash-attn
 `cu_seqlens` built from `seqlens_in_batch`: attention is block-diagonal causal, position ids restart
 per sequence.  Here the packed row goes to Qwen2ForCausalLM.forward(seqlens_in_batch=...), which runs
-the GEMMs / norms once over all packed rows and the tcgen05 FMHA once per sequence segment.
+the GEMMs / norms once over all packed rows and the wgmma FMHA once per sequence segment.
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""mm_projector on the sm_100a kernels — API mirror of MultimodalProjector
+"""mm_projector on the sm_90a kernels — API mirror of MultimodalProjector
 (llava/model/multimodal_projector/base_projector.py:134-252): `forward(x)` with
 `config.mm_projector_type` in {mlp_downsample, mlp_downsample_2x2_fix, mlp_downsample_3x3_fix,
 mlpNx_gelu, linear, identity}; state-dict names `layers.{1,2,4,...}.{weight,bias}`.

@@ -1,4 +1,4 @@
-"""Qwen2 / Llama-style causal LM on the sm_100a kernels (prefill + CUDA-graph decode).
+"""Qwen2 / Llama-style causal LM on the sm_90a kernels (prefill + CUDA-graph decode).
 
 The reference obtains this model from third-party `transformers` (AutoModelForCausalLM,
 llava/model/language_model/builder.py:173-180) and calls `self.llm(inputs_embeds=...)`
@@ -6,7 +6,7 @@ llava/model/language_model/builder.py:173-180) and calls `self.llm(inputs_embeds
 (llava_arch.py:833).  This module keeps that surface (`.model.embed_tokens`, `.model.layers`,
 `.model.norm`, `.lm_head`, `.config`, `.vocab_size`, `forward`, `generate`) and the HF state-dict
 names, while q/k/v and gate/up are stored fused (named parameters are views) so each decoder layer is
-  prefill: RMSNorm -> QKV GEMM -> RoPE+KV-append -> tcgen05 FMHA (paged) -> O GEMM(+res)
+  prefill: RMSNorm -> QKV GEMM -> RoPE+KV-append -> wgmma FMHA (paged) -> O GEMM(+res)
            -> RMSNorm -> gate/up GEMM (SwiGLU epilogue) -> down GEMM(+res)
   decode : [RMSNorm+QKV GEMV] -> [RoPE+append+split-KV attention] -> [O GEMV+res]
            -> [RMSNorm+gate/up GEMV+SwiGLU] -> [down GEMV+res]      (5 launches, CUDA-graphed)
@@ -265,7 +265,7 @@ class Qwen2ForCausalLM(nn.Module):
         dummy token / pad_to_multiple_of rows, mask 0) take no part in attention.  Equivalent of HF
         Qwen2 + flash_attn_varlen_func(cu_seqlens) under the reference's `_get_unpad_data` patch
         (llava/model/utils/packing.py:12-36): GEMMs / norms / RoPE once over all T rows, block-diagonal
-        causal attention as one tcgen05 FMHA launch per segment.  Returns logits [1, T, V]."""
+        causal attention as one wgmma FMHA launch per segment.  Returns logits [1, T, V]."""
         cfg = self.config
         Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
         x = inputs_embeds[0].to(self.dtype).contiguous().clone()
@@ -339,8 +339,7 @@ class Qwen2ForCausalLM(nn.Module):
     # ---- decode ----
     def decoder(self, max_new_tokens: int):
         """Greedy decode engine: the CUDA graph of per-layer kernels (default) or, with
-        VILA_B200_DECODER=mega, the persistent whole-token mega-kernel (measured within 1 % of each
-        other on B200: 3.04 vs 3.06 ms/token, tools/bench_decode.py)."""
+        VILA_B200_DECODER=mega, the persistent whole-token mega-kernel."""
         import os
         kind = MegaDecoder if os.environ.get("VILA_B200_DECODER", "graph") == "mega" else GraphDecoder
         if (self._decoder is None or self._decoder.max_new < max_new_tokens
@@ -549,14 +548,13 @@ class GraphDecoder:
         attention, combine) + lm_head GEMV + finalize"""
         return (7 if self.split_tokens else 5) * self.llm.config.num_hidden_layers + 2
 
-    LONG_CTX = 1024  # above: tcgen05 split-KV path (16.8 us at 2000 tokens vs 24.4 for the SIMT kernel)
+    LONG_CTX = 1024  # above: the wgmma split-KV path
 
     def pick_splits(self, ctx: int):
         """-> (num_splits, split_tokens).  Up to 512 tokens: 0 = one CTA per query head, nothing to
-        combine (a pure latency chain at these sizes; measured equal to the 8-split kernel at 280-410
-        tokens, slower at 1000: tools/bench_decode_attn.py).  Up to 2048: 8 splits = one thread-block cluster
+        combine (a pure latency chain at these sizes).  Up to 2048: 8 splits = one thread-block cluster
         per KV head of the SIMT kernel (DSMEM combine), split_tokens = 0.  Long contexts
-        (video: 16K-66K tokens = 34-135 MB of K/V per layer) are a bandwidth problem: the tcgen05 FMHA
+        (video: 16K-66K tokens = 34-135 MB of K/V per layer) are a bandwidth problem: the wgmma FMHA
         kernel in split-KV mode, one CTA per SM (Hkv * splits <= #SMs), every split a whole number of
         128-token pages and all splits of (nearly) equal length."""
         if self._fixed_splits is not None:
@@ -598,8 +596,8 @@ class GraphDecoder:
                 ops.decode_attention_split(self.qkv, self.position, cache.k(li), cache.v(li),
                                            cache.page_table, self.attn, self.o_partial, self.lse,
                                            llm.inv_freq, Hq, Hkv, D, self.num_splits, self.split_tokens,
-                                           D ** -0.5)  # separate combine launch: measured faster than
-                #                              the fused last-CTA combine (28.6 vs 54 us at 16.4K tokens)
+                                           D ** -0.5)  # separate combine launch (no fused last-CTA combine:
+                #                              one CTA per KV head would walk all partial rows serially)
             else:
                 ops.decode_attention(self.qkv, self.position, cache.k(li), cache.v(li), cache.page_table,
                                      self.attn, self.ws, self.counters, llm.inv_freq, Hq, Hkv, D,

@@ -1,4 +1,4 @@
-"""SigLIP vision tower on the sm_100a kernels.
+"""SigLIP vision tower on the sm_90a kernels.
 
 API mirror of the reference wrappers:
   SiglipVisionTower(VisionTower)          llava/model/multimodal_encoder/siglip_encoder.py:25-36
@@ -6,7 +6,7 @@ API mirror of the reference wrappers:
   VisionTowerDynamicS2 (.scales, .resize_output_to_scale_idx, forward_feature)   :251-271
 State-dict names equal the reference's (`vision_tower.vision_model.encoder.layers.N.self_attn.q_proj.weight`
 ...), but q/k/v live in ONE fused [3C, C] buffer (the named parameters are views into it) so the
-three projections are a single tcgen05 GEMM (SURVEY §2.3 K3).
+three projections are a single wgmma GEMM (SURVEY §2.3 K3).
 """
 from __future__ import annotations
 

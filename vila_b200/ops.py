@@ -106,7 +106,7 @@ def fmha(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, *, B: int, Sq: int, 
          causal: bool, scale: float, out: Optional[torch.Tensor] = None,
          page_table: Optional[torch.Tensor] = None, variant: int = 0) -> torch.Tensor:
     """q [B*Sq, Hq, D] view; k/v either [B*Sk, Hkv, D] views or paged pools [P, 128, Hkv, D].
-    variant (test hook, vila_fmha_cfg): 0 heuristic, 1 one-tile kernel, 2 two-tile kernel."""
+    variant (test hook, vila_fmha_cfg): 0 default, 1 / 2 the wgmma kernel, 3 / 4 with polynomial exp2."""
     _chk(q, "q"); _chk(k, "k"); _chk(v, "v")
     assert q.dim() == 3 and q.stride(2) == 1
     Hq, D = q.shape[1], q.shape[2]
@@ -360,7 +360,7 @@ def decode_attention_split(qkv: torch.Tensor, position: torch.Tensor, k_pool: to
                            o_partial: torch.Tensor, lse: torch.Tensor, inv_freq: torch.Tensor, Hq: int,
                            Hkv: int, D: int, num_splits: int, split_tokens: int, scale: float,
                            counters: Optional[torch.Tensor] = None) -> None:
-    """Long-context decode attention: RoPE + KV append, tcgen05 FMHA in split-KV mode, combine
+    """Long-context decode attention: RoPE + KV append, wgmma FMHA in split-KV mode, combine
     (counters int32 [Hkv], zeroed once: the combine is fused into the split kernel)."""
     assert o_partial.dtype == torch.float32 and o_partial.numel() >= num_splits * Hq * D
     assert lse.dtype == torch.float32 and lse.numel() >= num_splits * Hq

@@ -1,4 +1,4 @@
-"""OpenAI-style chat-completions server on the sm_100a hot path (SURVEY §8 f3).
+"""OpenAI-style chat-completions server on the sm_90a hot path (SURVEY §8 f3).
 
 Mirrors the request / response shapes of the reference's `serving/server.py` (`ChatCompletionRequest`
 :84-95, content parts :45-62, `/chat/completions` :209-300: `data: {chunk}\n\n` server-sent events when

@@ -7,10 +7,10 @@ tokens per byte by B.  Here:
 
   * one paged pool `[L, 2, P, 128, Hkv, D]` holds the K/V of every slot; slot s owns the page-table row
     `page_tables[s]` (vLLM-style indirection: the kernels only ever see (pool, page-table row));
-  * a request is admitted by prefilling it into a free slot (the ordinary tcgen05 prefill path writes
+  * a request is admitted by prefilling it into a free slot (the ordinary wgmma prefill path writes
     straight into that slot's pages), its first token comes from the prefill;
-  * ONE CUDA graph advances all slots by one token: per layer RMSNorm → q/k/v GEMM (swap-AB skinny
-    tcgen05 kernel, M = slots: every weight byte is read once for the whole batch) → batched decode
+  * ONE CUDA graph advances all slots by one token: per layer RMSNorm → q/k/v GEMM (wgmma
+    kernel, M = slots: every weight byte is read once for the whole batch) → batched decode
     attention (`vila_decode_attention_batch`: one CTA per (query head, slot), RoPE + KV append fused,
     per-slot position and page-table row, idle slots skipped) → o-proj GEMM(+res) → RMSNorm → gate/up
     GEMM (SwiGLU epilogue) → down GEMM(+res); then lm_head GEMM, greedy arg-max, embedding gather and

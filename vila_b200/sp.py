@@ -1,4 +1,4 @@
-"""Sequence-parallel prefill (LongVILA, BASELINE config #5) — B200/NVSwitch design.
+"""Sequence-parallel prefill (LongVILA, BASELINE config #5) — NVSwitch design.
 
 Reference (what this replaces):
   inference: zigzag ring attention, llava/eval/vision_niah_vila/eval_vision_niah.py:83-140,
@@ -9,7 +9,7 @@ On NVSwitch every GPU reaches every peer at full bandwidth, and with GQA the KV 
 (2 KiB per token per layer), so the ring's P-1 serialized P2P rounds become ONE all-gather of K,V per
 layer that lands DIRECTLY in the paged KV pool: the page table encodes the zigzag permutation, so
 there is no reorder copy and no cross-rank softmax merge — each rank then runs the ordinary causal
-tcgen05 FMHA for its two query chunks against the (paged) full-length KV.
+wgmma FMHA for its two query chunks against the (paged) full-length KV.
 
 Host logic (partitioning, page tables, padding) is pure Python/torch-CPU and is covered by
 world_size-2 gloo tests; the kernels are the same C-ABI calls as the single-GPU path.
