@@ -221,8 +221,9 @@ int vila_decode_attention(const vila_decode_attn_params* p, void* stream);
 
 /* Batched decode attention for continuous batching over ONE shared paged pool: `batch` sequences, sequence
  * b uses qkv + b*qkv_stride, out + b*out_stride, position[b] (< 0: idle slot, skipped) and the page-table
- * row page_table + b*pt_stride (max_pages <= 32 valid entries: contexts up to 4096 tokens).  ws / counters /
- * num_splits of the struct are ignored.  One CTA per (query head, sequence); RoPE + KV append fused. */
+ * row page_table + b*pt_stride (max_pages <= 32 valid entries: contexts up to 4096 tokens; longer ones:
+ * vila_decode_attention_split_batch).  ws / counters / num_splits of the struct are ignored.  One CTA per
+ * (query head, sequence); RoPE + KV append fused. */
 int vila_decode_attention_batch(const vila_decode_attn_params* p, int batch, int qkv_stride,
                                 int out_stride, int pt_stride, int max_pages, void* stream);
 
@@ -250,6 +251,16 @@ typedef struct vila_decode_attn_split_params {
   float scale;
 } vila_decode_attn_split_params;
 int vila_decode_attention_split(const vila_decode_attn_split_params* p, void* stream);
+
+/* Batched form of vila_decode_attention_split for continuous batching at video contexts, over ONE shared
+ * paged pool: sequence b uses qkv + b*qkv_stride, out + b*out_stride, position[b] (< 0: idle slot, skipped
+ * entirely) and the page-table row page_table + b*pt_stride.  o_partial / lse / counters grow by `batch`:
+ * batch*num_splits*Hq*D floats, batch*num_splits*Hq floats and batch*Hkv ints; counters are required
+ * (zero before the first launch, self-cleaning).  Split CTAs past a sequence's length exit at once.
+ * Every non-idle sequence's output and appended K/V are bit-identical to vila_decode_attention_split with
+ * counters on that sequence alone with the same num_splits / split_tokens. */
+int vila_decode_attention_split_batch(const vila_decode_attn_split_params* p, int batch, int qkv_stride,
+                                      int out_stride, int pt_stride, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * vila_decode_mega — n_tokens greedy decode steps of the whole LLM in ONE persistent launch

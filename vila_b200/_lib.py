@@ -106,6 +106,7 @@ SIGNATURES = {
     "vila_decode_attention": [C.POINTER(DecodeAttnParams), c_void_p],
     "vila_decode_attention_batch": [C.POINTER(DecodeAttnParams), c_int, c_int, c_int, c_int, c_int, c_void_p],
     "vila_decode_attention_split": [C.POINTER(DecodeAttnSplitParams), c_void_p],
+    "vila_decode_attention_split_batch": [C.POINTER(DecodeAttnSplitParams), c_int, c_int, c_int, c_int, c_void_p],
     "vila_decode_mega": [C.POINTER(MegaParams), c_void_p],
 }
 _RESTYPES = {"vila_last_error": C.c_char_p}

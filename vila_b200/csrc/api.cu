@@ -303,6 +303,26 @@ int vila_decode_attention_split(const vila_decode_attn_split_params* p, void* st
   return vb::decode_attention_split(d, st(stream));
 }
 
+int vila_decode_attention_split_batch(const vila_decode_attn_split_params* p, int batch, int qkv_stride,
+                                      int out_stride, int pt_stride, void* stream) {
+  VB_REQUIRE_DEVICE();
+  vb::DecodeAttnSplitParams d;
+  d.qkv = mb(p->qkv);
+  d.position = p->position;
+  d.k_pool = mb(p->k_pool);
+  d.v_pool = mb(p->v_pool);
+  d.page_table = p->page_table;
+  d.kv_num_pages = p->kv_num_pages;
+  d.out = mb(p->out);
+  d.o_partial = p->o_partial;
+  d.lse = p->lse;
+  d.counters = p->counters;
+  d.inv_freq = p->inv_freq;
+  d.Hq = p->Hq; d.Hkv = p->Hkv; d.D = p->D; d.num_splits = p->num_splits; d.split_tokens = p->split_tokens;
+  d.scale = p->scale;
+  return vb::decode_attention_split_batch(d, batch, qkv_stride, out_stride, pt_stride, st(stream));
+}
+
 int vila_decode_mega(const vila_mega_params* p, void* stream) {
   VB_REQUIRE_DEVICE();
   static_assert(sizeof(vila_mega_layer) == sizeof(vb::MegaLayer), "layer struct mismatch");

@@ -252,12 +252,16 @@ __global__ void embed_splice_kernel(const uint4* __restrict__ table, const uint4
 // heads of a fused [S, (Hq+2Hkv)*D] buffer + KV append into the paged pool.
 // cos/sin are computed in fp32 and rounded to bf16 like HF (cos.to(dtype)); products are rounded
 // to bf16 before the sum as the reference's bf16 tensor ops do.
+// Row s of qkv starts at qkv + s*row_stride.  Decode (cache_pos0 < 0) of a batch of sequences: row s
+// uses the page-table row page_table + s*pt_stride, and a negative position marks an idle row that is
+// left untouched.
 __global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* __restrict__ pos,
                                int S, int Hq, int Hkv, int D,
                                const float* __restrict__ inv_freq_tab,
                                __nv_bfloat16* __restrict__ k_pool,
                                __nv_bfloat16* __restrict__ v_pool,
-                               const int32_t* __restrict__ page_table, int cache_pos0) {
+                               const int32_t* __restrict__ page_table, int cache_pos0,
+                               long row_stride, int pt_stride) {
   griddep_launch_dependents();
   griddep_wait();
   const int half = D / 2;
@@ -269,7 +273,8 @@ __global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* _
     long t = idx / half;
     const int hh = t % Ht;
     const int s = t / Ht;
-    __nv_bfloat16* base = qkv + ((long)s * Ht + hh) * D;
+    if (cache_pos0 < 0 && pos[s] < 0) continue;  // idle decode row
+    __nv_bfloat16* base = qkv + (long)s * row_stride + (long)hh * D;
     float x0 = __bfloat162float(base[i]), x1 = __bfloat162float(base[i + half]);
     if (hh < Hq + Hkv) {
       const float ang = (float)pos[s] * inv_freq_tab[i];
@@ -288,7 +293,7 @@ __global__ void rope_kv_kernel(__nv_bfloat16* __restrict__ qkv, const int32_t* _
       // cache_pos0 < 0: the cache slot is the position id itself (decode: the position lives in
       // device memory so that one captured graph serves every step)
       const int cpos = cache_pos0 < 0 ? pos[s] : cache_pos0 + s;
-      const int page = page_table[cpos >> 7];
+      const int page = page_table[(long)s * pt_stride + (cpos >> 7)];
       const int hk = (hh - Hq) % Hkv;
       __nv_bfloat16* pool = (hh < Hq + Hkv) ? k_pool : v_pool;
       __nv_bfloat16* dst = pool + (((long)page * 128 + (cpos & 127)) * Hkv + hk) * D;
@@ -554,7 +559,23 @@ int rope_kv_append(__nv_bfloat16* qkv, const int32_t* positions, int S, int Hq, 
   if (S == 0) return 0;
   const long total = (long)S * (Hq + 2 * Hkv) * (D / 2);
   VB_CUDA(launch_pdl(rope_kv_kernel, dim3(grid_for(total, 256)), dim3(256), 0, stream, qkv, positions, S, Hq, Hkv, D, inv_freq,
-                                                          k_pool, v_pool, page_table, cache_pos0));
+                                                          k_pool, v_pool, page_table, cache_pos0,
+                     (long)(Hq + 2 * Hkv) * D, 0));
+  return 0;
+}
+
+int rope_kv_append_decode_batch(__nv_bfloat16* qkv, long qkv_stride, const int32_t* positions, int batch,
+                                int Hq, int Hkv, int D, const float* inv_freq, __nv_bfloat16* k_pool,
+                                __nv_bfloat16* v_pool, const int32_t* page_table, int pt_stride,
+                                cudaStream_t stream) {
+  VB_CHECK(D % 2 == 0, "rope: head dim must be even");
+  VB_CHECK(k_pool != nullptr && v_pool != nullptr && page_table != nullptr,
+           "rope_kv_append_decode_batch: pools and page table required");
+  VB_CHECK(batch >= 1 && qkv_stride >= (long)(Hq + 2 * Hkv) * D && pt_stride >= 1,
+           "rope_kv_append_decode_batch: bad batch %d / strides", batch);
+  const long total = (long)batch * (Hq + 2 * Hkv) * (D / 2);
+  VB_CUDA(launch_pdl(rope_kv_kernel, dim3(grid_for(total, 256)), dim3(256), 0, stream, qkv, positions, batch, Hq,
+                     Hkv, D, inv_freq, k_pool, v_pool, page_table, -1, qkv_stride, pt_stride));
   return 0;
 }
 

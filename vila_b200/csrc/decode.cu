@@ -845,6 +845,52 @@ int decode_attention_split(const DecodeAttnSplitParams& p, cudaStream_t stream) 
 }
 
 
+// Batched long-context decode attention (continuous batching at video contexts): the two launches of
+// decode_attention_split with the fused combine, over `batch` sequences at once.  Sequence b's output is
+// bit-identical to decode_attention_split on that sequence alone with the same split configuration.
+int decode_attention_split_batch(const DecodeAttnSplitParams& p, int batch, int qkv_stride, int out_stride,
+                                 int pt_stride, cudaStream_t stream) {
+  VB_CHECK(p.D == 128, "decode_attention_split_batch: head_dim must be 128 (got %d)", p.D);
+  VB_CHECK(p.Hq % p.Hkv == 0, "decode_attention_split_batch: Hq %% Hkv != 0");
+  VB_CHECK(batch >= 1, "decode_attention_split_batch: bad batch %d", batch);
+  VB_CHECK(p.num_splits >= 1 && p.split_tokens > 0 && p.split_tokens % 128 == 0,
+           "decode_attention_split_batch: bad split configuration (%d x %d)", p.num_splits, p.split_tokens);
+  VB_CHECK(p.counters != nullptr, "decode_attention_split_batch: counters are required");
+  VB_CHECK(qkv_stride >= (p.Hq + 2 * p.Hkv) * p.D && qkv_stride % 8 == 0 && out_stride >= p.Hq * p.D &&
+               pt_stride >= 1,
+           "decode_attention_split_batch: bad strides (qkv %d, out %d, page table %d)", qkv_stride, out_stride,
+           pt_stride);
+  const int G = p.Hq / p.Hkv;
+  int rc = rope_kv_append_decode_batch(p.qkv, qkv_stride, p.position, batch, p.Hq, p.Hkv, p.D, p.inv_freq,
+                                       p.k_pool, p.v_pool, p.page_table, pt_stride, stream);
+  if (rc) return rc;
+  FmhaParams f;
+  f.q = p.qkv;
+  f.q_tok_stride = p.D;
+  f.q_head_stride = static_cast<int64_t>(G) * p.D;
+  f.k = p.k_pool;
+  f.v = p.v_pool;
+  f.kv_page_stride = static_cast<int64_t>(128) * p.Hkv * p.D;
+  f.kv_tok_stride = static_cast<int64_t>(p.Hkv) * p.D;
+  f.kv_head_stride = p.D;
+  f.kv_num_pages = p.kv_num_pages;
+  f.page_table = p.page_table;
+  f.page_table_stride = pt_stride;
+  f.o = p.out;
+  f.o_tok_stride = p.D;
+  f.o_head_stride = static_cast<int64_t>(G) * p.D;
+  f.B = p.num_splits;
+  f.Sq = G;
+  f.Sk = p.split_tokens;
+  f.Hq = p.Hkv;
+  f.Hkv = p.Hkv;
+  f.D = p.D;
+  f.causal = 0;
+  f.scale = p.scale;
+  return fmha_decode_split(f, p.position, p.split_tokens, p.o_partial, p.lse, p.counters, stream, batch,
+                           qkv_stride, out_stride);
+}
+
 int decode_attention_batch(const DecodeAttnParams& p, int batch, int qkv_stride, int out_stride,
                            int pt_stride, int max_pages, cudaStream_t stream) {
   VB_CHECK(p.D == 128, "decode_attention_batch: head_dim must be 128 (got %d)", p.D);

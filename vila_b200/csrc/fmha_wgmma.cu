@@ -77,6 +77,14 @@ struct FmhaKernelArgs {
   float* o_partial;  // [splits][Hq][Sq][D]
   float* lse_out;    // [splits][Hq][Sq]
   int* split_counters;  // [Hq] zero-initialised, self-cleaning; non-null: the last CTA of a head combines into o
+  // batched split mode (fmha_decode_split with batch > 0): blockIdx.x is the sequence.  Sequence s reads
+  // sk_dev[s] (< 0: idle, every CTA exits), the page-table row page_table + s*page_table_stride and the
+  // Q rows at 4th tensor-map coordinate s; its partials, lse and counters are the s-th [splits][Hq][Sq]
+  // block, its output starts at o + s*o_seq_stride.  Split CTAs past the sequence's length exit without
+  // writing anything and the combine reads only the splits that hold tokens (the skipped ones would add
+  // exact zeros: same bits as the single-sequence combine over all splits).
+  int batched;
+  int64_t o_seq_stride;
 };
 
 // kPolyEvery: every n-th exponential of a thread's row values uses ex2_poly (0: none)
@@ -102,8 +110,10 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   // causal: heaviest (last) query tiles first
-  const int qt = a.causal ? static_cast<int>(gridDim.x) - 1 - static_cast<int>(blockIdx.x)
-                          : static_cast<int>(blockIdx.x);
+  const int qt = a.batched ? 0
+                 : a.causal ? static_cast<int>(gridDim.x) - 1 - static_cast<int>(blockIdx.x)
+                            : static_cast<int>(blockIdx.x);
+  const int seq = a.batched ? static_cast<int>(blockIdx.x) : 0;
   const int h = blockIdx.y;
   const int b = blockIdx.z;
   const int hk = h / (a.Hq / a.Hkv);
@@ -129,9 +139,15 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   int Sk = a.Sk;
   int blk0 = 0;              // first KV block (page-table index) of this CTA
   const int qb = split_mode ? 0 : b;  // batch entry the queries / outputs belong to
+  const int32_t* page_table = a.page_table;
+  int total = 0;             // split mode: tokens of the sequence, the new one included
   if (split_mode) {
-    const int total = *a.sk_dev + 1;
+    total = a.sk_dev[seq] + 1;
     const int start = b * a.split_tokens;
+    if (a.batched) {
+      if (start >= total) return;  // idle sequence (total <= 0) or split past its length (block-uniform)
+      page_table += static_cast<int64_t>(seq) * a.page_table_stride;
+    }
     blk0 = start / BKV;
     Sk = max(0, min(a.split_tokens, total - start));
   }
@@ -152,14 +168,14 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       mbar_arrive_expect_tx(q_full, C::kTileBytes);
 #pragma unroll
       for (int c = 0; c < C::kChunks; ++c)
-        tma_load_4d(q_s + c * C::kChunkBytes, &tm_q, q_full, c * CW, h, qb * a.Sq + qt * BQ, 0);
+        tma_load_4d(q_s + c * C::kChunkBytes, &tm_q, q_full, c * CW, h, qb * a.Sq + qt * BQ, seq);
       for (int j = 0; j < nblk; ++j) {
         const int s = j & 1;
         const uint32_t par = ((j >> 1) & 1) ^ 1;
         int tok, page;
         if (a.paged) {
           tok = 0;
-          page = a.page_table ? a.page_table[split_mode ? blk0 + j : b * a.page_table_stride + j] : blk0 + j;
+          page = page_table ? page_table[split_mode ? blk0 + j : b * a.page_table_stride + j] : blk0 + j;
         } else {
           tok = b * a.Sk + j * BKV;
           page = 0;
@@ -299,14 +315,17 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   }
 
   if (split_mode) {
+    const int64_t seq_rows = static_cast<int64_t>(seq) * gridDim.z * a.Hq * a.Sq;
+    float* lse_out = a.lse_out + seq_rows;
+    float* o_partial = a.o_partial + seq_rows * a.D;
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
       const int q_idx = q_idx0 + 8 * hh;
       if (q_idx >= a.Sq) continue;
       const float inv = l[hh] > 0.f ? 1.f / l[hh] : 0.f;
       const int64_t r = (static_cast<int64_t>(b) * a.Hq + h) * a.Sq + q_idx;
-      if ((lane & 3) == 0) a.lse_out[r] = l[hh] > 0.f ? m[hh] + log2f(l[hh]) : -INFINITY;
-      float* dst = a.o_partial + r * a.D;
+      if ((lane & 3) == 0) lse_out[r] = l[hh] > 0.f ? m[hh] + log2f(l[hh]) : -INFINITY;
+      float* dst = o_partial + r * a.D;
 #pragma unroll
       for (int n = 0; n < DP / 8; ++n) {
         const int d = 8 * n + col0;
@@ -319,32 +338,36 @@ fmha_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       // Fused combine: the LAST split CTA of this head to finish merges all partials (fixed split
       // order -> deterministic) and writes the bf16 output, saving the separate combine launch.
       const int nthr = 128 * n_wg;
+      // splits taking part: all of them, or (batched) those holding tokens of this sequence
+      const int nsp = a.batched ? min(static_cast<int>(gridDim.z), (total + a.split_tokens - 1) / a.split_tokens)
+                                : static_cast<int>(gridDim.z);
+      int* counter = a.split_counters + static_cast<int64_t>(seq) * a.Hq + h;
       __threadfence();                  // this thread's partial rows are visible device-wide
       named_bar_sync(1, nthr);
       if (ctid == 0) {
-        const int prev = atomicAdd(&a.split_counters[h], 1);
-        *is_last_s = (prev == static_cast<int>(gridDim.z) - 1);
-        if (*is_last_s) a.split_counters[h] = 0;  // re-arm for the next launch / graph replay
+        const int prev = atomicAdd(counter, 1);
+        *is_last_s = (prev == nsp - 1);
+        if (*is_last_s) *counter = 0;  // re-arm for the next launch / graph replay
       }
       named_bar_sync(1, nthr);
       if (*is_last_s && ctid < 128) {
         __threadfence();
-        const int nsp = static_cast<int>(gridDim.z);
         const int d = ctid;                         // 128 threads <-> D = 128 columns
+        __nv_bfloat16* o = a.o + static_cast<int64_t>(seq) * a.o_seq_stride;
         for (int g = 0; g < a.Sq; ++g) {
           float mx = -INFINITY;
           for (int s = 0; s < nsp; ++s)
-            mx = fmaxf(mx, __ldcg(&a.lse_out[(static_cast<int64_t>(s) * a.Hq + h) * a.Sq + g]));
+            mx = fmaxf(mx, __ldcg(&lse_out[(static_cast<int64_t>(s) * a.Hq + h) * a.Sq + g]));
           float den = 0.f, acc = 0.f;
           for (int s = 0; s < nsp; ++s) {
             const int64_t r = (static_cast<int64_t>(s) * a.Hq + h) * a.Sq + g;
-            const float v = __ldcg(&a.lse_out[r]);
+            const float v = __ldcg(&lse_out[r]);
             const float w = (v == -INFINITY) ? 0.f : exp2f(v - mx);
             den += w;
-            acc += w * __ldcg(&a.o_partial[r * a.D + d]);
+            acc += w * __ldcg(&o_partial[r * a.D + d]);
           }
           const float inv_den = den > 0.f ? 1.f / den : 0.f;  // same arithmetic as decode_combine_kernel
-          a.o[static_cast<int64_t>(g) * a.o_tok_stride + static_cast<int64_t>(h) * a.o_head_stride + d] =
+          o[static_cast<int64_t>(g) * a.o_tok_stride + static_cast<int64_t>(h) * a.o_head_stride + d] =
               __float2bfloat16(acc * inv_den);
         }
       }
@@ -374,18 +397,23 @@ struct SplitArgs {
   float* o_partial;
   float* lse_out;
   int* counters;
+  int batch;              // > 0: batched split mode, one sequence per blockIdx.x
+  int64_t q_seq_stride;   // elements between the query rows of consecutive sequences
+  int64_t o_seq_stride;
 };
 
 template <int DP, int CW, int kPolyEvery = 0>
 int launch_fmha(const FmhaParams& p, cudaStream_t stream, const SplitArgs* split = nullptr) {
   using C = FmhaCfg<DP, CW>;
   CUtensorMap tq, tk, tv;
+  const int batch = split ? split->batch : 0;
   {
-    // split mode: the queries are ONE set of Sq rows shared by all splits (blockIdx.z)
+    // split mode: the queries are ONE set of Sq rows shared by all splits (blockIdx.z); batched: one
+    // such set per sequence along the 4th dimension
     const uint64_t q_rows = (uint64_t)(split ? 1 : p.B) * p.Sq;
-    uint64_t dims[4] = {(uint64_t)p.D, (uint64_t)p.Hq, q_rows, 1};
+    uint64_t dims[4] = {(uint64_t)p.D, (uint64_t)p.Hq, q_rows, batch > 0 ? (uint64_t)batch : 1};
     uint64_t str[3] = {(uint64_t)p.q_head_stride, (uint64_t)p.q_tok_stride,
-                       (uint64_t)p.q_tok_stride * q_rows};
+                       batch > 0 ? (uint64_t)split->q_seq_stride : (uint64_t)p.q_tok_stride * q_rows};
     uint32_t box[4] = {CW, 1, BQ, 1};
     if (make_tmap_nd_bf16(&tq, p.q, 4, dims, str, box, C::kSwizzleBytes)) return 1;
   }
@@ -419,12 +447,14 @@ int launch_fmha(const FmhaParams& p, cudaStream_t stream, const SplitArgs* split
   a.o_partial = split ? split->o_partial : nullptr;
   a.lse_out = split ? split->lse_out : nullptr;
   a.split_counters = split ? split->counters : nullptr;
+  a.batched = batch > 0 ? 1 : 0;
+  a.o_seq_stride = batch > 0 ? split->o_seq_stride : 0;
   auto kern = fmha_fwd_kernel<DP, CW, kPolyEvery>;
   static PerDeviceOnce attr_once;
   if (attr_once.first()) {
     VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmem));
   }
-  dim3 grid((p.Sq + BQ - 1) / BQ, p.Hq, p.B);
+  dim3 grid(batch > 0 ? batch : (p.Sq + BQ - 1) / BQ, p.Hq, p.B);
   VB_CUDA(launch_pdl(kern, grid, dim3(kThreads), C::kSmem, stream, tq, tk, tv, a));
   return 0;
 }
@@ -447,15 +477,24 @@ int fmha_prefill(const FmhaParams& p, cudaStream_t stream) { return fmha_prefill
 // splits of split_tokens tokens each, the sequence length is *n_tok_minus_1 + 1 (device memory, read
 // after the dependency wait, so one captured graph serves every decode position), K/V paged.  Writes
 // normalised fp32 partials [B][Hq][Sq][D] and their log2-sum-exp [B][Hq][Sq]; non-causal.
+//
+// batch > 0: `batch` sequences in one launch (blockIdx.x), sequence s with length n_tok_minus_1[s] + 1
+// (< 0: idle), queries at p.q + s*q_seq_stride, page-table row p.page_table + s*p.page_table_stride,
+// partials / lse / counters the s-th block of [B][Hq][Sq][D] / [B][Hq][Sq] / [Hq], output at
+// p.o + s*o_seq_stride; the fused combine (counters) is required.
 int fmha_decode_split(const FmhaParams& p, const int32_t* n_tok_minus_1, int split_tokens,
-                      float* o_partial, float* lse, int* counters, cudaStream_t stream) {
+                      float* o_partial, float* lse, int* counters, cudaStream_t stream,
+                      int batch, int64_t q_seq_stride, int64_t o_seq_stride) {
   VB_CHECK(p.D == 128, "fmha_decode_split: head dim must be 128");
   VB_CHECK(p.kv_page_stride != 0 && p.page_table != nullptr, "fmha_decode_split: K/V must be paged");
   VB_CHECK(split_tokens > 0 && split_tokens % BKV == 0, "fmha_decode_split: split_tokens %% 128 != 0");
   VB_CHECK(p.Sq >= 1 && p.Sq <= BQ && !p.causal, "fmha_decode_split: 1..128 query rows, non-causal");
   VB_CHECK(n_tok_minus_1 && o_partial && lse, "fmha_decode_split: null output / length pointer");
   VB_CHECK(counters == nullptr || p.o != nullptr, "fmha_decode_split: fused combine needs the output pointer");
-  SplitArgs sa{n_tok_minus_1, split_tokens, o_partial, lse, counters};
+  VB_CHECK(batch == 0 || (counters != nullptr && q_seq_stride % 8 == 0 && q_seq_stride > 0),
+           "fmha_decode_split: a batch needs counters and a query stride that is a positive multiple of 8");
+  VB_CHECK(p.B >= 1 && p.B <= 65535, "fmha_decode_split: 1..65535 splits (got %d)", p.B);
+  SplitArgs sa{n_tok_minus_1, split_tokens, o_partial, lse, counters, batch, q_seq_stride, o_seq_stride};
   return launch_fmha<128, 64>(p, stream, &sa);
 }
 

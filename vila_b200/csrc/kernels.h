@@ -67,8 +67,10 @@ int fmha_prefill(const FmhaParams& p, cudaStream_t stream);
 int fmha_prefill_cfg(int variant, const FmhaParams& p, cudaStream_t stream);
 // split-KV mode of the attention kernel for decode at long context (see fmha_wgmma.cu)
 // counters != nullptr ([Hq] ints, zero-initialised once): the last split CTA of a head combines into p.o
+// batch > 0: that many sequences in one launch (per-sequence lengths, page-table rows, work buffers)
 int fmha_decode_split(const FmhaParams& p, const int32_t* n_tok_minus_1, int split_tokens,
-                      float* o_partial, float* lse, int* counters, cudaStream_t stream);
+                      float* o_partial, float* lse, int* counters, cudaStream_t stream,
+                      int batch = 0, int64_t q_seq_stride = 0, int64_t o_seq_stride = 0);
 
 // ---- norms ---------------------------------------------------------------------------------------
 int layernorm_bf16(const __nv_bfloat16* x, const __nv_bfloat16* w, const __nv_bfloat16* b,
@@ -114,6 +116,12 @@ int rope_table(const int32_t* positions, int S, int D, const float* inv_freq, __
 int rope_kv_append(__nv_bfloat16* qkv, const int32_t* positions, int S, int Hq, int Hkv, int D,
                    const float* inv_freq, __nv_bfloat16* k_pool, __nv_bfloat16* v_pool,
                    const int32_t* page_table, int cache_pos0, cudaStream_t stream);
+// decode step of `batch` sequences: row b of qkv at qkv + b*qkv_stride, position positions[b] (< 0: idle
+// row, untouched), page-table row page_table + b*pt_stride; the k / v rows go to slot = position
+int rope_kv_append_decode_batch(__nv_bfloat16* qkv, long qkv_stride, const int32_t* positions, int batch,
+                                int Hq, int Hkv, int D, const float* inv_freq, __nv_bfloat16* k_pool,
+                                __nv_bfloat16* v_pool, const int32_t* page_table, int pt_stride,
+                                cudaStream_t stream);
 
 // same with cos / sin read from rope_table(positions) (long prefills; bit-identical)
 int rope_kv_append_table(__nv_bfloat16* qkv, const __nv_bfloat16* table, int S, int Hq, int Hkv, int D,
@@ -176,6 +184,11 @@ struct DecodeAttnSplitParams {
   float scale;
 };
 int decode_attention_split(const DecodeAttnSplitParams& p, cudaStream_t stream);
+// batch of sequences over ONE shared paged pool, long contexts: sequence b uses qkv + b*qkv_stride,
+// out + b*out_stride, position[b] (< 0: idle) and page_table + b*pt_stride; o_partial / lse / counters
+// hold `batch` blocks of the single-sequence sizes; counters are required (fused combine)
+int decode_attention_split_batch(const DecodeAttnSplitParams& p, int batch, int qkv_stride, int out_stride,
+                                 int pt_stride, cudaStream_t stream);
 
 // ---- persistent decode mega-kernel (decode_mega.cu) -------------------------------------------
 struct MegaLayer {  // device-resident array, one entry per decoder layer

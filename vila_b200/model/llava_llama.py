@@ -584,10 +584,12 @@ class LlavaLlamaModel(nn.Module):
 
     @torch.inference_mode()
     def generate_batch(self, requests: List[Dict[str, Any]], max_new_tokens: int = 128, slots: int = 8,
-                       max_tokens_per_slot: int = 2048, eos_token_id=None) -> List[List[int]]:
+                       max_tokens_per_slot: Optional[int] = None, eos_token_id=None) -> List[List[int]]:
         """Serve several independent requests with continuous batching over one shared paged KV pool
         (vila_b200/serving.py; the reference's servers run them one at a time, serving/server.py:65-73).
         requests: dicts with the `generate` arguments (`input_ids` [1, T], `media`, `media_config`).
+        max_tokens_per_slot None: sized from the requests (serving.slot_geometry: 2048 tokens unless a
+        request needs more, e.g. video or dynamic-S2 prompts).
         Greedy decoding; returns the new ids of every request in order."""
         from ..serving import generate_batch
         prompts = []

@@ -391,3 +391,32 @@ def decode_attention_batch(qkv: torch.Tensor, positions: torch.Tensor, k_pool: t
     check(_lib.load().vila_decode_attention_batch(C.byref(p), B, qkv.stride(0), out.stride(0),
                                                   page_tables.stride(0), min(32, page_tables.shape[1]),
                                                   _stream()), "vila_decode_attention_batch")
+
+
+def decode_attention_split_batch(qkv: torch.Tensor, positions: torch.Tensor, k_pool: torch.Tensor,
+                                 v_pool: torch.Tensor, page_tables: torch.Tensor, out: torch.Tensor,
+                                 o_partial: torch.Tensor, lse: torch.Tensor, counters: torch.Tensor,
+                                 inv_freq: torch.Tensor, Hq: int, Hkv: int, D: int, num_splits: int,
+                                 split_tokens: int, scale: float) -> None:
+    """Long-context decode attention of B sequences over one shared paged pool [P, 128, Hkv, D]:
+    qkv [B, (Hq+2Hkv)*D] (q / k rotated in place), positions int32 [B] (< 0: idle slot), page_tables
+    int32 [B, pages] (pages of the slot's tokens; num_splits * split_tokens must cover them), out
+    [B, Hq*D]; work buffers o_partial fp32 >= B*num_splits*Hq*D, lse fp32 >= B*num_splits*Hq, counters
+    int32 [B*Hkv] (zeroed once, self-cleaning)."""
+    _chk(qkv, "qkv"); _chk(out, "out")
+    B = qkv.shape[0]
+    assert qkv.dim() == 2 and out.shape == (B, Hq * D) and qkv.stride(1) == 1 and out.stride(1) == 1
+    assert positions.dtype == torch.int32 and positions.numel() == B and positions.is_contiguous()
+    assert page_tables.dtype == torch.int32 and page_tables.dim() == 2 and page_tables.shape[0] == B
+    assert page_tables.stride(1) == 1
+    assert o_partial.dtype == torch.float32 and o_partial.numel() >= B * num_splits * Hq * D
+    assert lse.dtype == torch.float32 and lse.numel() >= B * num_splits * Hq
+    assert counters.dtype == torch.int32 and counters.numel() >= B * Hkv
+    p = DecodeAttnSplitParams()
+    p.qkv, p.position, p.k_pool, p.v_pool = _p(qkv), _p(positions), _p(k_pool), _p(v_pool)
+    p.page_table, p.kv_num_pages, p.out = _p(page_tables), k_pool.shape[0], _p(out)
+    p.o_partial, p.lse, p.inv_freq, p.counters = _p(o_partial), _p(lse), _p(inv_freq), _p(counters)
+    p.Hq, p.Hkv, p.D, p.num_splits, p.split_tokens, p.scale = Hq, Hkv, D, num_splits, split_tokens, scale
+    check(_lib.load().vila_decode_attention_split_batch(C.byref(p), B, qkv.stride(0), out.stride(0),
+                                                        page_tables.stride(0), _stream()),
+          "vila_decode_attention_split_batch")

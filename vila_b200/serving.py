@@ -15,6 +15,9 @@ tokens per byte by B.  Here:
     per-slot position and page-table row, idle slots skipped) → o-proj GEMM(+res) → RMSNorm → gate/up
     GEMM (SwiGLU epilogue) → down GEMM(+res); then lm_head GEMM, greedy arg-max, embedding gather and
     position++ — all on the device, no host sync per token;
+  * slots longer than HEAD_KERNEL_TOKENS (video, dynamic-S2) are attended by the batched split-KV
+    kernel (`vila_decode_attention_split_batch`) in the same step; which kernel serves a slot follows
+    only from that slot's own length, so a request's ids never depend on its neighbours;
   * finished slots (EOS / budget) are harvested and refilled between graph replays.
 """
 from __future__ import annotations
@@ -27,6 +30,50 @@ import torch
 from . import ops
 
 PAGE = 128
+
+# A slot of at most this many tokens (the new one included) is attended by decode_attn_head_kernel,
+# longer slots by the batched split-KV kernel.  The head kernel could serve up to 4096 tokens (32-entry
+# page table), but above ~1K tokens the split-KV kernel is faster (DESIGN.md §4); 2048 is the lowest
+# threshold that leaves every slot of today's default 2048-token geometry on the head kernel.
+HEAD_KERNEL_TOKENS = 16 * PAGE
+# Split-KV configuration of the long slots: split j covers tokens [j*SPLIT_TOKENS, (j+1)*SPLIT_TOKENS).
+# SPLIT_TOKENS is the same for every ladder entry, so a slot's result does not depend on the entry in
+# use (the combine reads only the splits that hold tokens).  The ladder gives the number of splits
+# launched per (slot, KV head), sized from the longest active slot, so that a batch of short slots does
+# not launch thousands of CTAs that exit at once.  DESIGN.md §4 has the measurements behind both.
+SPLIT_TOKENS = 1024
+SPLIT_LADDER = (8, 16, 32, 68)
+MAX_SLOT_TOKENS = SPLIT_LADDER[-1] * SPLIT_TOKENS  # 69,632: a 256-frame LongVILA request + 1K new tokens
+
+
+def attention_config(longest: int) -> Optional[int]:
+    """Attention of a decode step whose longest active slot holds `longest` tokens (the run's appends
+    included): None = decode_attn_head_kernel only, else the number of splits of the split-KV kernel
+    (the smallest ladder entry covering `longest`)."""
+    if longest <= HEAD_KERNEL_TOKENS:
+        return None
+    for n in SPLIT_LADDER:
+        if n * SPLIT_TOKENS >= longest:
+            return n
+    raise ValueError(f"a slot of {longest} tokens exceeds the engine's limit ({MAX_SLOT_TOKENS})")
+
+
+def slot_geometry(prompt_lens: Sequence[int], max_new_tokens: int, check_every: int, slots: int,
+                  max_tokens_per_slot: Optional[int] = None) -> Tuple[int, Optional[int]]:
+    """-> (max_tokens_per_slot, total_pages or None for slots * pages_per_slot).
+
+    An explicit max_tokens_per_slot is kept as it is.  None sizes the slot from the requests: the
+    smallest page multiple >= 2048 that holds the longest prompt + max_new_tokens + check_every (at most
+    MAX_SLOT_TOKENS; a longer request is refused by generate_batch).  A batch that fits 2048 gets the
+    2048-token geometry and its full pool; a larger slot gets a pool of the page budgets of the `slots`
+    largest requests, so that one long request does not reserve `slots` long slots."""
+    if max_tokens_per_slot is not None:
+        return max_tokens_per_slot, None
+    budgets = sorted(((n + max_new_tokens + check_every + PAGE - 1) // PAGE for n in prompt_lens), reverse=True)
+    pages = min(max([2048 // PAGE] + budgets), MAX_SLOT_TOKENS // PAGE)
+    if pages == 2048 // PAGE:
+        return 2048, None
+    return pages * PAGE, min(sum(min(b, pages) for b in budgets[:slots]), slots * pages)
 
 
 class _SlotCache:
@@ -81,7 +128,8 @@ class BatchedDecoder:
         Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
         assert D == 128, "batched decode attention is specialised for head_dim 128"
         self.pages_per_slot = (max_tokens_per_slot + PAGE - 1) // PAGE
-        assert self.pages_per_slot <= 32, "vila_decode_attention_batch serves contexts up to 4096 tokens"
+        assert self.pages_per_slot * PAGE <= MAX_SLOT_TOKENS, \
+            f"slots of up to {MAX_SLOT_TOKENS} tokens (asked for {max_tokens_per_slot})"
         P = total_pages if total_pages is not None else slots * self.pages_per_slot
         self.pool = torch.zeros(cfg.num_hidden_layers, 2, P, PAGE, Hkv, D, device=dev, dtype=dt)
         self.allocator = PageAllocator(P)
@@ -96,8 +144,27 @@ class BatchedDecoder:
         self.max_new = max_new
         self.hist = torch.zeros(slots, max_new + 8, dtype=torch.int64, device=dev)
         self.step_idx = torch.zeros(slots, 1, dtype=torch.int64, device=dev)  # per-slot write column
-        self.graph: Optional[torch.cuda.CUDAGraph] = None
-        self.launches_per_step = 7 * cfg.num_hidden_layers + 2
+        # attention configurations this slot size can need (attention_config): None, then ladder entries
+        self.configs: List[Optional[int]] = [None] + [
+            n for i, n in enumerate(SPLIT_LADDER)
+            if self.pages_per_slot * PAGE > (SPLIT_LADDER[i - 1] * SPLIT_TOKENS if i else HEAD_KERNEL_TOKENS)]
+        self.graphs: Dict[Optional[int], torch.cuda.CUDAGraph] = {}  # configuration -> step graph
+        self.config: Optional[int] = None  # configuration of the last run()
+        if len(self.configs) > 1:
+            n_max = self.configs[-1]
+            # per-step copies of `positions` that hide the long slots from the head kernel and the short
+            # ones from the split-KV kernel, and the split-KV work buffers (shared by all layers)
+            self.pos_head = torch.full((slots,), -1, dtype=torch.int32, device=dev)
+            self.pos_split = torch.full((slots,), -1, dtype=torch.int32, device=dev)
+            self.o_partial = torch.zeros(slots * n_max * Hq * D, device=dev, dtype=torch.float32)
+            self.lse = torch.zeros(slots * n_max * Hq, device=dev, dtype=torch.float32)
+            self.counters = torch.zeros(slots * Hkv, device=dev, dtype=torch.int32)
+
+    @property
+    def launches_per_step(self) -> int:
+        """library kernels of one step in the configuration of the last run(): 7 per layer (9 with the
+        split-KV kernel: RoPE/append and attention added) + final RMSNorm and lm_head"""
+        return (7 if self.config is None else 9) * self.llm.config.num_hidden_layers + 2
 
     # ---- admission ------------------------------------------------------------------------------
     @torch.inference_mode()
@@ -135,15 +202,26 @@ class BatchedDecoder:
                                                                       device=self.page_tables.device)
 
     # ---- one decode step for every active slot ----------------------------------------------------
-    def _step(self) -> None:
+    def _step(self, num_splits: Optional[int]) -> None:
         llm, cfg = self.llm, self.llm.config
         Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
         x = self.x
+        pos_head = self.positions
+        if num_splits is not None:  # slot length pos + 1 picks the kernel (idle slots stay -1 in both)
+            pos_head = self.pos_head
+            long = self.positions >= HEAD_KERNEL_TOKENS
+            pos_head.copy_(self.positions).masked_fill_(long, -1)
+            self.pos_split.copy_(self.positions).masked_fill_(~long, -1)
         for li, layer in enumerate(llm.model.layers):
             h = ops.rmsnorm(x, layer.input_layernorm.weight, cfg.rms_norm_eps)
             qkv = ops.linear(h, layer._qkv_w, layer._qkv_b, static_w=True)
-            ops.decode_attention_batch(qkv, self.positions, self.pool[li, 0], self.pool[li, 1],
+            ops.decode_attention_batch(qkv, pos_head, self.pool[li, 0], self.pool[li, 1],
                                        self.page_tables, self.attn, llm.inv_freq, Hq, Hkv, D, D ** -0.5)
+            if num_splits is not None:
+                ops.decode_attention_split_batch(qkv, self.pos_split, self.pool[li, 0], self.pool[li, 1],
+                                                 self.page_tables, self.attn, self.o_partial, self.lse,
+                                                 self.counters, llm.inv_freq, Hq, Hkv, D, num_splits,
+                                                 SPLIT_TOKENS, D ** -0.5)
             ops.linear(self.attn, layer.self_attn.o_proj.weight, residual=x, out=x, static_w=True)
             h = ops.rmsnorm(x, layer.post_attention_layernorm.weight, cfg.rms_norm_eps)
             a = ops.linear(h, layer._gu_w, swiglu=True, static_w=True)
@@ -161,29 +239,35 @@ class BatchedDecoder:
 
     @torch.inference_mode()
     def run(self, n_tokens: int) -> None:
-        if self.graph is None:
+        if not self.graphs:
             raise RuntimeError("call capture() (with every slot idle) before run()")
+        longest = 0
         for s_ in range(self.slots):  # pages for the tokens this call will append
             if self._pos_host[s_] >= 0:
                 self._ensure_pages(s_, self._pos_host[s_] + n_tokens + 1)
                 self._pos_host[s_] += n_tokens
+                longest = max(longest, self._pos_host[s_])  # tokens attended by the slot's last step
+        self.config = attention_config(min(longest, self.pages_per_slot * PAGE))
+        g = self.graphs[self.config]
         for _ in range(n_tokens):
-            self.graph.replay()
+            g.replay()
 
     @torch.inference_mode()
     def capture(self) -> None:
-        """Capture the step graph.  Must be called with every slot idle (positions < 0): the capture
-        launches the kernels once, idle slots are skipped by the attention kernel and leave no trace."""
-        if self.graph is not None:
+        """Capture the step graph of every attention configuration this slot size can need.  Must be
+        called with every slot idle (positions < 0): the capture launches the kernels once, idle slots
+        are skipped by the attention kernels and leave no trace."""
+        if self.graphs:
             return
         assert bool((self.positions < 0).all()), "capture() with idle slots only"
         saved = (self.tokens.clone(), self.hist.clone(), self.step_idx.clone(), self.x.clone())
-        self._step()  # eager warm-up (allocator, function attributes); state restored below
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            self._step()
-        self.graph = g
+        for c in self.configs:
+            self._step(c)  # eager warm-up (allocator, function attributes); state restored below
+            torch.cuda.synchronize()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self._step(c)
+            self.graphs[c] = g
         for dst, src in zip((self.tokens, self.hist, self.step_idx, self.x), saved):
             dst.copy_(src)
 
@@ -194,13 +278,18 @@ class BatchedDecoder:
 
 @torch.inference_mode()
 def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eos_token_ids: Sequence[int] = (),
-                   slots: int = 8, max_tokens_per_slot: int = 2048, check_every: int = 8,
+                   slots: int = 8, max_tokens_per_slot: Optional[int] = None, check_every: int = 8,
                    decoder: Optional[BatchedDecoder] = None, total_pages: Optional[int] = None) -> List[List[int]]:
     """Greedy-decode `prompts` (list of inputs_embeds [S_i, hidden]) with continuous batching: at most
     `slots` requests in flight; a finished request (EOS or max_new_tokens) frees its slot for the next
-    one in the queue.  Returns the new ids per request (EOS included), in request order."""
-    dec = decoder or BatchedDecoder(llm, slots, max_tokens_per_slot, max_new=max_new_tokens,
-                                    total_pages=total_pages)
+    one in the queue.  Returns the new ids per request (EOS included), in request order.
+    max_tokens_per_slot None: the slot and the pool are sized from the requests (slot_geometry)."""
+    if decoder is None:
+        max_tokens_per_slot, pool_pages = slot_geometry([p.shape[0] for p in prompts], max_new_tokens,
+                                                        check_every, slots, max_tokens_per_slot)
+        decoder = BatchedDecoder(llm, slots, max_tokens_per_slot, max_new=max_new_tokens,
+                                 total_pages=total_pages if total_pages is not None else pool_pages)
+    dec = decoder
     dec.capture()
     cap = dec.pages_per_slot * PAGE
     for p in prompts:
