@@ -541,14 +541,24 @@ def test_gemv_argmax_and_finalize(cuda):
         assert expect == int(torch.argmax(ref))
 
 
-@pytest.mark.parametrize("ctx,splits", [(0, 1), (5, 1), (300, 4), (1000, 8), (130, 16),
-                                        (0, 0), (5, 0), (127, 0), (128, 0), (300, 0), (407, 0), (1023, 0),  # 0: one CTA per query head
-                                        (16448, 37), (16448, 64), (65814, 37), (65814, 64), (4000, 8)])
-def test_decode_attention(cuda, ctx, splits):
+_DECODE_CASES = [(0, 1), (5, 1), (300, 4), (1000, 8), (130, 16),
+                 (0, 0), (5, 0), (127, 0), (128, 0), (300, 0), (407, 0), (1023, 0),  # 0: one CTA per query head
+                 (16448, 37), (16448, 64), (65814, 37), (65814, 64), (4000, 8)]
+# GQA groups of the decoder's models: G=7 (NVILA-8B), G=8 (NVILA-Lite-3B), G=2 (the tiny test model);
+# splits 0 (one CTA per query head), 8 (one cluster per KV head), 16 (global-memory combine)
+_DECODE_GQA_CASES = [(ctx, s, hq, hkv) for hq, hkv in ((28, 4), (16, 2), (4, 2)) for s in (0, 8, 16)
+                     for ctx in (5, 300, 1000) if not (hq == 28 and (ctx, s) in _DECODE_CASES)]
+
+
+@pytest.mark.parametrize("ctx,splits,Hq,Hkv",
+                         [pytest.param(c, s, 28, 4, id=f"{c}-{s}") for c, s in _DECODE_CASES] +
+                         [pytest.param(*case, id="-".join(map(str, case))) for case in _DECODE_GQA_CASES])
+def test_decode_attention(cuda, ctx, splits, Hq, Hkv):
     """(16448, *) / (65814, *): decode right after a 64-frame / 256-frame video prefill (README.md:69-70
     publishes decode throughput for exactly that), splits as GraphDecoder.pick_splits chooses them."""
+    from tests.helpers import report_rel
     ops = _ops()
-    Hq, Hkv, D = 28, 4, 128
+    D = 128
     g = torch.Generator(device="cuda").manual_seed(ctx + splits)
     n_pages = max(16, (ctx + 1 + 127) // 128 + 3)
     perm = torch.randperm(n_pages, device=cuda, generator=g).to(torch.int32).contiguous()
@@ -581,7 +591,7 @@ def test_decode_attention(cuda, ctx, splits):
     k_all = torch.cat([k_hist, kr.transpose(0, 1)], 0)
     v_all = torch.cat([v_hist, vn], 0)
     ref = ref_attention(qr.transpose(0, 1)[None], k_all[None], v_all[None], True, D ** -0.5)[0, 0]
-    assert rel_err(out.view(Hq, D), ref) < 1.5e-2
+    report_rel(f"decode_attention Hq={Hq} Hkv={Hkv} ctx={ctx} splits={splits}", out.view(Hq, D), ref, 1.5e-2)
     # KV append happened
     assert torch.equal(k_pool[perm[ctx // 128], ctx % 128], kr.transpose(0, 1)[0])
     assert torch.equal(v_pool[perm[ctx // 128], ctx % 128], vn[0])

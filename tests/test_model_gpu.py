@@ -81,7 +81,8 @@ def test_encode_images_dynamic_s2(cuda, idx):
 
 @pytest.mark.parametrize("decoder", ["mega", "graph"])
 def test_generate_greedy_matches_oracle(cuda, decoder, monkeypatch):
-    """decoder: persistent mega-kernel (default) or the CUDA graph of per-layer kernels"""
+    """decoder: the CUDA graph of per-layer kernels (default) or the persistent mega-kernel
+    (VILA_B200_DECODER=mega)"""
     from vila_b200.model import tiny_test_config
     monkeypatch.setenv("VILA_B200_DECODER", decoder)
     cfg = tiny_test_config(llm_layers=3)
@@ -107,8 +108,9 @@ def test_generate_greedy_matches_oracle(cuda, decoder, monkeypatch):
 
 
 def test_decode_logits_match_prefill(cuda):
-    """KV-cached decode (GEMV + split-KV attention path) must agree with re-running the prefill
-    (GEMM + FMHA path) on the extended sequence."""
+    """Incremental prefill (prefill_hidden with Sq=1, token by token on the KV cache) must agree with
+    one prefill of the whole sequence.  No decode kernel runs here: the decode engines are compared
+    with the oracle step by step in test_decode_engines_gpu.py."""
     from vila_b200.model import tiny_test_config
     cfg = tiny_test_config(llm_layers=2)
     model = build(cfg, seed=7)
