@@ -198,6 +198,16 @@ typedef struct vila_gemv_params {
 } vila_gemv_params;
 int vila_gemv(const vila_gemv_params* p, void* stream);
 
+/* vila_gemv with FP8 weights: p->w is [N, K] e4m3 (1 byte per element, 16-byte aligned), w_scale is fp32
+ * [N], one scale per output row; x, bias, residual, norm_w and y stay bf16 and the VILA_FLAG_* meanings
+ * are unchanged.  acc_n = sum_k float(w[n,k]) * float(x[k]) in fp32, then v = acc_n * w_scale[n] enters
+ * vila_gemv's epilogue (bias, residual, SwiGLU, argmax).  Needs K % 16 == 0; there is no register-staged
+ * variant, so an unsupported shape is an error, never a launch.  Halves the weight bytes a decode token
+ * streams.  Replaces the reference's quantized loading (load_8bit / load_4bit,
+ * llava/model/builder.py:42-51) and the weight-only quantized deployment of its README ("Quantization
+ * and Deployment"). */
+int vila_gemv_fp8(const vila_gemv_params* p, const float* w_scale, void* stream);
+
 int vila_argmax_finalize(unsigned long long* key, int32_t* token_out, int32_t* token_hist,
                          int32_t* step_counter, int32_t* position, const void* embed_table,
                          void* x_next, int hidden, void* stream);

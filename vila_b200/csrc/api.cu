@@ -224,8 +224,7 @@ int vila_rope_table(const int32_t* positions, int S, int D, const float* inv_fre
   return vb::rope_table(positions, S, D, inv_freq, mb(table), st(stream));
 }
 
-int vila_gemv(const vila_gemv_params* p, void* stream) {
-  VB_REQUIRE_DEVICE();
+static vb::GemvParams to_gemv(const vila_gemv_params* p) {
   vb::GemvParams g;
   g.x = cb(p->x);
   g.w = cb(p->w);
@@ -238,7 +237,20 @@ int vila_gemv(const vila_gemv_params* p, void* stream) {
   g.K = p->K;
   g.flags = p->flags;
   g.argmax_key = p->argmax_key;
-  return vb::gemv_bf16(g, st(stream));
+  g.w_scale = nullptr;
+  return g;
+}
+
+int vila_gemv(const vila_gemv_params* p, void* stream) {
+  VB_REQUIRE_DEVICE();
+  return vb::gemv_bf16(to_gemv(p), st(stream));
+}
+
+int vila_gemv_fp8(const vila_gemv_params* p, const float* w_scale, void* stream) {
+  VB_REQUIRE_DEVICE();
+  vb::GemvParams g = to_gemv(p);
+  g.w_scale = w_scale;
+  return vb::gemv_tma_fp8(g, st(stream));
 }
 
 int vila_argmax_finalize(unsigned long long* key, int32_t* token_out, int32_t* token_hist,

@@ -12,6 +12,11 @@
 //   Fusions: RMSNorm(x) prologue, bias, residual, SwiGLU (interleaved gate/up rows), greedy argmax.
 //   Partial sums of the k-parts of a row are parked in slots and added in a fixed order.
 //
+//   FP8 form (gemv_tma_fp8): W is e4m3 [N, K] with one fp32 scale per row.  The row sum is
+//   acc_n = sum_k float(q[n,k]) * float(x[k]) in fp32 (cvt.rn.f16x2.e4m3x2 is exact: every e4m3 value
+//   is an f16 value), the k-parts are added in the same fixed order, and v = acc_n * w_scale[n] enters
+//   the bf16 kernel's epilogue unchanged.  Half the bytes per row: the ring holds twice the stages.
+//
 // Replaces cuBLAS GEMV behind nn.Linear + ATen RMSNorm / SiLU / mul / add / argmax at decode time
 // (modeling_qwen2.py:81-95,164-176,223-226; HF lm_head + greedy argmax).
 #include "common.cuh"
@@ -22,7 +27,9 @@ namespace {
 
 constexpr int kWarps = 8;
 constexpr int kThreads = kWarps * 32;
-constexpr int kMaxStages = 6;
+// ring slots per warp: 6 for bf16 weights; 12 for e4m3, whose chunks of the same rows are half as long
+template <bool kFp8>
+constexpr int max_stages() { return kFp8 ? 12 : 6; }
 
 
 __device__ __forceinline__ float dot8(const uint4& w, const uint4& x, float acc) {
@@ -35,6 +42,37 @@ __device__ __forceinline__ float dot8(const uint4& w, const uint4& x, float acc)
   acc = fmaf(bf_lo(w.w), bf_lo(x.w), acc);
   acc = fmaf(bf_hi(w.w), bf_hi(x.w), acc);
   return acc;
+}
+
+// two e4m3 (low byte = lower k) -> two floats, exactly
+__device__ __forceinline__ float2 e4m3x2_to_float2(uint32_t v) {
+  uint32_t h;
+  asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h) : "h"(static_cast<uint16_t>(v)));
+  __half2 hh;
+  memcpy(&hh, &h, sizeof(h));
+  return __half22float2(hh);
+}
+
+// 16 e4m3 weights against 16 bf16 activations (xa: k 0..7, xb: k 8..15)
+__device__ __forceinline__ float dot16_e4m3(const uint4& w, const uint4& xa, const uint4& xb, float acc) {
+  const uint32_t ws[4] = {w.x, w.y, w.z, w.w};
+  const uint32_t xs[8] = {xa.x, xa.y, xa.z, xa.w, xb.x, xb.y, xb.z, xb.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float2 a = e4m3x2_to_float2(ws[i]), b = e4m3x2_to_float2(ws[i] >> 16);
+    acc = fmaf(a.x, bf_lo(xs[2 * i]), acc);
+    acc = fmaf(a.y, bf_hi(xs[2 * i]), acc);
+    acc = fmaf(b.x, bf_lo(xs[2 * i + 1]), acc);
+    acc = fmaf(b.y, bf_hi(xs[2 * i + 1]), acc);
+  }
+  return acc;
+}
+
+// one 16-byte weight vector v of a chunk against the matching activations xv (of that chunk)
+template <bool kFp8>
+__device__ __forceinline__ float dot_vec(const uint4& w, const uint4* xv, int v, float acc) {
+  if constexpr (kFp8) return dot16_e4m3(w, xv[2 * v], xv[2 * v + 1], acc);
+  else return dot8(w, xv[v], acc);
 }
 
 __device__ __forceinline__ uint32_t float_order(float f) {
@@ -55,14 +93,18 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
 struct TmaGemvLayout {
   int chunk_elems;   // K / ksplit
   int stages;
-  int x_off, nw_off, acc_off, ring_off, bar_off, total;
+  int x_off, nw_off, acc_off, sc_off, ring_off, bar_off, total;  // sc: row scales (fp8 only)
 };
 
+template <bool kFp8>
 __global__ void __launch_bounds__(kThreads, 1)
 gemv_tma_kernel(GemvParams p, int rows_per_block, int ksplit, TmaGemvLayout L) {
+  constexpr int kMaxStages = max_stages<kFp8>();
+  constexpr int kElemBytes = kFp8 ? 1 : 2;
   extern __shared__ __align__(128) uint8_t smem[];
   uint4* xs = reinterpret_cast<uint4*>(smem + L.x_off);
   float* acc = reinterpret_cast<float*>(smem + L.acc_off);
+  float* sc = reinterpret_cast<float*>(smem + L.sc_off);
   uint8_t* ring = smem + L.ring_off;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bar_off);
   __shared__ float red[32];
@@ -73,8 +115,8 @@ gemv_tma_kernel(GemvParams p, int rows_per_block, int ksplit, TmaGemvLayout L) {
   const int nrows = min(rows_per_block, p.N - row0);
   if (nrows <= 0) return;
   const int nvec = p.K >> 3;
-  const int chunk_bytes = L.chunk_elems * 2;
-  const int chunk_vecs = L.chunk_elems >> 3;
+  const int chunk_bytes = L.chunk_elems * kElemBytes;
+  const int chunk_vecs = chunk_bytes >> 4;  // 16-byte weight vectors per chunk
   const int items = nrows * ksplit;
   const int n_my = items > warp ? (items - warp + kWarps - 1) / kWarps : 0;
   uint8_t* my_ring = ring + static_cast<size_t>(warp) * L.stages * chunk_bytes;
@@ -95,7 +137,8 @@ gemv_tma_kernel(GemvParams p, int rows_per_block, int ksplit, TmaGemvLayout L) {
   auto issue = [&](int j) {  // lane 0 only: copy item j of this warp into slot j % stages
     const int item = warp + j * kWarps;
     const int r = item / ksplit, part = item - r * ksplit;
-    const __nv_bfloat16* src = p.w + static_cast<size_t>(row0 + r) * p.K + part * L.chunk_elems;
+    const uint8_t* src = reinterpret_cast<const uint8_t*>(p.w) +
+                         (static_cast<size_t>(row0 + r) * p.K + part * L.chunk_elems) * kElemBytes;
     const int s = j % L.stages;
     mbar_arrive_expect_tx(&my_bars[s], chunk_bytes);
     bulk_g2s(my_ring + static_cast<size_t>(s) * chunk_bytes, src, chunk_bytes, &my_bars[s]);
@@ -112,7 +155,15 @@ gemv_tma_kernel(GemvParams p, int rows_per_block, int ksplit, TmaGemvLayout L) {
       bulk_g2s(nws, p.norm_w, x_bytes, &x_bar[1]);
     }
   }
+  if constexpr (kFp8) {  // row scales are parameters too (plain loads: a row block need not be 16-byte aligned)
+    if (early)
+      for (int i = threadIdx.x; i < nrows; i += kThreads) sc[i] = p.w_scale[row0 + i];
+  }
   griddep_wait();
+  if constexpr (kFp8) {
+    if (!early)
+      for (int i = threadIdx.x; i < nrows; i += kThreads) sc[i] = p.w_scale[row0 + i];
+  }
   // ---- prologue: x arrives as ONE bulk copy (a register-staged loop of dependent LDG -> STS round
   // trips per slice would stall the full weight rings, and with them the HBM stream) ----
   if (lane == 0) {
@@ -170,15 +221,15 @@ gemv_tma_kernel(GemvParams p, int rows_per_block, int ksplit, TmaGemvLayout L) {
     const int r = item / ksplit, part = item - r * ksplit;
     mbar_wait(&my_bars[s], (j / L.stages) & 1);
     const uint4* wv = reinterpret_cast<const uint4*>(my_ring + static_cast<size_t>(s) * chunk_bytes);
-    const uint4* xv = xs + part * chunk_vecs;
+    const uint4* xv = xs + part * (L.chunk_elems >> 3);
     float s0 = 0.f, s1 = 0.f;
     int v = lane;
     for (; v + 32 < chunk_vecs; v += 64) {
       const uint4 a = wv[v], b = wv[v + 32];
-      s0 = dot8(a, xv[v], s0);
-      s1 = dot8(b, xv[v + 32], s1);
+      s0 = dot_vec<kFp8>(a, xv, v, s0);
+      s1 = dot_vec<kFp8>(b, xv, v + 32, s1);
     }
-    if (v < chunk_vecs) s0 = dot8(wv[v], xv[v], s0);
+    if (v < chunk_vecs) s0 = dot_vec<kFp8>(wv[v], xv, v, s0);
     const float tot = warp_sum(s0 + s1);
     __syncwarp();  // every lane is done reading slot s
     if (lane == 0) {
@@ -206,6 +257,10 @@ gemv_tma_kernel(GemvParams p, int rows_per_block, int ksplit, TmaGemvLayout L) {
   if (p.flags & 1) {
     for (int j = threadIdx.x; j < (nrows >> 1); j += blockDim.x) {
       float g = acc[2 * j], u = acc[2 * j + 1];
+      if constexpr (kFp8) {
+        g *= sc[2 * j];
+        u *= sc[2 * j + 1];
+      }
       if (p.bias) {
         g += __bfloat162float(p.bias[row0 + 2 * j]);
         u += __bfloat162float(p.bias[row0 + 2 * j + 1]);
@@ -219,6 +274,7 @@ gemv_tma_kernel(GemvParams p, int rows_per_block, int ksplit, TmaGemvLayout L) {
   unsigned long long best = 0ull;
   for (int r = threadIdx.x; r < nrows; r += blockDim.x) {
     float v = acc[r];
+    if constexpr (kFp8) v *= sc[r];
     if (p.bias) v += __bfloat162float(p.bias[row0 + r]);
     v = bf16_round(v);
     if (p.residual) v = bf16_round(v + __bfloat162float(p.residual[row0 + r]));
@@ -242,10 +298,11 @@ gemv_tma_kernel(GemvParams p, int rows_per_block, int ksplit, TmaGemvLayout L) {
   }
 }
 
-}  // namespace
-
-// returns 0 on launch, -1 if the shape does not fit this kernel (caller falls back to the LSU kernel)
-int gemv_tma_bf16(const GemvParams& p, cudaStream_t stream) {
+template <bool kFp8>
+int gemv_tma_launch(const GemvParams& p, cudaStream_t stream) {
+  constexpr int kMaxStages = max_stages<kFp8>();
+  constexpr int kElemBytes = kFp8 ? 1 : 2;
+  constexpr int kElemAlign = 16 / kElemBytes;  // chunk elements per 16-byte weight vector
   const int sms = num_sms();
   int rows_per_block = (p.N + sms - 1) / sms;
   if ((p.flags & 1) && (rows_per_block & 1)) rows_per_block += 1;
@@ -259,16 +316,17 @@ int gemv_tma_bf16(const GemvParams& p, cudaStream_t stream) {
     return -1;
   const int x1_bytes = (p.K * 2 + 127) / 128 * 128;
   const int x_bytes = x1_bytes * (p.norm_w ? 2 : 1);  // x (+ norm weight staging)
+  const int sc_bytes = kFp8 ? rows_per_block * 4 : 0;  // row scales
   TmaGemvLayout L;
   int ksplit = -1;
   for (int ks = 1; ks <= 128; ++ks) {
     if (p.K % ks) continue;
     const int ce = p.K / ks;
-    if (ce % 8) continue;
-    const int cb = ce * 2;
+    if (ce % kElemAlign) continue;
+    const int cb = ce * kElemBytes;
     if (cb > 8192) continue;
     if (cb < 512) break;
-    const int acc_bytes = (rows_per_block * ks * 4 + 127) / 128 * 128;
+    const int acc_bytes = (rows_per_block * ks * 4 + sc_bytes + 127) / 128 * 128;
     const int ring_budget = kSmemBudget - x_bytes - acc_bytes - (kWarps * kMaxStages + 2) * 8 - 256;
     int st = ring_budget / (kWarps * cb);
     if (st > kMaxStages) st = kMaxStages;
@@ -279,11 +337,12 @@ int gemv_tma_bf16(const GemvParams& p, cudaStream_t stream) {
   }
   if (ksplit < 0) return -1;
   L.chunk_elems = p.K / ksplit;
-  const int chunk_bytes = L.chunk_elems * 2;
+  const int chunk_bytes = L.chunk_elems * kElemBytes;
   L.x_off = 0;
   L.nw_off = x1_bytes;
   L.acc_off = x_bytes;
-  L.ring_off = (L.acc_off + rows_per_block * ksplit * 4 + 127) / 128 * 128;
+  L.sc_off = L.acc_off + rows_per_block * ksplit * 4;
+  L.ring_off = (L.sc_off + sc_bytes + 127) / 128 * 128;
   {
     // recompute stages for the final ksplit (the loop may have broken on an earlier candidate)
     const int ring_budget = kSmemBudget - L.ring_off - (kWarps * kMaxStages + 2) * 8 - 256;
@@ -296,12 +355,31 @@ int gemv_tma_bf16(const GemvParams& p, cudaStream_t stream) {
   L.total = L.bar_off + (kWarps * kMaxStages + 2) * 8;
   static PerDeviceOnce attr_once;
   if (attr_once.first()) {
-    VB_CUDA(cudaFuncSetAttribute(gemv_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    VB_CUDA(cudaFuncSetAttribute(gemv_tma_kernel<kFp8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  224 * 1024));
   }
-  VB_CUDA(launch_pdl(gemv_tma_kernel, dim3(grid), dim3(kThreads), static_cast<size_t>(L.total), stream,
+  VB_CUDA(launch_pdl(gemv_tma_kernel<kFp8>, dim3(grid), dim3(kThreads), static_cast<size_t>(L.total), stream,
                      p, rows_per_block, ksplit, L));
   return 0;
+}
+
+}  // namespace
+
+// returns 0 on launch, -1 if the shape does not fit this kernel (caller falls back to the LSU kernel)
+int gemv_tma_bf16(const GemvParams& p, cudaStream_t stream) { return gemv_tma_launch<false>(p, stream); }
+
+// e4m3 weights: this kernel or an error, never a fallback
+int gemv_tma_fp8(const GemvParams& p, cudaStream_t stream) {
+  VB_CHECK(p.N > 0 && p.K > 0 && p.K % 16 == 0, "gemv_fp8: bad shape N=%d K=%d (K %% 16 == 0)", p.N, p.K);
+  VB_CHECK(!(p.flags & 1) || p.N % 2 == 0, "gemv_fp8: swiglu needs even N");
+  VB_CHECK(!(p.flags & 4), "gemv_fp8: there is no register-staged variant for e4m3 weights");
+  VB_CHECK(p.w_scale != nullptr, "gemv_fp8: w_scale is required");
+  VB_CHECK(!(reinterpret_cast<uintptr_t>(p.w) & 15) && !(reinterpret_cast<uintptr_t>(p.x) & 15) &&
+               !(p.norm_w && (reinterpret_cast<uintptr_t>(p.norm_w) & 15)),
+           "gemv_fp8: w, x and norm_w must be 16-byte aligned");
+  const int rc = gemv_tma_launch<true>(p, stream);
+  VB_CHECK(rc >= 0, "gemv_fp8: N=%d K=%d does not fit the TMA ring (K / ksplit >= 512 bytes)", p.N, p.K);
+  return rc;
 }
 
 }  // namespace vb

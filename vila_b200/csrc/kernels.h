@@ -131,7 +131,7 @@ int rope_kv_append_table(__nv_bfloat16* qkv, const __nv_bfloat16* table, int S, 
 // ---- decode (M == 1) ----------------------------------------------------------------------------
 struct GemvParams {
   const __nv_bfloat16* x;       // [K]
-  const __nv_bfloat16* w;       // [N, K]
+  const __nv_bfloat16* w;       // [N, K] (gemv_tma_fp8: e4m3 bytes)
   const __nv_bfloat16* bias;    // [N] or null
   const __nv_bfloat16* norm_w;  // [K] or null: fused RMSNorm prologue on x
   float norm_eps;
@@ -141,9 +141,11 @@ struct GemvParams {
   int flags;   // bit0: SwiGLU (rows interleaved gate, up); bit1: weights are static (stream before the PDL wait); bit2: force the register-staged kernel
   // optional fused greedy argmax over y (lm_head): 64-bit packed (value, ~index) max-reduction
   unsigned long long* argmax_key;
+  const float* w_scale;  // [N] per-row scale of e4m3 weights (gemv_tma_fp8 only)
 };
 int gemv_bf16(const GemvParams& p, cudaStream_t stream);
 int gemv_tma_bf16(const GemvParams& p, cudaStream_t stream);  // -1: shape not supported
+int gemv_tma_fp8(const GemvParams& p, cudaStream_t stream);   // e4m3 weights, K % 16 == 0
 // token = argmax key; token_hist[step++] = token; position++; key = 0; x_next = embed_table[token]
 int argmax_finalize(unsigned long long* key, int32_t* token_out, int32_t* token_hist,
                     int32_t* step_counter, int32_t* position, const __nv_bfloat16* embed_table,

@@ -110,7 +110,11 @@ def config_from_dir(model_dir: Path) -> LlavaConfig:
                        mm_projector_type=proj.get("mm_projector_type", "mlp_downsample"), **kw)
 
 
-def load_pretrained(model_path: str, device="cuda", model_cls=None) -> LlavaLlamaModel:
+def load_pretrained(model_path: str, device="cuda", model_cls=None, decode_weights: str = "bf16") -> LlavaLlamaModel:
+    """decode_weights: "bf16" or "fp8", the weights the single-stream greedy decoder streams
+    (Qwen2ForCausalLM.set_decode_weights); the checkpoint and every other path stay bf16."""
+    if decode_weights not in ("bf16", "fp8"):
+        raise ValueError(f"decode_weights must be 'bf16' or 'fp8', got {decode_weights!r}")
     d = Path(model_path)
     cfg = config_from_dir(d)
     tok = None
@@ -149,6 +153,7 @@ def load_pretrained(model_path: str, device="cuda", model_cls=None) -> LlavaLlam
     with torch.no_grad():
         for k, p in own.items():
             p.copy_(sd[k].to(p.dtype))
+    model.llm.set_decode_weights(decode_weights)
     return model
 
 

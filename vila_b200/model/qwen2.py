@@ -128,6 +128,26 @@ def unsupported_generation_options(generation_config, kwargs) -> List[str]:
     return bad
 
 
+E4M3_MAX = 448.0
+
+
+def quantize_e4m3_rows(w: torch.Tensor, rows_per_chunk: int = 16384):
+    """Weight-only FP8 with one scale per output row, no calibration data:
+        amax_n = max_k |W[n,k]| (fp32);  s_n = amax_n / 448, or 1 for an all-zero row;
+        q = (W.float() / s_n).to(float8_e4m3fn)   (round to nearest even; |W / s| <= 448, no saturation)
+    -> (q [N, K] float8_e4m3fn, s [N] fp32).  Rows are converted in chunks to bound the fp32 temporary."""
+    N, K = w.shape
+    q = torch.empty(N, K, dtype=torch.float8_e4m3fn, device=w.device)
+    s = torch.empty(N, dtype=torch.float32, device=w.device)
+    for a in range(0, N, rows_per_chunk):
+        wf = w[a:a + rows_per_chunk].float()
+        amax = wf.abs().amax(dim=1)
+        sc = torch.where(amax > 0, amax / E4M3_MAX, torch.ones_like(amax))
+        q[a:a + rows_per_chunk] = (wf / sc[:, None]).to(torch.float8_e4m3fn)
+        s[a:a + rows_per_chunk] = sc
+    return q, s
+
+
 class Qwen2ForCausalLM(nn.Module):
     def __init__(self, cfg: Qwen2Config, device="cuda", dtype=torch.bfloat16):
         super().__init__()
@@ -154,6 +174,8 @@ class Qwen2ForCausalLM(nn.Module):
         self.generation_config = None
         self._decoder = None
         self._prefill_graphs = {}
+        self.decode_weights = "bf16"
+        self._fp8_weights = None
 
     # ---- HF-style accessors ----
     @property
@@ -337,6 +359,32 @@ class Qwen2ForCausalLM(nn.Module):
     __call__ = forward
 
     # ---- decode ----
+    def set_decode_weights(self, fmt: str) -> None:
+        """Weights the single-stream greedy decoder (GraphDecoder: generate's greedy path, stream_greedy,
+        sequence-parallel greedy generate) streams per token.
+          "bf16"  the parameters themselves (default); frees any FP8 copies.
+          "fp8"   e4m3 copies with one fp32 scale per output row (quantize_e4m3_rows) of every layer's
+                  fused qkv, o_proj, interleaved gate/up and down_proj weights and of lm_head (a tied
+                  lm_head is quantized as its own copy).  Half the bytes per token; for NVILA-8B the
+                  copies take ~7.1 GB next to the bf16 weights, which stay.
+        The copies are plain attributes: state_dict() and save_pretrained do not change.  What stays
+        bf16 in either mode: the prefill (prompt K/V and last hidden state), the vision tower and
+        projector, BatchedDecoder / generate_batch, the eager sampling / logits-processor path and the
+        embedding gather.  Either call drops the cached decoder (its graphs bake in weight pointers)."""
+        if fmt not in ("bf16", "fp8"):
+            raise ValueError(f"decode weights must be 'bf16' or 'fp8', got {fmt!r}")
+        self._decoder = None
+        self._fp8_weights = None
+        if fmt == "fp8":
+            with torch.no_grad():
+                layers = [SimpleNamespace(qkv=quantize_e4m3_rows(layer._qkv_w),
+                                          o=quantize_e4m3_rows(layer.self_attn.o_proj.weight),
+                                          gu=quantize_e4m3_rows(layer._gu_w),
+                                          down=quantize_e4m3_rows(layer.mlp.down_proj.weight))
+                          for layer in self.model.layers]
+                self._fp8_weights = SimpleNamespace(layers=layers, lm_head=quantize_e4m3_rows(self.lm_head.weight))
+        self.decode_weights = fmt
+
     def decoder(self, max_new_tokens: int):
         """Greedy decode engine: the CUDA graph of per-layer kernels (default) or, with
         VILA_B200_DECODER=mega, the persistent whole-token mega-kernel."""
@@ -507,7 +555,12 @@ class GraphDecoder:
     """Greedy decode loop living entirely on the device: per token 5 launches per layer + lm_head
     GEMV(argmax) + finalize (token history, position++, next embedding gather), captured in a CUDA
     graph and replayed without host synchronisation (the reference runs ~400 launches and one D2H
-    stopping-criteria sync per token, SURVEY §3.1 HOT LOOP C)."""
+    stopping-criteria sync per token, SURVEY §3.1 HOT LOOP C).
+
+    The decoder streams the weights of the LLM's decode-weight mode at construction
+    (Qwen2ForCausalLM.set_decode_weights): in "fp8" mode every GEMV of start() and of each step, lm_head
+    included, runs vila_gemv_fp8 on the e4m3 copies, so the first token is an fp8 lm_head result too.
+    The prompt's K/V and last hidden state come from the bf16 prefill in either mode."""
 
     MAX_SPLITS = 64
 
@@ -516,6 +569,7 @@ class GraphDecoder:
         cfg = llm.config
         dev, dt = llm.device, llm.dtype
         self.max_new = max_new
+        self.fp8 = llm._fp8_weights  # None: bf16 weights.  Held here: the graphs bake in its pointers
         Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
         self._fixed_splits = num_splits
         self.num_splits = 8 if num_splits is None else num_splits
@@ -586,12 +640,33 @@ class GraphDecoder:
                                                               else tokens)
         return self.cache
 
+    def _weights(self, li: Optional[int]):
+        """-> (qkv, o, gate/up, down) of layer li, or lm_head for li None: each a dict of ops.gemv's
+        weight arguments (w, and w_scale in fp8 mode)"""
+        llm = self.llm
+        if self.fp8 is not None:
+            if li is None:
+                return dict(w=self.fp8.lm_head[0], w_scale=self.fp8.lm_head[1])
+            f = self.fp8.layers[li]
+            return tuple(dict(w=q, w_scale=s) for q, s in (f.qkv, f.o, f.gu, f.down))
+        if li is None:
+            return dict(w=llm.lm_head.weight)
+        layer = llm.model.layers[li]
+        return tuple(dict(w=w) for w in (layer._qkv_w, layer.self_attn.o_proj.weight, layer._gu_w,
+                                         layer.mlp.down_proj.weight))
+
+    def _lm_head(self):
+        cfg = self.llm.config
+        ops.gemv(self.x, norm_w=self.llm.model.norm.weight, norm_eps=cfg.rms_norm_eps, argmax_key=self.key,
+                 write_out=False, static_w=True, **self._weights(None))
+
     def _step(self):
         llm, cfg, cache = self.llm, self.llm.config, self.cache
         Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
         for li, layer in enumerate(llm.model.layers):
-            ops.gemv(self.x, layer._qkv_w, bias=layer._qkv_b, norm_w=layer.input_layernorm.weight,
-                     norm_eps=cfg.rms_norm_eps, out=self.qkv, static_w=True)
+            w_qkv, w_o, w_gu, w_down = self._weights(li)
+            ops.gemv(self.x, bias=layer._qkv_b, norm_w=layer.input_layernorm.weight,
+                     norm_eps=cfg.rms_norm_eps, out=self.qkv, static_w=True, **w_qkv)
             if self.split_tokens:
                 ops.decode_attention_split(self.qkv, self.position, cache.k(li), cache.v(li),
                                            cache.page_table, self.attn, self.o_partial, self.lse,
@@ -602,25 +677,23 @@ class GraphDecoder:
                 ops.decode_attention(self.qkv, self.position, cache.k(li), cache.v(li), cache.page_table,
                                      self.attn, self.ws, self.counters, llm.inv_freq, Hq, Hkv, D,
                                      self.num_splits, D ** -0.5)
-            ops.gemv(self.attn, layer.self_attn.o_proj.weight, residual=self.x, out=self.x, static_w=True)
-            ops.gemv(self.x, layer._gu_w, norm_w=layer.post_attention_layernorm.weight,
-                     norm_eps=cfg.rms_norm_eps, swiglu=True, out=self.act, static_w=True)
-            ops.gemv(self.act, layer.mlp.down_proj.weight, residual=self.x, out=self.x, static_w=True)
-        ops.gemv(self.x, llm.lm_head.weight, norm_w=llm.model.norm.weight,
-                 norm_eps=cfg.rms_norm_eps, argmax_key=self.key, write_out=False, static_w=True)
+            ops.gemv(self.attn, residual=self.x, out=self.x, static_w=True, **w_o)
+            ops.gemv(self.x, norm_w=layer.post_attention_layernorm.weight,
+                     norm_eps=cfg.rms_norm_eps, swiglu=True, out=self.act, static_w=True, **w_gu)
+            ops.gemv(self.act, residual=self.x, out=self.x, static_w=True, **w_down)
+        self._lm_head()
         ops.argmax_finalize(self.key, self.token, self.hist, self.step, self.position,
                             llm.model.embed_tokens.weight, self.x)
 
     def start(self, last_hidden: torch.Tensor, cache: PagedKVCache) -> None:
         """Seed the loop from the prefill: first new token = argmax(lm_head(norm(last_hidden)))."""
         assert cache is self.cache
-        llm, cfg = self.llm, self.llm.config
+        llm = self.llm
         self.step.zero_()
         self.key.zero_()
         self.position.fill_(cache.length - 1)  # finalize increments -> position of the new token
         self.x.copy_(last_hidden)
-        ops.gemv(self.x, llm.lm_head.weight, norm_w=llm.model.norm.weight,
-                 norm_eps=cfg.rms_norm_eps, argmax_key=self.key, write_out=False, static_w=True)
+        self._lm_head()
         ops.argmax_finalize(self.key, self.token, self.hist, self.step, self.position,
                             llm.model.embed_tokens.weight, self.x)
         self._started = 1
@@ -654,6 +727,9 @@ class MegaDecoder(GraphDecoder):
     ahead across layer / token boundaries, grid barriers between phases."""
 
     def __init__(self, llm: Qwen2ForCausalLM, max_new: int, num_splits: int = 8):
+        if llm.decode_weights != "bf16":
+            raise NotImplementedError("the decode mega-kernel streams bf16 weights only: use the graph decoder "
+                                      f"for decode_weights={llm.decode_weights!r}")
         super().__init__(llm, max_new, num_splits)  # the mega-kernel keeps 8 cluster-free splits
         cfg = llm.config
         dev = llm.device

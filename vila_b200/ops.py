@@ -319,10 +319,25 @@ def linear_qkv_rope(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tenso
 def gemv(x: torch.Tensor, w: torch.Tensor, *, bias=None, norm_w=None, norm_eps: float = 1e-6,
          residual=None, swiglu: bool = False, out: Optional[torch.Tensor] = None,
          argmax_key: Optional[torch.Tensor] = None, write_out: bool = True,
-         static_w: bool = False, variant: int = 0) -> Optional[torch.Tensor]:
-    _chk(x, "x"); _chk(w, "w")
+         static_w: bool = False, variant: int = 0, w_scale: Optional[torch.Tensor] = None
+         ) -> Optional[torch.Tensor]:
+    """y = W x with the fused RMSNorm prologue and bias / residual / SwiGLU / argmax epilogues.
+    w bf16 [N, K]; or w torch.float8_e4m3fn [N, K] with w_scale fp32 [N] (one scale per row), which
+    runs vila_gemv_fp8 (TMA-ring kernel only: variant=1 is refused)."""
+    fp8 = w.dtype == torch.float8_e4m3fn
+    _chk(x, "x"); _chk(w, "w", torch.float8_e4m3fn if fp8 else torch.bfloat16)
     N, K = w.shape
     assert x.numel() == K and w.is_contiguous()
+    if fp8:
+        if w_scale is None:
+            raise ValueError("gemv: float8_e4m3fn weights need w_scale (fp32 [N])")
+        _chk(w_scale, "w_scale", torch.float32)
+        if w_scale.shape != (N,) or not w_scale.is_contiguous():
+            raise ValueError(f"gemv: w_scale must be a contiguous fp32 [{N}] tensor, got {tuple(w_scale.shape)}")
+        if variant == 1:
+            raise ValueError("gemv: the register-staged variant has no float8_e4m3fn form")
+    elif w_scale is not None:
+        raise ValueError("gemv: w_scale is only meaningful with float8_e4m3fn weights")
     if out is None and write_out:
         out = torch.empty((N // 2 if swiglu else N,), dtype=torch.bfloat16, device=x.device)
     p = GemvParams()
@@ -331,7 +346,10 @@ def gemv(x: torch.Tensor, w: torch.Tensor, *, bias=None, norm_w=None, norm_eps: 
     p.residual, p.y = _p(residual), _p(out)
     p.N, p.K, p.flags = N, K, (1 if swiglu else 0) | (2 if static_w else 0) | (4 if variant == 1 else 0)
     p.argmax_key = _p(argmax_key)
-    check(_lib.load().vila_gemv(C.byref(p), _stream()), "vila_gemv")
+    if fp8:
+        check(_lib.load().vila_gemv_fp8(C.byref(p), _p(w_scale), _stream()), "vila_gemv_fp8")
+    else:
+        check(_lib.load().vila_gemv(C.byref(p), _stream()), "vila_gemv")
     return out
 
 
