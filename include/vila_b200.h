@@ -208,6 +208,18 @@ int vila_gemv(const vila_gemv_params* p, void* stream);
  * and Deployment"). */
 int vila_gemv_fp8(const vila_gemv_params* p, const float* w_scale, void* stream);
 
+/* vila_gemv with 4-bit weights (W4A16): groups of 128 consecutive k of a row share a bf16 scale s and a uint8
+ * zero point z, and w = (q - z) * s for the 4-bit code q.  p->w holds the codes as packed by
+ * quantize_w4_groups (vila_b200/model/qwen2.py, which owns the byte order: 16-row tiles in mma fragment
+ * order, ceil(N / 16) * 16 * K / 2 bytes, 16-byte aligned); w_scale is bf16 [N, K / 128] and w_zero uint8
+ * [N, K / 128].  p->K is the logical K.  x, bias, residual, norm_w and y stay bf16 and the VILA_FLAG_*
+ * meanings are unchanged; the epilogue is vila_gemv's (bias, residual, SwiGLU, argmax) and the k-parts
+ * are added in a fixed order, so results are bit-repeatable.  Needs K % 128 == 0; there is no
+ * register-staged variant, so an unsupported shape is an error, never a launch.  A quarter of the bf16
+ * weight bytes.  Replaces the reference's 4-bit loading (load_4bit, llava/model/builder.py:44-51) and
+ * its TinyChat W4A16 deployment (AWQ, group 128; README "Quantization and Deployment"). */
+int vila_gemv_w4a16(const vila_gemv_params* p, const void* w_scale, const uint8_t* w_zero, void* stream);
+
 int vila_argmax_finalize(unsigned long long* key, int32_t* token_out, int32_t* token_hist,
                          int32_t* step_counter, int32_t* position, const void* embed_table,
                          void* x_next, int hidden, void* stream);

@@ -102,6 +102,7 @@ SIGNATURES = {
     "vila_rope_table": [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p],
     "vila_gemv": [C.POINTER(GemvParams), c_void_p],
     "vila_gemv_fp8": [C.POINTER(GemvParams), c_void_p, c_void_p],
+    "vila_gemv_w4a16": [C.POINTER(GemvParams), c_void_p, c_void_p, c_void_p],
     "vila_argmax_finalize": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                              c_int, c_void_p],
     "vila_decode_attention": [C.POINTER(DecodeAttnParams), c_void_p],

@@ -253,6 +253,11 @@ int vila_gemv_fp8(const vila_gemv_params* p, const float* w_scale, void* stream)
   return vb::gemv_tma_fp8(g, st(stream));
 }
 
+int vila_gemv_w4a16(const vila_gemv_params* p, const void* w_scale, const uint8_t* w_zero, void* stream) {
+  VB_REQUIRE_DEVICE();
+  return vb::gemv_tma_w4a16(to_gemv(p), cb(w_scale), w_zero, st(stream));
+}
+
 int vila_argmax_finalize(unsigned long long* key, int32_t* token_out, int32_t* token_hist,
                          int32_t* step_counter, int32_t* position, const void* embed_table,
                          void* x_next, int hidden, void* stream) {

@@ -17,6 +17,10 @@
 //   is an f16 value), the k-parts are added in the same fixed order, and v = acc_n * w_scale[n] enters
 //   the bf16 kernel's epilogue unchanged.  Half the bytes per row: the ring holds twice the stages.
 //
+//   W4A16 form (gemv_tma_w4a16, gemv_w4_kernel below): 4-bit codes with a bf16 scale and a uint8 zero
+//   point per group of 128 k; its own main loop runs mma.sync on 16-row tiles, the prologue and the
+//   epilogue are those of the bf16 form.
+//
 // Replaces cuBLAS GEMV behind nn.Linear + ATen RMSNorm / SiLU / mul / add / argmax at decode time
 // (modeling_qwen2.py:81-95,164-176,223-226; HF lm_head + greedy argmax).
 #include "common.cuh"
@@ -95,6 +99,109 @@ struct TmaGemvLayout {
   int stages;
   int x_off, nw_off, acc_off, sc_off, ring_off, bar_off, total;  // sc: row scales (fp8 only)
 };
+
+// Fused RMSNorm prologue, in place on x in shared memory (every thread of the block takes part):
+// x <- bf16(bf16(x * rstd) * norm_w), the norm weight arriving on nw_bar.
+__device__ __forceinline__ void rmsnorm_x_in_smem(const GemvParams& p, uint4* xs, const uint4* nws, int nvec,
+                                                  float* red, uint64_t* nw_bar) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float s = 0.f;
+  for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
+    const uint4 v = xs[i];
+    float t;
+    t = bf_lo(v.x); s += t * t;
+    t = bf_hi(v.x); s += t * t;
+    t = bf_lo(v.y); s += t * t;
+    t = bf_hi(v.y); s += t * t;
+    t = bf_lo(v.z); s += t * t;
+    t = bf_hi(v.z); s += t * t;
+    t = bf_lo(v.w); s += t * t;
+    t = bf_hi(v.w); s += t * t;
+  }
+  s = warp_sum(s);
+  if (lane == 0) red[warp] = s;
+  __syncthreads();
+  float t = lane < kWarps ? red[lane] : 0.f;
+  t = warp_sum(t);
+  const float rstd = rsqrtf(t / p.K + p.norm_eps);
+  mbar_wait(nw_bar, 0);
+  for (int i = threadIdx.x; i < nvec; i += blockDim.x) {  // each thread rewrites only its own slots
+    const uint4 v = xs[i], g = nws[i];
+    uint4 o;
+    o.x = pack_bf16(bf16_round(bf_lo(v.x) * rstd) * bf_lo(g.x), bf16_round(bf_hi(v.x) * rstd) * bf_hi(g.x));
+    o.y = pack_bf16(bf16_round(bf_lo(v.y) * rstd) * bf_lo(g.y), bf16_round(bf_hi(v.y) * rstd) * bf_hi(g.y));
+    o.z = pack_bf16(bf16_round(bf_lo(v.z) * rstd) * bf_lo(g.z), bf16_round(bf_hi(v.z) * rstd) * bf_hi(g.z));
+    o.w = pack_bf16(bf16_round(bf_lo(v.w) * rstd) * bf_lo(g.w), bf16_round(bf_hi(v.w) * rstd) * bf_hi(g.w));
+    xs[i] = o;
+  }
+}
+
+// Fixed-order reduction of the k-parts, in place: acc[i] <- sum_q acc[i*ksplit + q].  Rows are processed
+// in phases of blockDim.x; writing row i only overwrites slots of rows <= i, which have been read in this
+// or an earlier phase.
+__device__ __forceinline__ void reduce_kparts(float* acc, int nrows, int ksplit) {
+  if (ksplit > 1) {
+    for (int base = 0; base < nrows; base += blockDim.x) {
+      const int i = base + threadIdx.x;
+      float tot = 0.f;
+      if (i < nrows)
+        for (int q = 0; q < ksplit; ++q) tot += acc[i * ksplit + q];
+      __syncthreads();
+      if (i < nrows) acc[i] = tot;
+      __syncthreads();
+    }
+  }
+}
+
+// Epilogue on the row sums acc[0, nrows) (times the row scales sc with kScaled): bias, residual, SwiGLU
+// (interleaved gate / up rows), greedy argmax.
+template <bool kScaled>
+__device__ __forceinline__ void gemv_epilogue(const GemvParams& p, const float* acc, const float* sc, int row0,
+                                              int nrows, unsigned long long* best_s) {
+  const int lane = threadIdx.x & 31;
+  if (p.flags & 1) {
+    for (int j = threadIdx.x; j < (nrows >> 1); j += blockDim.x) {
+      float g = acc[2 * j], u = acc[2 * j + 1];
+      if constexpr (kScaled) {
+        g *= sc[2 * j];
+        u *= sc[2 * j + 1];
+      }
+      if (p.bias) {
+        g += __bfloat162float(p.bias[row0 + 2 * j]);
+        u += __bfloat162float(p.bias[row0 + 2 * j + 1]);
+      }
+      g = bf16_round(g);
+      u = bf16_round(u);
+      p.y[(row0 >> 1) + j] = __float2bfloat16(bf16_round(silu_f(g)) * u);
+    }
+    return;
+  }
+  unsigned long long best = 0ull;
+  for (int r = threadIdx.x; r < nrows; r += blockDim.x) {
+    float v = acc[r];
+    if constexpr (kScaled) v *= sc[r];
+    if (p.bias) v += __bfloat162float(p.bias[row0 + r]);
+    v = bf16_round(v);
+    if (p.residual) v = bf16_round(v + __bfloat162float(p.residual[row0 + r]));
+    if (p.y) p.y[row0 + r] = __float2bfloat16(v);
+    if (p.argmax_key) {
+      const unsigned long long key =
+          (static_cast<unsigned long long>(float_order(v)) << 32) |
+          static_cast<unsigned long long>(0xffffffffu - static_cast<uint32_t>(row0 + r));
+      best = key > best ? key : best;
+    }
+  }
+  if (p.argmax_key) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o);
+      best = other > best ? other : best;
+    }
+    if (lane == 0) atomicMax(best_s, best);
+    __syncthreads();
+    if (threadIdx.x == 0) atomicMax(p.argmax_key, *best_s);
+  }
+}
 
 template <bool kFp8>
 __global__ void __launch_bounds__(kThreads, 1)
@@ -181,37 +288,7 @@ gemv_tma_kernel(GemvParams p, int rows_per_block, int ksplit, TmaGemvLayout L) {
   if (threadIdx.x == 0) best_s = 0ull;
   __syncthreads();  // barrier initialisation by warp 0 is visible to every warp
   mbar_wait(&x_bar[0], 0);
-  if (p.norm_w != nullptr) {
-    float s = 0.f;
-    for (int i = threadIdx.x; i < nvec; i += blockDim.x) {
-      const uint4 v = xs[i];
-      float t;
-      t = bf_lo(v.x); s += t * t;
-      t = bf_hi(v.x); s += t * t;
-      t = bf_lo(v.y); s += t * t;
-      t = bf_hi(v.y); s += t * t;
-      t = bf_lo(v.z); s += t * t;
-      t = bf_hi(v.z); s += t * t;
-      t = bf_lo(v.w); s += t * t;
-      t = bf_hi(v.w); s += t * t;
-    }
-    s = warp_sum(s);
-    if (lane == 0) red[warp] = s;
-    __syncthreads();
-    float t = lane < kWarps ? red[lane] : 0.f;
-    t = warp_sum(t);
-    const float rstd = rsqrtf(t / p.K + p.norm_eps);
-    mbar_wait(&x_bar[1], 0);
-    for (int i = threadIdx.x; i < nvec; i += blockDim.x) {  // each thread rewrites only its own slots
-      const uint4 v = xs[i], g = nws[i];
-      uint4 o;
-      o.x = pack_bf16(bf16_round(bf_lo(v.x) * rstd) * bf_lo(g.x), bf16_round(bf_hi(v.x) * rstd) * bf_hi(g.x));
-      o.y = pack_bf16(bf16_round(bf_lo(v.y) * rstd) * bf_lo(g.y), bf16_round(bf_hi(v.y) * rstd) * bf_hi(g.y));
-      o.z = pack_bf16(bf16_round(bf_lo(v.z) * rstd) * bf_lo(g.z), bf16_round(bf_hi(v.z) * rstd) * bf_hi(g.z));
-      o.w = pack_bf16(bf16_round(bf_lo(v.w) * rstd) * bf_lo(g.w), bf16_round(bf_hi(v.w) * rstd) * bf_hi(g.w));
-      xs[i] = o;
-    }
-  }
+  if (p.norm_w != nullptr) rmsnorm_x_in_smem(p, xs, nws, nvec, red, &x_bar[1]);
   __syncthreads();
 
   // ---- main loop: consume this warp's ring ----
@@ -238,64 +315,8 @@ gemv_tma_kernel(GemvParams p, int rows_per_block, int ksplit, TmaGemvLayout L) {
     }
   }
   __syncthreads();
-  if (ksplit > 1) {
-    // fixed-order reduction of the k-parts, in place: acc[i] <- sum_q acc[i*ksplit + q].  Rows are
-    // processed in phases of blockDim.x; writing row i only overwrites slots of rows <= i, which
-    // have been read in this or an earlier phase.
-    for (int base = 0; base < nrows; base += blockDim.x) {
-      const int i = base + threadIdx.x;
-      float tot = 0.f;
-      if (i < nrows)
-        for (int q = 0; q < ksplit; ++q) tot += acc[i * ksplit + q];
-      __syncthreads();
-      if (i < nrows) acc[i] = tot;
-      __syncthreads();
-    }
-  }
-
-  // ---- epilogue ----
-  if (p.flags & 1) {
-    for (int j = threadIdx.x; j < (nrows >> 1); j += blockDim.x) {
-      float g = acc[2 * j], u = acc[2 * j + 1];
-      if constexpr (kFp8) {
-        g *= sc[2 * j];
-        u *= sc[2 * j + 1];
-      }
-      if (p.bias) {
-        g += __bfloat162float(p.bias[row0 + 2 * j]);
-        u += __bfloat162float(p.bias[row0 + 2 * j + 1]);
-      }
-      g = bf16_round(g);
-      u = bf16_round(u);
-      p.y[(row0 >> 1) + j] = __float2bfloat16(bf16_round(silu_f(g)) * u);
-    }
-    return;
-  }
-  unsigned long long best = 0ull;
-  for (int r = threadIdx.x; r < nrows; r += blockDim.x) {
-    float v = acc[r];
-    if constexpr (kFp8) v *= sc[r];
-    if (p.bias) v += __bfloat162float(p.bias[row0 + r]);
-    v = bf16_round(v);
-    if (p.residual) v = bf16_round(v + __bfloat162float(p.residual[row0 + r]));
-    if (p.y) p.y[row0 + r] = __float2bfloat16(v);
-    if (p.argmax_key) {
-      const unsigned long long key =
-          (static_cast<unsigned long long>(float_order(v)) << 32) |
-          static_cast<unsigned long long>(0xffffffffu - static_cast<uint32_t>(row0 + r));
-      best = key > best ? key : best;
-    }
-  }
-  if (p.argmax_key) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o);
-      best = other > best ? other : best;
-    }
-    if (lane == 0) atomicMax(&best_s, best);
-    __syncthreads();
-    if (threadIdx.x == 0) atomicMax(p.argmax_key, best_s);
-  }
+  reduce_kparts(acc, nrows, ksplit);
+  gemv_epilogue<kFp8>(p, acc, sc, row0, nrows, &best_s);
 }
 
 template <bool kFp8>
@@ -363,6 +384,237 @@ int gemv_tma_launch(const GemvParams& p, cudaStream_t stream) {
   return 0;
 }
 
+// ---------------------------------------------------------------------------------------------------
+// W4A16 form (gemv_tma_w4a16): 4-bit codes q in groups of 128 consecutive k of a row, each group with a
+// bf16 scale s and a uint8 zero point z, w = (q - z) * s.  The products run on the tensor cores:
+// mma.sync m16n8k16 (bf16 in, fp32 accumulate) with a 16-row weight tile as A and x as B, broadcast to
+// all 8 columns (so every column of D holds the same row sums).  Dequantisation to the A fragment is
+// exact and cheap: 0x4300 | q is the bf16 value 128 + q, and subtracting the bf16 128 + z leaves q - z.
+// Each group's 8 mma steps accumulate into a fresh fragment, which is scaled by s in fp32 and added to
+// the row sum; the k-parts of a row are then added in a fixed order, as in the bf16 and fp8 forms.
+//
+// Packed code layout (written by quantize_w4_groups, vila_b200/model/qwen2.py): rows in tiles of 16
+// (N padded with zero codes), each tile's K/2 * 16 bytes contiguous, as [K/64][32 lanes][4 u32].  In the
+// 64-k block at k = b, lane (g = lane / 4, c = lane % 4) owns u32 j (mma step j) holding rows g and g + 8
+// at k0 = b + 16c + 4j .. k0 + 3, nibble i + 4m of it in bf16x2 register i, half m:
+//   nibble 0 / 4: row g, k0 / k0+1      nibble 1 / 5: row g+8, k0 / k0+1
+//   nibble 2 / 6: row g, k0+2 / k0+3    nibble 3 / 7: row g+8, k0+2 / k0+3
+// which is the A fragment of m16n8k16 with mma k index (2c, 2c+1, 2c+8, 2c+9) mapped to k0 + (0, 1, 2, 3);
+// x's B fragment under the same mapping is x[k0 .. k0+3], so a lane reads its x as two plain 16-byte words
+// per 64-k block.
+constexpr int kW4TileRows = 16;
+constexpr int kW4Group = 128;
+constexpr int kW4GroupBytes = kW4TileRows * kW4Group / 2;  // one group of one tile: 1 KB
+constexpr int kW4MaxStages = 12;
+
+__device__ __forceinline__ void mma_bf16_m16n8k16(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2,
+                                                  uint32_t a3, uint32_t b0, uint32_t b1) {
+  asm("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+      "{%0, %1, %2, %3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+
+// bf16x2 {128 + nibble i, 128 + nibble i + 4} of w, minus the bf16x2 {128 + z, 128 + z}: exactly q - z
+__device__ __forceinline__ uint32_t w4_pair(uint32_t w, int i, uint32_t zz) {
+  uint32_t v;  // (w >> 4i) & 0x000f000f | 0x43004300 as one LOP3 (the compiler splits the C form in two)
+  asm("lop3.b32 %0, %1, %2, %3, 0xea;" : "=r"(v) : "r"(w >> (4 * i)), "n"(0x000f000f), "n"(0x43004300));
+  __nv_bfloat162 a, b;
+  memcpy(&a, &v, 4);
+  memcpy(&b, &zz, 4);
+  const __nv_bfloat162 d = __hsub2(a, b);
+  uint32_t r;
+  memcpy(&r, &d, 4);
+  return r;
+}
+
+// one 64-k block: 4 mma steps on the weight word wq (u32 j = step j) and this lane's x words xa, xb
+__device__ __forceinline__ void w4_block(float (&d)[4], const uint4& wq, const uint4& xa, const uint4& xb,
+                                         uint32_t zg, uint32_t zg8) {
+  const uint32_t ws[4] = {wq.x, wq.y, wq.z, wq.w};
+  const uint32_t xw[8] = {xa.x, xa.y, xa.z, xa.w, xb.x, xb.y, xb.z, xb.w};
+#pragma unroll
+  for (int j = 0; j < 4; ++j)
+    mma_bf16_m16n8k16(d, w4_pair(ws[j], 0, zg), w4_pair(ws[j], 1, zg8), w4_pair(ws[j], 2, zg),
+                      w4_pair(ws[j], 3, zg8), xw[2 * j], xw[2 * j + 1]);
+}
+
+struct W4GemvLayout {
+  int chunk_groups;  // groups per (tile, k-part) item: G / ksplit
+  int stages;
+  int x_off, nw_off, acc_off, gs_off, gz_off, ring_off, bar_off, total;  // gs / gz: group scales / zeros
+};
+
+__global__ void __launch_bounds__(kThreads, 1)
+gemv_w4_kernel(GemvParams p, const __nv_bfloat16* __restrict__ w_gscale, const uint8_t* __restrict__ w_zero,
+               int rows_per_block, int ksplit, W4GemvLayout L) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  uint4* xs = reinterpret_cast<uint4*>(smem + L.x_off);
+  float* acc = reinterpret_cast<float*>(smem + L.acc_off);
+  __nv_bfloat16* gs = reinterpret_cast<__nv_bfloat16*>(smem + L.gs_off);  // [rows_per_block][G]
+  uint8_t* gz = smem + L.gz_off;                                           // [rows_per_block][G]
+  uint8_t* ring = smem + L.ring_off;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bar_off);
+  __shared__ float red[32];
+  __shared__ unsigned long long best_s;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int row0 = blockIdx.x * rows_per_block;
+  const int nrows = min(rows_per_block, p.N - row0);
+  if (nrows <= 0) return;
+  const int ntiles = (nrows + kW4TileRows - 1) / kW4TileRows;
+  const int G = p.K / kW4Group;
+  const int nvec = p.K >> 3;
+  const int chunk_bytes = L.chunk_groups * kW4GroupBytes;
+  const int items = ntiles * ksplit;
+  const int n_my = items > warp ? (items - warp + kWarps - 1) / kWarps : 0;
+  uint8_t* my_ring = ring + static_cast<size_t>(warp) * L.stages * chunk_bytes;
+  uint64_t* my_bars = bars + warp * kW4MaxStages;
+
+  uint64_t* x_bar = bars + kWarps * kW4MaxStages;  // [0]: x arrived, [1]: norm weight arrived
+  if (lane == 0) {
+    for (int s = 0; s < L.stages; ++s) mbar_init(&my_bars[s], 1);
+    if (warp == 0) {
+      mbar_init(&x_bar[0], 1);
+      mbar_init(&x_bar[1], 1);
+    }
+    fence_barrier_init();
+  }
+  __syncwarp();
+  griddep_launch_dependents();
+
+  const size_t tile_bytes = static_cast<size_t>(p.K) * (kW4TileRows / 2);
+  auto issue = [&](int j) {  // lane 0 only: copy item j of this warp into slot j % stages
+    const int item = warp + j * kWarps;
+    const int t = item / ksplit, part = item - t * ksplit;
+    const uint8_t* src = reinterpret_cast<const uint8_t*>(p.w) +
+                         static_cast<size_t>(row0 / kW4TileRows + t) * tile_bytes +
+                         static_cast<size_t>(part) * chunk_bytes;
+    const int s = j % L.stages;
+    mbar_arrive_expect_tx(&my_bars[s], chunk_bytes);
+    bulk_g2s(my_ring + static_cast<size_t>(s) * chunk_bytes, src, chunk_bytes, &my_bars[s]);
+  };
+  // group parameters of the block's rows (rows past N of the last tile: s = 0, z = 0)
+  auto load_params = [&]() {
+    for (int i = threadIdx.x; i < ntiles * kW4TileRows * G; i += kThreads) {
+      const bool in = i < nrows * G;
+      gs[i] = in ? w_gscale[static_cast<size_t>(row0) * G + i] : __float2bfloat16(0.f);
+      gz[i] = in ? w_zero[static_cast<size_t>(row0) * G + i] : 0;
+    }
+  };
+
+  const bool early = (p.flags & 2) != 0;  // static weights: stream before the dependency wait
+  const uint32_t x_bytes = static_cast<uint32_t>(p.K) * 2;
+  uint4* nws = reinterpret_cast<uint4*>(smem + L.nw_off);
+  int issued = 0;
+  if (early && lane == 0) {
+    for (; issued < L.stages && issued < n_my; ++issued) issue(issued);
+    if (warp == 0 && p.norm_w != nullptr) {
+      mbar_arrive_expect_tx(&x_bar[1], x_bytes);
+      bulk_g2s(nws, p.norm_w, x_bytes, &x_bar[1]);
+    }
+  }
+  if (early) load_params();  // parameters too
+  griddep_wait();
+  if (!early) load_params();
+  if (lane == 0) {
+    if (warp == 0) {
+      mbar_arrive_expect_tx(&x_bar[0], x_bytes);
+      bulk_g2s(xs, p.x, x_bytes, &x_bar[0]);
+      if (!early && p.norm_w != nullptr) {
+        mbar_arrive_expect_tx(&x_bar[1], x_bytes);
+        bulk_g2s(nws, p.norm_w, x_bytes, &x_bar[1]);
+      }
+    }
+    if (!early)
+      for (; issued < L.stages && issued < n_my; ++issued) issue(issued);
+  }
+  if (threadIdx.x == 0) best_s = 0ull;
+  __syncthreads();  // barrier initialisation and the group parameters are visible to every warp
+  mbar_wait(&x_bar[0], 0);
+  if (p.norm_w != nullptr) rmsnorm_x_in_smem(p, xs, nws, nvec, red, &x_bar[1]);
+  __syncthreads();
+
+  // ---- main loop: consume this warp's ring; item = (16-row tile, k-part of chunk_groups groups) ----
+  const int g = lane >> 2, c = lane & 3;
+  for (int j = 0; j < n_my; ++j) {
+    const int s = j % L.stages;
+    const int item = warp + j * kWarps;
+    const int t = item / ksplit, part = item - t * ksplit;
+    mbar_wait(&my_bars[s], (j / L.stages) & 1);
+    const uint4* wv = reinterpret_cast<const uint4*>(my_ring + static_cast<size_t>(s) * chunk_bytes) + lane;
+    const int grp0 = part * L.chunk_groups;
+    const int pr = (t * kW4TileRows + g) * G + grp0;  // parameters of row g; row g + 8 at pr + 8 * G
+    const uint4* xv = xs + grp0 * (kW4Group / 8) + 2 * c;
+    float sum_g = 0.f, sum_g8 = 0.f;
+    for (int q = 0; q < L.chunk_groups; ++q) {
+      const uint32_t zg = (0x4300u | gz[pr + q]) * 0x10001u;
+      const uint32_t zg8 = (0x4300u | gz[pr + 8 * G + q]) * 0x10001u;
+      float d0[4] = {0.f, 0.f, 0.f, 0.f}, d1[4] = {0.f, 0.f, 0.f, 0.f};  // two chains of 4 dependent mma
+      w4_block(d0, wv[64 * q], xv[16 * q], xv[16 * q + 1], zg, zg8);
+      w4_block(d1, wv[64 * q + 32], xv[16 * q + 8], xv[16 * q + 9], zg, zg8);
+      sum_g = fmaf(__bfloat162float(gs[pr + q]), d0[0] + d1[0], sum_g);
+      sum_g8 = fmaf(__bfloat162float(gs[pr + 8 * G + q]), d0[2] + d1[2], sum_g8);
+    }
+    __syncwarp();  // every lane is done reading slot s
+    if (c == 0) {  // lanes 4g .. 4g+3 hold the same sums (the 8 columns of D are equal)
+      acc[(t * kW4TileRows + g) * ksplit + part] = sum_g;  // slot = row * ksplit + part
+      acc[(t * kW4TileRows + g + 8) * ksplit + part] = sum_g8;
+    }
+    if (lane == 0 && j + L.stages < n_my) issue(j + L.stages);
+  }
+  __syncthreads();
+  reduce_kparts(acc, nrows, ksplit);
+  gemv_epilogue<false>(p, acc, nullptr, row0, nrows, &best_s);
+}
+
+int gemv_w4_launch(const GemvParams& p, const __nv_bfloat16* w_gscale, const uint8_t* w_zero, cudaStream_t stream) {
+  const int sms = num_sms();
+  const int tiles = (p.N + kW4TileRows - 1) / kW4TileRows;
+  const int tiles_per_block = (tiles + sms - 1) / sms;
+  const int rows_per_block = tiles_per_block * kW4TileRows;  // even: a SwiGLU pair never straddles blocks
+  const int grid = (tiles + tiles_per_block - 1) / tiles_per_block;
+  const int G = p.K / kW4Group;
+  constexpr int kSmemBudget = 220 * 1024;
+  const int x1_bytes = (p.K * 2 + 127) / 128 * 128;
+  const int x_bytes = x1_bytes * (p.norm_w ? 2 : 1);
+  const int gp_bytes = (rows_per_block * G * 3 + 127) / 128 * 128;  // bf16 scales + uint8 zeros
+  const int bar_bytes = (kWarps * kW4MaxStages + 2) * 8;
+  // k-parts: whole groups per item; the largest chunk (<= 8 KB) with >= 3 stages per warp, unless the
+  // block then has fewer than 6 items per warp (a block's rows are few: split K further)
+  W4GemvLayout L;
+  int ksplit = -1;
+  for (int ks = 1; ks <= G; ++ks) {
+    if (G % ks) continue;
+    const int cb = G / ks * kW4GroupBytes;
+    if (cb > 8192) continue;
+    const int acc_bytes = (rows_per_block * ks * 4 + 127) / 128 * 128;
+    const int st = (kSmemBudget - x_bytes - acc_bytes - gp_bytes - bar_bytes - 256) / (kWarps * cb);
+    if (st < 3) continue;
+    ksplit = ks;
+    if (static_cast<long>(tiles_per_block) * ks >= 6L * kWarps) break;
+  }
+  if (ksplit < 0) return -1;
+  L.chunk_groups = G / ksplit;
+  const int chunk_bytes = L.chunk_groups * kW4GroupBytes;
+  L.x_off = 0;
+  L.nw_off = x1_bytes;
+  L.acc_off = x_bytes;
+  L.gs_off = L.acc_off + (rows_per_block * ksplit * 4 + 127) / 128 * 128;
+  L.gz_off = L.gs_off + rows_per_block * G * 2;
+  L.ring_off = L.gs_off + gp_bytes;
+  L.stages = std::min(kW4MaxStages, (kSmemBudget - L.ring_off - bar_bytes - 256) / (kWarps * chunk_bytes));
+  L.bar_off = (L.ring_off + kWarps * L.stages * chunk_bytes + 127) / 128 * 128;
+  L.total = L.bar_off + bar_bytes;
+  static PerDeviceOnce attr_once;
+  if (attr_once.first()) {
+    VB_CUDA(cudaFuncSetAttribute(gemv_w4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024));
+  }
+  VB_CUDA(launch_pdl(gemv_w4_kernel, dim3(grid), dim3(kThreads), static_cast<size_t>(L.total), stream, p,
+                     w_gscale, w_zero, rows_per_block, ksplit, L));
+  return 0;
+}
+
 }  // namespace
 
 // returns 0 on launch, -1 if the shape does not fit this kernel (caller falls back to the LSU kernel)
@@ -379,6 +631,21 @@ int gemv_tma_fp8(const GemvParams& p, cudaStream_t stream) {
            "gemv_fp8: w, x and norm_w must be 16-byte aligned");
   const int rc = gemv_tma_launch<true>(p, stream);
   VB_CHECK(rc >= 0, "gemv_fp8: N=%d K=%d does not fit the TMA ring (K / ksplit >= 512 bytes)", p.N, p.K);
+  return rc;
+}
+
+// 4-bit weights with group-128 scales and zero points: this kernel or an error, never a fallback
+int gemv_tma_w4a16(const GemvParams& p, const __nv_bfloat16* w_gscale, const uint8_t* w_zero, cudaStream_t stream) {
+  VB_CHECK(p.N > 0 && p.K > 0 && p.K % kW4Group == 0, "gemv_w4a16: bad shape N=%d K=%d (K %% 128 == 0)", p.N,
+           p.K);
+  VB_CHECK(!(p.flags & 1) || p.N % 2 == 0, "gemv_w4a16: swiglu needs even N");
+  VB_CHECK(!(p.flags & 4), "gemv_w4a16: there is no register-staged variant for 4-bit weights");
+  VB_CHECK(w_gscale != nullptr && w_zero != nullptr, "gemv_w4a16: group scales and zero points are required");
+  VB_CHECK(!(reinterpret_cast<uintptr_t>(p.w) & 15) && !(reinterpret_cast<uintptr_t>(p.x) & 15) &&
+               !(p.norm_w && (reinterpret_cast<uintptr_t>(p.norm_w) & 15)),
+           "gemv_w4a16: w, x and norm_w must be 16-byte aligned");
+  const int rc = gemv_w4_launch(p, w_gscale, w_zero, stream);
+  VB_CHECK(rc >= 0, "gemv_w4a16: N=%d K=%d does not fit the TMA ring", p.N, p.K);
   return rc;
 }
 

@@ -131,7 +131,7 @@ int rope_kv_append_table(__nv_bfloat16* qkv, const __nv_bfloat16* table, int S, 
 // ---- decode (M == 1) ----------------------------------------------------------------------------
 struct GemvParams {
   const __nv_bfloat16* x;       // [K]
-  const __nv_bfloat16* w;       // [N, K] (gemv_tma_fp8: e4m3 bytes)
+  const __nv_bfloat16* w;       // [N, K] (gemv_tma_fp8: e4m3 bytes; gemv_tma_w4a16: packed 4-bit codes)
   const __nv_bfloat16* bias;    // [N] or null
   const __nv_bfloat16* norm_w;  // [K] or null: fused RMSNorm prologue on x
   float norm_eps;
@@ -146,6 +146,9 @@ struct GemvParams {
 int gemv_bf16(const GemvParams& p, cudaStream_t stream);
 int gemv_tma_bf16(const GemvParams& p, cudaStream_t stream);  // -1: shape not supported
 int gemv_tma_fp8(const GemvParams& p, cudaStream_t stream);   // e4m3 weights, K % 16 == 0
+// 4-bit weights packed by quantize_w4_groups (vila_b200/model/qwen2.py), bf16 scales and uint8 zero
+// points [N, K / 128]; K % 128 == 0
+int gemv_tma_w4a16(const GemvParams& p, const __nv_bfloat16* w_gscale, const uint8_t* w_zero, cudaStream_t stream);
 // token = argmax key; token_hist[step++] = token; position++; key = 0; x_next = embed_table[token]
 int argmax_finalize(unsigned long long* key, int32_t* token_out, int32_t* token_hist,
                     int32_t* step_counter, int32_t* position, const __nv_bfloat16* embed_table,

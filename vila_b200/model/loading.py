@@ -111,10 +111,10 @@ def config_from_dir(model_dir: Path) -> LlavaConfig:
 
 
 def load_pretrained(model_path: str, device="cuda", model_cls=None, decode_weights: str = "bf16") -> LlavaLlamaModel:
-    """decode_weights: "bf16" or "fp8", the weights the single-stream greedy decoder streams
+    """decode_weights: "bf16", "fp8" or "w4a16", the weights the single-stream greedy decoder streams
     (Qwen2ForCausalLM.set_decode_weights); the checkpoint and every other path stay bf16."""
-    if decode_weights not in ("bf16", "fp8"):
-        raise ValueError(f"decode_weights must be 'bf16' or 'fp8', got {decode_weights!r}")
+    if decode_weights not in ("bf16", "fp8", "w4a16"):
+        raise ValueError(f"decode_weights must be 'bf16', 'fp8' or 'w4a16', got {decode_weights!r}")
     d = Path(model_path)
     cfg = config_from_dir(d)
     tok = None

@@ -148,6 +148,72 @@ def quantize_e4m3_rows(w: torch.Tensor, rows_per_chunk: int = 16384):
     return q, s
 
 
+W4_GROUP = 128  # consecutive k of one row sharing a scale and a zero point
+W4_TILE = 16    # rows per packed tile (the m of the kernel's mma.sync m16n8k16)
+
+
+def _w4_pack(q: torch.Tensor) -> torch.Tensor:
+    """codes q uint8 [R, K] (0..15, R % 16 == 0) -> packed bytes [R / 16, 8 K] in the order
+    vila_gemv_w4a16 reads (gemv_tma.cu): per 16-row tile [K/64][lane = 4g + c][mma step j][4 bytes], where
+    the 8 nibbles of (tile, 64-k block b, g, c, j) are rows (g, g + 8) x k0 + (0..3), k0 = b + 16c + 4j,
+    nibble p = 4 * (k % 2) + 2 * (k // 2 % 2) + (row is g + 8)."""
+    R, K = q.shape
+    t = q.view(R // W4_TILE, 2, 8, K // 64, 4, 4, 2, 2)      # [tile, h, g, b, c, j, kh, kl]
+    t = t.permute(0, 3, 2, 4, 5, 7, 6, 1).reshape(-1, 2)    # [tile, b, g, c, j, kl, kh, h] -> nibble pairs
+    return (t[:, 0] | (t[:, 1] << 4)).view(R // W4_TILE, 8 * K)
+
+
+def _w4_unpack(packed: torch.Tensor, K: int) -> torch.Tensor:
+    """inverse of _w4_pack -> codes uint8 [R, K]"""
+    T = packed.shape[0]
+    nib = torch.stack([packed & 15, packed >> 4], dim=-1)   # [T, 8K, 2]
+    t = nib.view(T, K // 64, 8, 4, 4, 2, 2, 2)              # [tile, b, g, c, j, kl, kh, h]
+    return t.permute(0, 7, 2, 1, 3, 4, 6, 5).reshape(T * W4_TILE, K)
+
+
+def quantize_w4_groups(w: torch.Tensor, rows_per_chunk: int = 16384):
+    """Weight-only 4-bit with a scale and a zero point per group of 128 consecutive k of a row (the
+    reference's TinyChat W4A16 / AWQ format, round to nearest, no calibration data).  Per row n and group g,
+    in fp32 on the bf16 values:
+        lo = min(0, min w), hi = max(0, max w);  s = bf16((hi - lo) / 15), or 1 if that is 0
+        z = clamp(round(-lo / s), 0, 15);  q = clamp(round(w / s) + z, 0, 15)   (round half to even)
+    dequantized (q - z) * s; zero is exact.  -> (packed uint8 [ceil(N/16), 8 K], s bf16 [N, K/128],
+    z uint8 [N, K/128]).  The packed byte order is vila_gemv_w4a16's and known only to this module:
+    dequantize_w4_groups reads it back.  Rows are converted in chunks to bound the fp32 temporary."""
+    N, K = w.shape
+    if K % W4_GROUP:
+        raise ValueError(f"quantize_w4_groups: K = {K} is not a multiple of {W4_GROUP}")
+    G = K // W4_GROUP
+    rows_per_chunk = max(W4_TILE, rows_per_chunk // W4_TILE * W4_TILE)
+    T = (N + W4_TILE - 1) // W4_TILE
+    packed = torch.empty(T, 8 * K, dtype=torch.uint8, device=w.device)
+    s = torch.empty(N, G, dtype=torch.bfloat16, device=w.device)
+    z = torch.empty(N, G, dtype=torch.uint8, device=w.device)
+    for a in range(0, N, rows_per_chunk):
+        wf = w[a:a + rows_per_chunk].float().view(-1, G, W4_GROUP)
+        lo = wf.amin(dim=2).clamp(max=0)
+        hi = wf.amax(dim=2).clamp(min=0)
+        sc = ((hi - lo) / 15).to(torch.bfloat16).float()
+        sc = torch.where(sc == 0, torch.ones_like(sc), sc)
+        zp = torch.round(-lo / sc).clamp(0, 15)
+        q = (torch.round(wf / sc[..., None]) + zp[..., None]).clamp(0, 15).to(torch.uint8).view(-1, K)
+        n = q.shape[0]
+        if n % W4_TILE:  # the last tile: rows past N are zero codes
+            q = torch.cat([q, q.new_zeros(W4_TILE - n % W4_TILE, K)])
+        packed[a // W4_TILE:a // W4_TILE + q.shape[0] // W4_TILE] = _w4_pack(q)
+        s[a:a + n] = sc.to(torch.bfloat16)
+        z[a:a + n] = zp.to(torch.uint8)
+    return packed, s, z
+
+
+def dequantize_w4_groups(packed: torch.Tensor, s: torch.Tensor, z: torch.Tensor) -> torch.Tensor:
+    """(packed, s, z) of quantize_w4_groups -> the weights it stands for, (q - z) * s in fp32 [N, K]"""
+    N, G = s.shape
+    K = G * W4_GROUP
+    q = _w4_unpack(packed, K)[:N].float().view(N, G, W4_GROUP)
+    return ((q - z.float()[..., None]) * s.float()[..., None]).view(N, K)
+
+
 class Qwen2ForCausalLM(nn.Module):
     def __init__(self, cfg: Qwen2Config, device="cuda", dtype=torch.bfloat16):
         super().__init__()
@@ -176,6 +242,7 @@ class Qwen2ForCausalLM(nn.Module):
         self._prefill_graphs = {}
         self.decode_weights = "bf16"
         self._fp8_weights = None
+        self._w4_weights = None
 
     # ---- HF-style accessors ----
     @property
@@ -367,14 +434,37 @@ class Qwen2ForCausalLM(nn.Module):
                   fused qkv, o_proj, interleaved gate/up and down_proj weights and of lm_head (a tied
                   lm_head is quantized as its own copy).  Half the bytes per token; for NVILA-8B the
                   copies take ~7.1 GB next to the bf16 weights, which stay.
-        The copies are plain attributes: state_dict() and save_pretrained do not change.  What stays
-        bf16 in either mode: the prefill (prompt K/V and last hidden state), the vision tower and
-        projector, BatchedDecoder / generate_batch, the eager sampling / logits-processor path and the
-        embedding gather.  Either call drops the cached decoder (its graphs bake in weight pointers)."""
-        if fmt not in ("bf16", "fp8"):
-            raise ValueError(f"decode weights must be 'bf16' or 'fp8', got {fmt!r}")
+          "w4a16" 4-bit copies with a bf16 scale and a uint8 zero point per group of 128 k
+                  (quantize_w4_groups, run by vila_gemv_w4a16) of the same layer weights; lm_head gets an
+                  e4m3 copy as in "fp8" mode (TinyChat / AWQ keep the output layer out of 4-bit).  For
+                  NVILA-8B 3.96 GB per token.  Every linear K must be a multiple of 128 (ValueError
+                  before anything is quantized).
+        The copies are plain attributes: state_dict() and save_pretrained do not change, and switching
+        modes frees the previous ones.  What stays bf16 in every mode: the prefill (prompt K/V and last
+        hidden state), the vision tower and projector, BatchedDecoder / generate_batch, the eager sampling
+        / logits-processor path and the embedding gather.  Every call drops the cached decoder (its graphs
+        bake in weight pointers)."""
+        if fmt not in ("bf16", "fp8", "w4a16"):
+            raise ValueError(f"decode weights must be 'bf16', 'fp8' or 'w4a16', got {fmt!r}")
+        if fmt == "w4a16":
+            cfg = self.config
+            ks = {"hidden_size": cfg.hidden_size, "num_attention_heads * head_dim":
+                  cfg.num_attention_heads * cfg.head_dim, "intermediate_size": cfg.intermediate_size}
+            bad = [f"{k} = {v}" for k, v in ks.items() if v % W4_GROUP]
+            if bad:
+                raise ValueError(f"w4a16 decode weights need every linear K to be a multiple of {W4_GROUP}: "
+                                 + ", ".join(bad))
         self._decoder = None
         self._fp8_weights = None
+        self._w4_weights = None
+        if fmt == "w4a16":
+            with torch.no_grad():
+                layers = [SimpleNamespace(qkv=quantize_w4_groups(layer._qkv_w),
+                                          o=quantize_w4_groups(layer.self_attn.o_proj.weight),
+                                          gu=quantize_w4_groups(layer._gu_w),
+                                          down=quantize_w4_groups(layer.mlp.down_proj.weight))
+                          for layer in self.model.layers]
+                self._w4_weights = SimpleNamespace(layers=layers, lm_head=quantize_e4m3_rows(self.lm_head.weight))
         if fmt == "fp8":
             with torch.no_grad():
                 layers = [SimpleNamespace(qkv=quantize_e4m3_rows(layer._qkv_w),
@@ -559,8 +649,9 @@ class GraphDecoder:
 
     The decoder streams the weights of the LLM's decode-weight mode at construction
     (Qwen2ForCausalLM.set_decode_weights): in "fp8" mode every GEMV of start() and of each step, lm_head
-    included, runs vila_gemv_fp8 on the e4m3 copies, so the first token is an fp8 lm_head result too.
-    The prompt's K/V and last hidden state come from the bf16 prefill in either mode."""
+    included, runs vila_gemv_fp8 on the e4m3 copies, so the first token is an fp8 lm_head result too.  In
+    "w4a16" mode the layer GEMVs run vila_gemv_w4a16 on the 4-bit copies and lm_head vila_gemv_fp8 on its
+    e4m3 copy.  The prompt's K/V and last hidden state come from the bf16 prefill in every mode."""
 
     MAX_SPLITS = 64
 
@@ -569,7 +660,9 @@ class GraphDecoder:
         cfg = llm.config
         dev, dt = llm.device, llm.dtype
         self.max_new = max_new
-        self.fp8 = llm._fp8_weights  # None: bf16 weights.  Held here: the graphs bake in its pointers
+        # None unless in that mode.  Held here: the graphs bake in their pointers
+        self.fp8 = llm._fp8_weights
+        self.w4 = llm._w4_weights
         Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
         self._fixed_splits = num_splits
         self.num_splits = 8 if num_splits is None else num_splits
@@ -642,8 +735,13 @@ class GraphDecoder:
 
     def _weights(self, li: Optional[int]):
         """-> (qkv, o, gate/up, down) of layer li, or lm_head for li None: each a dict of ops.gemv's
-        weight arguments (w, and w_scale in fp8 mode)"""
+        weight arguments (w, and w_scale in fp8 mode, w_scale and w_zero for w4a16 layers)"""
         llm = self.llm
+        if self.w4 is not None:
+            if li is None:
+                return dict(w=self.w4.lm_head[0], w_scale=self.w4.lm_head[1])
+            f = self.w4.layers[li]
+            return tuple(dict(w=p, w_scale=s, w_zero=z) for p, s, z in (f.qkv, f.o, f.gu, f.down))
         if self.fp8 is not None:
             if li is None:
                 return dict(w=self.fp8.lm_head[0], w_scale=self.fp8.lm_head[1])

@@ -319,14 +319,33 @@ def linear_qkv_rope(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tenso
 def gemv(x: torch.Tensor, w: torch.Tensor, *, bias=None, norm_w=None, norm_eps: float = 1e-6,
          residual=None, swiglu: bool = False, out: Optional[torch.Tensor] = None,
          argmax_key: Optional[torch.Tensor] = None, write_out: bool = True,
-         static_w: bool = False, variant: int = 0, w_scale: Optional[torch.Tensor] = None
-         ) -> Optional[torch.Tensor]:
+         static_w: bool = False, variant: int = 0, w_scale: Optional[torch.Tensor] = None,
+         w_zero: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
     """y = W x with the fused RMSNorm prologue and bias / residual / SwiGLU / argmax epilogues.
     w bf16 [N, K]; or w torch.float8_e4m3fn [N, K] with w_scale fp32 [N] (one scale per row), which
-    runs vila_gemv_fp8 (TMA-ring kernel only: variant=1 is refused)."""
+    runs vila_gemv_fp8; or w uint8, the packed 4-bit codes of quantize_w4_groups, with w_scale bf16
+    [N, K/128] and w_zero uint8 [N, K/128] (one scale and zero point per group of 128 k), which runs
+    vila_gemv_w4a16.  The quantized forms are TMA-ring kernels only: variant=1 is refused."""
     fp8 = w.dtype == torch.float8_e4m3fn
-    _chk(x, "x"); _chk(w, "w", torch.float8_e4m3fn if fp8 else torch.bfloat16)
-    N, K = w.shape
+    w4 = w.dtype == torch.uint8
+    _chk(x, "x"); _chk(w, "w", w.dtype if fp8 or w4 else torch.bfloat16)
+    if w4:
+        if w_scale is None or w_zero is None:
+            raise ValueError("gemv: packed 4-bit weights need w_scale (bf16 [N, K/128]) and w_zero (uint8 [N, K/128])")
+        _chk(w_scale, "w_scale"); _chk(w_zero, "w_zero", torch.uint8)
+        if w_scale.dim() != 2 or w_zero.shape != w_scale.shape or not (w_scale.is_contiguous() and w_zero.is_contiguous()):
+            raise ValueError(f"gemv: w_scale and w_zero must be contiguous [N, K/128] tensors of one shape, got "
+                             f"{tuple(w_scale.shape)} and {tuple(w_zero.shape)}")
+        N, K = w_scale.shape[0], w_scale.shape[1] * 128
+        if w.shape != ((N + 15) // 16, 8 * K) or not w.is_contiguous():
+            raise ValueError(f"gemv: packed 4-bit weights of [{N}, {K}] must be a contiguous uint8 "
+                             f"[{(N + 15) // 16}, {8 * K}] tensor, got {tuple(w.shape)}")
+        if variant == 1:
+            raise ValueError("gemv: the register-staged variant has no 4-bit form")
+    elif w_zero is not None:
+        raise ValueError("gemv: w_zero is only meaningful with packed 4-bit (uint8) weights")
+    else:
+        N, K = w.shape
     assert x.numel() == K and w.is_contiguous()
     if fp8:
         if w_scale is None:
@@ -336,8 +355,8 @@ def gemv(x: torch.Tensor, w: torch.Tensor, *, bias=None, norm_w=None, norm_eps: 
             raise ValueError(f"gemv: w_scale must be a contiguous fp32 [{N}] tensor, got {tuple(w_scale.shape)}")
         if variant == 1:
             raise ValueError("gemv: the register-staged variant has no float8_e4m3fn form")
-    elif w_scale is not None:
-        raise ValueError("gemv: w_scale is only meaningful with float8_e4m3fn weights")
+    elif w_scale is not None and not w4:
+        raise ValueError("gemv: w_scale is only meaningful with float8_e4m3fn or packed 4-bit weights")
     if out is None and write_out:
         out = torch.empty((N // 2 if swiglu else N,), dtype=torch.bfloat16, device=x.device)
     p = GemvParams()
@@ -348,6 +367,8 @@ def gemv(x: torch.Tensor, w: torch.Tensor, *, bias=None, norm_w=None, norm_eps: 
     p.argmax_key = _p(argmax_key)
     if fp8:
         check(_lib.load().vila_gemv_fp8(C.byref(p), _p(w_scale), _stream()), "vila_gemv_fp8")
+    elif w4:
+        check(_lib.load().vila_gemv_w4a16(C.byref(p), _p(w_scale), _p(w_zero), _stream()), "vila_gemv_w4a16")
     else:
         check(_lib.load().vila_gemv(C.byref(p), _stream()), "vila_gemv")
     return out
