@@ -220,6 +220,40 @@ int vila_gemv_fp8(const vila_gemv_params* p, const float* w_scale, void* stream)
  * its TinyChat W4A16 deployment (AWQ, group 128; README "Quantization and Deployment"). */
 int vila_gemv_w4a16(const vila_gemv_params* p, const void* w_scale, const uint8_t* w_zero, void* stream);
 
+/* Batched decode step on the quantized weights: y[m, :] = epilogue(W x[m, :]) for M = 1..16 activation
+ * rows in one launch, every weight byte read once.  w, w_scale and w_zero are the same copies as for
+ * vila_gemv_fp8 / vila_gemv_w4a16.  Row m of x is at x + m * ldx, of residual at residual + m * ld_res and
+ * of y at y + m * ldy (element strides, 16-byte multiples; x, w, y and residual 16-byte aligned).
+ * Epilogue per (row, m): the e4m3 row scale, bias, residual (may alias y: added in place) or SwiGLU on
+ * interleaved (gate, up) rows (y then has N / 2 values per row); no RMSNorm prologue and no argmax.
+ * Each output row depends on its own x row only: the partition follows from (N, K) and the device, and
+ * every sum runs in a fixed order, so a row's bits do not change with M or with the other rows.
+ * Errors, never a launch: M outside 1..16, K % 128 != 0 (w4a16) or K % 16 != 0 (fp8), misaligned
+ * pointers or strides, missing scales or zero points, odd N with SwiGLU, flags other than
+ * VILA_FLAG_SWIGLU | VILA_FLAG_STATIC_W.
+ * vila_gemv_batch_fp8 replaces the Linear layers of a batched decode step (HF nn.Linear at
+ * modeling_qwen2.py:81-95,164-176,223-226 over a batch of sequences) on e4m3 weights; vila_gemv_batch_w4a16
+ * the TinyChat W4A16 GEMM of the reference's 4-bit deployment (README "Quantization and Deployment"). */
+typedef struct vila_gemv_batch_params {
+  const void* x;
+  int64_t ldx;
+  const void* w;
+  const void* bias;
+  const void* residual;
+  int64_t ld_res;
+  void* y;
+  int64_t ldy;
+  int32_t M, N, K;
+  int32_t flags;
+} vila_gemv_batch_params;
+int vila_gemv_batch_fp8(const vila_gemv_batch_params* p, const float* w_scale, void* stream);
+int vila_gemv_batch_w4a16(const vila_gemv_batch_params* p, const void* w_scale, const uint8_t* w_zero,
+                          void* stream);
+/* The partition vila_gemv_batch_* use for (N, K) on the current device (fp8: 1 for e4m3 weights, 0 for
+ * w4a16): out[0] cluster size, out[1] CTAs, out[2] 16-row tiles per cluster, out[3] k-parts per slice,
+ * out[4] cudaOccupancyMaxActiveClusters at that cluster size, out[5] dynamic shared memory per CTA. */
+int vila_gemv_batch_partition(int N, int K, int fp8, int32_t* out);
+
 int vila_argmax_finalize(unsigned long long* key, int32_t* token_out, int32_t* token_hist,
                          int32_t* step_counter, int32_t* position, const void* embed_table,
                          void* x_next, int hidden, void* stream);

@@ -36,6 +36,14 @@ class GemvParams(C.Structure):
     ]
 
 
+class GemvBatchParams(C.Structure):
+    _fields_ = [
+        ("x", c_void_p), ("ldx", c_i64), ("w", c_void_p), ("bias", c_void_p), ("residual", c_void_p),
+        ("ld_res", c_i64), ("y", c_void_p), ("ldy", c_i64),
+        ("M", C.c_int32), ("N", C.c_int32), ("K", C.c_int32), ("flags", C.c_int32),
+    ]
+
+
 class DecodeAttnParams(C.Structure):
     _fields_ = [
         ("qkv", c_void_p), ("position", c_void_p), ("k_pool", c_void_p), ("v_pool", c_void_p),
@@ -103,6 +111,9 @@ SIGNATURES = {
     "vila_gemv": [C.POINTER(GemvParams), c_void_p],
     "vila_gemv_fp8": [C.POINTER(GemvParams), c_void_p, c_void_p],
     "vila_gemv_w4a16": [C.POINTER(GemvParams), c_void_p, c_void_p, c_void_p],
+    "vila_gemv_batch_fp8": [C.POINTER(GemvBatchParams), c_void_p, c_void_p],
+    "vila_gemv_batch_w4a16": [C.POINTER(GemvBatchParams), c_void_p, c_void_p, c_void_p],
+    "vila_gemv_batch_partition": [c_int, c_int, c_int, c_i32_p],
     "vila_argmax_finalize": [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                              c_int, c_void_p],
     "vila_decode_attention": [C.POINTER(DecodeAttnParams), c_void_p],

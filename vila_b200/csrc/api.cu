@@ -258,6 +258,43 @@ int vila_gemv_w4a16(const vila_gemv_params* p, const void* w_scale, const uint8_
   return vb::gemv_tma_w4a16(to_gemv(p), cb(w_scale), w_zero, st(stream));
 }
 
+static vb::GemvBatchArgs to_gemv_batch(const vila_gemv_batch_params* p) {
+  vb::GemvBatchArgs g;
+  g.x = cb(p->x);
+  g.ldx = p->ldx;
+  g.w = p->w;
+  g.bias = cb(p->bias);
+  g.residual = cb(p->residual);
+  g.ld_res = p->ld_res;
+  g.y = mb(p->y);
+  g.ldy = p->ldy;
+  g.M = p->M;
+  g.N = p->N;
+  g.K = p->K;
+  g.flags = p->flags;
+  return g;
+}
+
+// the Linear layers of a batched decode step (modeling_qwen2.py:81-95,164-176,223-226) on e4m3 weights
+int vila_gemv_batch_fp8(const vila_gemv_batch_params* p, const float* w_scale, void* stream) {
+  VB_REQUIRE_DEVICE();
+  VB_CHECK(p != nullptr, "vila_gemv_batch_fp8: params are required");
+  return vb::gemv_batch_fp8(to_gemv_batch(p), w_scale, st(stream));
+}
+
+// the TinyChat W4A16 GEMM of the reference's 4-bit deployment (README "Quantization and Deployment")
+int vila_gemv_batch_w4a16(const vila_gemv_batch_params* p, const void* w_scale, const uint8_t* w_zero,
+                          void* stream) {
+  VB_REQUIRE_DEVICE();
+  VB_CHECK(p != nullptr, "vila_gemv_batch_w4a16: params are required");
+  return vb::gemv_batch_w4a16(to_gemv_batch(p), cb(w_scale), w_zero, st(stream));
+}
+
+int vila_gemv_batch_partition(int N, int K, int fp8, int32_t* out) {
+  VB_REQUIRE_DEVICE();
+  return vb::gemv_batch_partition(N, K, fp8, out);
+}
+
 int vila_argmax_finalize(unsigned long long* key, int32_t* token_out, int32_t* token_hist,
                          int32_t* step_counter, int32_t* position, const void* embed_table,
                          void* x_next, int hidden, void* stream) {

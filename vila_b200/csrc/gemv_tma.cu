@@ -615,6 +615,458 @@ int gemv_w4_launch(const GemvParams& p, const __nv_bfloat16* w_gscale, const uin
   return 0;
 }
 
+// ---------------------------------------------------------------------------------------------------
+// Batched form (gemv_batch_kernel): y[m, :] = epilogue(W x[m, :]) for M <= 16 activation rows, on the
+// quantized copies of the W4A16 and FP8 forms, unchanged.  The mma.sync m16n8k16 of the W4A16 form takes
+// x as its B operand; here column g of B column tile t is x row 8t + g, so one A fragment serves 8 (kNT =
+// 1) or 16 (kNT = 2) rows of x and every weight byte is still read once per launch.
+//   * w4a16: A fragments from w4_pair as in gemv_w4_kernel; each group's fp32 fragment is scaled by s.
+//   * e4m3: an item is a 16-row tile x k-part copied as 16 row segments; in the ring the rows are
+//     padded to a pitch of 64 mod 128 bytes, so lanes g = 0, 1 of a quarter-warp read different banks.
+//     Lane (g, c) reads 16 contiguous bytes of rows g and g + 8 at k0 = b + 16c of the 64-k block b, the
+//     W4 layout's k order, so the x words are those of the W4 path.  e4m3 -> f16 -> f32 -> bf16 is exact.
+//     The row scale, staged in shared memory with the weights' parameters, multiplies the finished row sum.
+// K is cut into `cluster` slices (whole units: groups of 128 k, or 16 k for e4m3) streamed by the CTAs of
+// one thread-block cluster, which share a row block: each rank stages only its slice of the x rows.  The
+// ranks' fp32 partial sums are added through DSMEM in rank order, each rank finishing a share of the rows.
+// The partition (cluster size, row blocks, k-parts) follows from (N, K, format) and the device only, and
+// every sum runs in a fixed order: an output row depends on its own x row alone, for any M.
+constexpr int kBatchMaxStages = 12;
+constexpr int kBatchMaxRows = 16;
+constexpr int kBatchSmemBudget = 220 * 1024;
+constexpr int kBatchXBudget = 100 * 1024;     // x slice + cluster partial sums, per CTA
+constexpr int kBatchXBudgetOne = 120 * 1024;  // x of a cluster of one (no partial sums)
+
+struct BatchLayout {
+  int cluster;            // CTAs per cluster, each streaming one k-slice of the cluster's row block
+  int tiles_per_cluster;  // 16-row tiles per row block
+  int unit;               // k per slice unit: 128 (one w4 group) or 16 (e4m3)
+  int units;              // K / unit
+  int max_units;          // units of the largest slice
+  int parts;              // k-parts per slice: items per tile
+  int slot_bytes;         // ring slot (one item)
+  int row_pitch;          // e4m3: bytes per weight row in a slot
+  int x_pitch;            // bytes per x row in shared memory
+  int stages;
+  int x_off, part_off, gs_off, gz_off, ring_off, bar_off, total;  // gs: w4 group scales or e4m3 row scales
+};
+
+// two e4m3 (low byte = lower k) -> bf16x2, exactly
+__device__ __forceinline__ uint32_t e4m3x2_to_bf16x2(uint32_t v) {
+  const float2 f = e4m3x2_to_float2(v);
+  uint32_t r;
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(f.y), "f"(f.x));
+  return r;
+}
+
+__device__ __forceinline__ float ld_dsmem_f32(uint32_t cluster_addr) {
+  float v;
+  asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(cluster_addr));
+  return v;
+}
+
+// epilogue of one output element (row n, x row m), with the rounding points of gemv_epilogue; sc: the row
+// scales of the row block staged in shared memory, row n at sc[n - row0]
+template <bool kFp8>
+__device__ __forceinline__ void batch_finish(const GemvBatchArgs& p, const float* sc, int row0, int n, int m,
+                                             float v) {
+  if constexpr (kFp8) v *= sc[n - row0];
+  if (p.bias) v += __bfloat162float(p.bias[n]);
+  v = bf16_round(v);
+  if (p.residual) v = bf16_round(v + __bfloat162float(p.residual[m * p.ld_res + n]));
+  p.y[m * p.ldy + n] = __float2bfloat16(v);
+}
+template <bool kFp8>
+__device__ __forceinline__ void batch_finish_swiglu(const GemvBatchArgs& p, const float* sc, int row0, int n,
+                                                    int m, float g, float u) {  // n even: gate n, up n + 1
+  if constexpr (kFp8) {
+    g *= sc[n - row0];
+    u *= sc[n + 1 - row0];
+  }
+  if (p.bias) {
+    g += __bfloat162float(p.bias[n]);
+    u += __bfloat162float(p.bias[n + 1]);
+  }
+  g = bf16_round(g);
+  u = bf16_round(u);
+  p.y[m * p.ldy + (n >> 1)] = __float2bfloat16(bf16_round(silu_f(g)) * u);
+}
+
+template <bool kFp8, int kNT>
+__global__ void __launch_bounds__(kThreads, 1)
+gemv_batch_kernel(GemvBatchArgs p, const void* __restrict__ w_scale, const uint8_t* __restrict__ w_zero,
+                  BatchLayout L) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  uint8_t* xs = smem + L.x_off;                                             // [16][x_pitch]
+  float* part = reinterpret_cast<float*>(smem + L.part_off);                // [tiles * 16][16] (cluster > 1)
+  __nv_bfloat16* gs = reinterpret_cast<__nv_bfloat16*>(smem + L.gs_off);  // w4: [tiles * 16][max_units]
+  float* sc = reinterpret_cast<float*>(smem + L.gs_off);                    // e4m3: [tiles * 16] row scales
+  uint8_t* gz = smem + L.gz_off;
+  uint8_t* ring = smem + L.ring_off;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bar_off);
+  const float* row_scale = static_cast<const float*>(w_scale);
+  const __nv_bfloat16* gscale = static_cast<const __nv_bfloat16*>(w_scale);
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int rank = L.cluster > 1 ? static_cast<int>(cluster_ctarank()) : 0;
+  const int tile0 = static_cast<int>(blockIdx.x) / L.cluster * L.tiles_per_cluster;
+  const int ntiles = min(L.tiles_per_cluster, (p.N + 15) / 16 - tile0);  // the same on every rank
+  const int u0 = rank * L.units / L.cluster, nu = (rank + 1) * L.units / L.cluster - u0;  // this slice
+  const int k0 = u0 * L.unit;
+  const int my_tiles = ntiles > warp ? (ntiles - warp + kWarps - 1) / kWarps : 0;
+  const int n_my = my_tiles * L.parts;  // items (tile, part), the parts of a tile consecutive
+  uint8_t* my_ring = ring + static_cast<size_t>(warp) * L.stages * L.slot_bytes;
+  uint64_t* my_bars = bars + warp * kBatchMaxStages;
+  uint64_t* x_bar = bars + kWarps * kBatchMaxStages;
+
+  if (lane == 0) {
+    for (int s = 0; s < L.stages; ++s) mbar_init(&my_bars[s], 1);
+    if (warp == 0) mbar_init(x_bar, 1);
+    fence_barrier_init();
+  }
+  __syncwarp();
+  griddep_launch_dependents();
+
+  auto part_range = [&](int q, int& pu0) {  // units [pu0, pu0 + return) of the slice
+    pu0 = q * nu / L.parts;
+    return (q + 1) * nu / L.parts - pu0;
+  };
+  auto issue = [&](int j) {  // whole warp: copy item j of this warp into slot j % stages
+    const int t = tile0 + warp + (j / L.parts) * kWarps;
+    int pu0;
+    const int pu = part_range(j % L.parts, pu0);
+    const int s = j % L.stages;
+    uint8_t* dst = my_ring + static_cast<size_t>(s) * L.slot_bytes;
+    if constexpr (kFp8) {
+      const int rows = min(kW4TileRows, p.N - t * kW4TileRows), bytes = pu * L.unit;
+      if (lane == 0) mbar_arrive_expect_tx(&my_bars[s], rows * bytes);
+      __syncwarp();
+      if (lane < rows)
+        bulk_g2s(dst + lane * L.row_pitch,
+                 static_cast<const uint8_t*>(p.w) + static_cast<size_t>(t * kW4TileRows + lane) * p.K + k0 +
+                     pu0 * L.unit,
+                 bytes, &my_bars[s]);
+    } else {
+      if (lane == 0) {
+        const uint8_t* src = static_cast<const uint8_t*>(p.w) +
+                             static_cast<size_t>(t) * p.K * (kW4TileRows / 2) +
+                             static_cast<size_t>(u0 + pu0) * kW4GroupBytes;
+        mbar_arrive_expect_tx(&my_bars[s], pu * kW4GroupBytes);
+        bulk_g2s(dst, src, pu * kW4GroupBytes, &my_bars[s]);
+      }
+    }
+  };
+  auto load_params = [&]() {  // e4m3: row scales of the row block; w4: group scales / zeros of the slice
+    if constexpr (kFp8) {       // (rows past N: s = 0, z = 0)
+      for (int r = threadIdx.x; r < ntiles * kW4TileRows; r += kThreads) {
+        const int n = tile0 * kW4TileRows + r;
+        sc[r] = n < p.N ? row_scale[n] : 0.f;
+      }
+      return;
+    }
+    const int G = p.K / kW4Group;
+    for (int i = threadIdx.x; i < ntiles * kW4TileRows * nu; i += kThreads) {
+      const int r = i / nu, q = i - r * nu, n = tile0 * kW4TileRows + r;
+      const bool in = n < p.N;
+      gs[r * L.max_units + q] = in ? gscale[static_cast<size_t>(n) * G + u0 + q] : __float2bfloat16(0.f);
+      gz[r * L.max_units + q] = in ? w_zero[static_cast<size_t>(n) * G + u0 + q] : 0;
+    }
+  };
+
+  const bool early = (p.flags & 2) != 0;  // static weights: stream before the dependency wait
+  int issued = 0;
+  if (early) {
+    for (; issued < L.stages && issued < n_my; ++issued) issue(issued);
+    load_params();  // parameters too
+  }
+  griddep_wait();
+  if (!early) {
+    for (; issued < L.stages && issued < n_my; ++issued) issue(issued);
+    load_params();
+  }
+  // x rows of the slice: one bulk copy per row < M, rows M .. 8 kNT - 1 zero
+  const uint32_t x_bytes = static_cast<uint32_t>(nu * L.unit) * 2;
+  if (warp == 0) {
+    if (lane == 0) mbar_arrive_expect_tx(x_bar, p.M * x_bytes);
+    __syncwarp();
+    if (lane < p.M) bulk_g2s(xs + lane * L.x_pitch, p.x + lane * p.ldx + k0, x_bytes, x_bar);
+  }
+  for (int i = threadIdx.x; i < (8 * kNT - p.M) * (L.x_pitch >> 4); i += kThreads)
+    reinterpret_cast<uint4*>(xs + p.M * L.x_pitch)[i] = make_uint4(0, 0, 0, 0);
+  __syncthreads();  // barrier initialisation, group parameters and zero rows are visible to every warp
+  mbar_wait(x_bar, 0);
+
+  // ---- main loop; lane (g, c) sums rows g, g + 8 of its tile for x rows 8t + 2c, 8t + 2c + 1 ----
+  const int g = lane >> 2, c = lane & 3;
+  const uint8_t* xl = xs + g * L.x_pitch + 32 * c;  // + 8 x_pitch per column tile
+  float run[kNT][2][2];
+#pragma unroll
+  for (int t = 0; t < kNT; ++t) run[t][0][0] = run[t][0][1] = run[t][1][0] = run[t][1][1] = 0.f;
+  for (int j = 0; j < n_my; ++j) {
+    const int s = j % L.stages, q = j % L.parts;
+    const int tl = warp + (j / L.parts) * kWarps;  // tile of the row block
+    int pu0;
+    const int pu = part_range(q, pu0);
+    mbar_wait(&my_bars[s], (j / L.stages) & 1);
+    const uint8_t* slot = my_ring + static_cast<size_t>(s) * L.slot_bytes;
+    if constexpr (kFp8) {
+      float d[2][kNT][4];  // two chains: even and odd 64-k blocks
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int t = 0; t < kNT; ++t) d[h][t][0] = d[h][t][1] = d[h][t][2] = d[h][t][3] = 0.f;
+      const int kq = pu * L.unit;
+      const uint8_t* xq = xl + pu0 * L.unit * 2;
+      for (int kb = 0; kb < kq; kb += 128) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int k = kb + 64 * h;
+          const bool in = k + 16 * c < kq;  // a part ends on a 16-k boundary
+          const uint4 z4 = make_uint4(0, 0, 0, 0);
+          const uint4 wa = in ? *reinterpret_cast<const uint4*>(slot + g * L.row_pitch + k + 16 * c) : z4;
+          const uint4 wb = in ? *reinterpret_cast<const uint4*>(slot + (g + 8) * L.row_pitch + k + 16 * c) : z4;
+          uint32_t xw[kNT][8];
+#pragma unroll
+          for (int t = 0; t < kNT; ++t) {
+            const uint8_t* xp = xq + t * 8 * L.x_pitch + 2 * k;
+            const uint4 xa = in ? *reinterpret_cast<const uint4*>(xp) : z4;
+            const uint4 xb = in ? *reinterpret_cast<const uint4*>(xp + 16) : z4;
+            xw[t][0] = xa.x; xw[t][1] = xa.y; xw[t][2] = xa.z; xw[t][3] = xa.w;
+            xw[t][4] = xb.x; xw[t][5] = xb.y; xw[t][6] = xb.z; xw[t][7] = xb.w;
+          }
+          const uint32_t ra[4] = {wa.x, wa.y, wa.z, wa.w}, rb[4] = {wb.x, wb.y, wb.z, wb.w};
+#pragma unroll
+          for (int s4 = 0; s4 < 4; ++s4) {
+            const uint32_t a0 = e4m3x2_to_bf16x2(ra[s4]), a1 = e4m3x2_to_bf16x2(rb[s4]);
+            const uint32_t a2 = e4m3x2_to_bf16x2(ra[s4] >> 16), a3 = e4m3x2_to_bf16x2(rb[s4] >> 16);
+#pragma unroll
+            for (int t = 0; t < kNT; ++t)
+              mma_bf16_m16n8k16(d[h][t], a0, a1, a2, a3, xw[t][2 * s4], xw[t][2 * s4 + 1]);
+          }
+        }
+      }
+#pragma unroll
+      for (int t = 0; t < kNT; ++t) {
+        run[t][0][0] += d[0][t][0] + d[1][t][0];
+        run[t][0][1] += d[0][t][1] + d[1][t][1];
+        run[t][1][0] += d[0][t][2] + d[1][t][2];
+        run[t][1][1] += d[0][t][3] + d[1][t][3];
+      }
+    } else {
+      const uint4* wv = reinterpret_cast<const uint4*>(slot) + lane;
+      const int pr = (tl * kW4TileRows + g) * L.max_units + pu0;  // row g; row g + 8 at + 8 max_units
+      const uint8_t* xq = xl + pu0 * kW4Group * 2;
+      for (int gq = 0; gq < pu; ++gq) {
+        const uint32_t zg = (0x4300u | gz[pr + gq]) * 0x10001u;
+        const uint32_t zg8 = (0x4300u | gz[pr + 8 * L.max_units + gq]) * 0x10001u;
+        const float sg = __bfloat162float(gs[pr + gq]), sg8 = __bfloat162float(gs[pr + 8 * L.max_units + gq]);
+        float d[2][kNT][4];  // two chains of 4 dependent mma per column tile: the two 64-k blocks
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint4 wq = wv[64 * gq + 32 * h];
+          uint32_t xw[kNT][8];
+#pragma unroll
+          for (int t = 0; t < kNT; ++t) {
+            const uint8_t* xp = xq + t * 8 * L.x_pitch + gq * kW4Group * 2 + 128 * h;
+            const uint4 xa = *reinterpret_cast<const uint4*>(xp), xb = *reinterpret_cast<const uint4*>(xp + 16);
+            xw[t][0] = xa.x; xw[t][1] = xa.y; xw[t][2] = xa.z; xw[t][3] = xa.w;
+            xw[t][4] = xb.x; xw[t][5] = xb.y; xw[t][6] = xb.z; xw[t][7] = xb.w;
+            d[h][t][0] = d[h][t][1] = d[h][t][2] = d[h][t][3] = 0.f;
+          }
+          const uint32_t ws[4] = {wq.x, wq.y, wq.z, wq.w};
+#pragma unroll
+          for (int s4 = 0; s4 < 4; ++s4) {
+            const uint32_t a0 = w4_pair(ws[s4], 0, zg), a1 = w4_pair(ws[s4], 1, zg8);
+            const uint32_t a2 = w4_pair(ws[s4], 2, zg), a3 = w4_pair(ws[s4], 3, zg8);
+#pragma unroll
+            for (int t = 0; t < kNT; ++t)
+              mma_bf16_m16n8k16(d[h][t], a0, a1, a2, a3, xw[t][2 * s4], xw[t][2 * s4 + 1]);
+          }
+        }
+#pragma unroll
+        for (int t = 0; t < kNT; ++t) {
+          run[t][0][0] = fmaf(sg, d[0][t][0] + d[1][t][0], run[t][0][0]);
+          run[t][0][1] = fmaf(sg, d[0][t][1] + d[1][t][1], run[t][0][1]);
+          run[t][1][0] = fmaf(sg8, d[0][t][2] + d[1][t][2], run[t][1][0]);
+          run[t][1][1] = fmaf(sg8, d[0][t][3] + d[1][t][3], run[t][1][1]);
+        }
+      }
+    }
+    __syncwarp();  // every lane is done reading slot s
+    if (j + L.stages < n_my) issue(j + L.stages);
+    if (q == L.parts - 1) {  // the tile's slice is summed
+      const int n0 = (tile0 + tl) * kW4TileRows + g;
+#pragma unroll
+      for (int t = 0; t < kNT; ++t)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int n = n0 + 8 * h, m = 8 * t + 2 * c + e;
+            const float v = run[t][h][e];
+            run[t][h][e] = 0.f;
+            if (L.cluster > 1) {
+              part[((tl * kW4TileRows) + g + 8 * h) * kBatchMaxRows + m] = v;
+            } else if (p.flags & 1) {
+              const float u = __shfl_down_sync(0xffffffffu, v, 4);  // row n + 1: lane g + 1
+              if (!(g & 1) && n < p.N && m < p.M) batch_finish_swiglu<kFp8>(p, sc, tile0 * kW4TileRows, n, m, v, u);
+            } else if (n < p.N && m < p.M) {
+              batch_finish<kFp8>(p, sc, tile0 * kW4TileRows, n, m, v);
+            }
+          }
+    }
+  }
+  if (L.cluster > 1) {
+    cluster_sync_all();  // every rank's partial sums are written
+    const int rows = ntiles * kW4TileRows;
+    const int share = ((rows + L.cluster - 1) / L.cluster + 1) & ~1;  // even: SwiGLU pairs stay together
+    const int r0 = rank * share, r1 = min(rows, r0 + share);
+    const uint32_t part_addr = smem_u32(part);
+    const bool swiglu = (p.flags & 1) != 0;
+    const int per = swiglu ? 2 : 1;
+    for (int i = threadIdx.x; i < (r1 - r0) / per * p.M; i += kThreads) {
+      const int r = r0 + i / p.M * per, m = i % p.M, n = tile0 * kW4TileRows + r;
+      if (n >= p.N) continue;
+      float v = 0.f, u = 0.f;
+      for (int k = 0; k < L.cluster; ++k) {  // ranks in order
+        const uint32_t a = mapa_u32(part_addr + (r * kBatchMaxRows + m) * 4, k);
+        v += ld_dsmem_f32(a);
+        if (swiglu) u += ld_dsmem_f32(a + kBatchMaxRows * 4);
+      }
+      if (swiglu) batch_finish_swiglu<kFp8>(p, sc, tile0 * kW4TileRows, n, m, v, u);
+      else batch_finish<kFp8>(p, sc, tile0 * kW4TileRows, n, m, v);
+    }
+    cluster_sync_all();  // no CTA leaves while its partial sums are read
+  }
+}
+
+template <bool kFp8, int kNT>
+int batch_set_smem_attr() {
+  static PerDeviceOnce once;
+  if (once.first()) {
+    VB_CUDA(cudaFuncSetAttribute(gemv_batch_kernel<kFp8, kNT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 224 * 1024));
+  }
+  return 0;
+}
+
+// clusters of `cluster` CTAs that can be resident at once with one CTA per SM (from the device only)
+int batch_max_active_clusters(int cluster) {
+  static int cache[64][4] = {};
+  int dev = 0;
+  VB_CUDA(cudaGetDevice(&dev));
+  int ci = cluster == 1 ? 0 : cluster == 2 ? 1 : cluster == 4 ? 2 : 3;
+  int& v = cache[dev & 63][ci];
+  if (v == 0) {
+    if (batch_set_smem_attr<false, 2>() != 0) return -1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(cluster);
+    cfg.blockDim = dim3(kThreads);
+    cfg.dynamicSmemBytes = 224 * 1024;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = cluster;
+    attr.val.clusterDim.y = attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    int n = 0;
+    VB_CUDA(cudaOccupancyMaxActiveClusters(&n, gemv_batch_kernel<false, 2>, &cfg));
+    v = n > 0 ? n : -1;
+  }
+  return v;
+}
+
+// The partition of one (N, K, format) on this device: the smallest cluster whose x slice and partial sums
+// fit kBatchXBudget (else a cluster of one, if its x fits kBatchXBudgetOne), then the fewest k-parts per
+// slice that leave >= 3 ring stages per warp.  -1: no partition fits.
+int batch_partition(int N, int K, bool fp8, BatchLayout& L) {
+  const int sms = num_sms();
+  const int tiles = (N + kW4TileRows - 1) / kW4TileRows;
+  L.unit = fp8 ? 16 : kW4Group;
+  L.units = K / L.unit;
+  auto x_pitch = [&](int cl) { return ((L.units + cl - 1) / cl * L.unit * 2 + 127) / 128 * 128 + 16; };
+  auto tpc = [&](int cl) {
+    int active = batch_max_active_clusters(cl);
+    int n = std::max(1, std::min(sms / cl, active > 0 ? active : sms / cl));
+    return (tiles + n - 1) / n;
+  };
+  L.cluster = 0;
+  for (int cl = 1; cl <= 8; cl *= 2) {
+    if (L.units < 4 * cl) break;
+    const int xb = kBatchMaxRows * x_pitch(cl), pb = cl > 1 ? tpc(cl) * kW4TileRows * kBatchMaxRows * 4 : 0;
+    if (xb + pb <= kBatchXBudget) {
+      L.cluster = cl;
+      break;
+    }
+  }
+  if (L.cluster == 0) {
+    if (kBatchMaxRows * x_pitch(1) > kBatchXBudgetOne) return -1;
+    L.cluster = 1;
+  }
+  L.tiles_per_cluster = tpc(L.cluster);
+  L.max_units = (L.units + L.cluster - 1) / L.cluster;
+  L.x_pitch = x_pitch(L.cluster);
+  const int rows = L.tiles_per_cluster * kW4TileRows;
+  L.x_off = 0;
+  L.part_off = kBatchMaxRows * L.x_pitch;
+  L.gs_off = L.part_off + (L.cluster > 1 ? rows * kBatchMaxRows * 4 : 0);
+  L.gz_off = L.gs_off + (fp8 ? rows * 4 : rows * L.max_units * 2);  // e4m3 row scales / w4 group scales
+  L.ring_off = (L.gz_off + (fp8 ? 0 : rows * L.max_units) + 127) / 128 * 128;
+  const int bar_bytes = (kWarps * kBatchMaxStages + 1) * 8;
+  const int max_chunk = fp8 ? 32 : 8;  // units per item: <= 512 bytes per e4m3 row, <= 8 w4 groups
+  for (L.parts = (L.max_units + max_chunk - 1) / max_chunk; L.parts <= L.max_units; ++L.parts) {
+    const int chunk = (L.max_units + L.parts - 1) / L.parts;
+    L.row_pitch = fp8 ? (chunk * L.unit + 127) / 128 * 128 + 64 : 0;
+    L.slot_bytes = fp8 ? kW4TileRows * L.row_pitch : chunk * kW4GroupBytes;
+    L.stages = std::min(kBatchMaxStages, (kBatchSmemBudget - L.ring_off - bar_bytes) / (kWarps * L.slot_bytes));
+    if (L.stages >= 3) break;
+  }
+  if (L.parts > L.max_units || L.stages < 3) return -1;
+  L.bar_off = (L.ring_off + kWarps * L.stages * L.slot_bytes + 127) / 128 * 128;
+  L.total = L.bar_off + bar_bytes;
+  return 0;
+}
+
+template <bool kFp8, int kNT>
+int gemv_batch_launch(const GemvBatchArgs& p, const void* w_scale, const uint8_t* w_zero, const BatchLayout& L,
+                      cudaStream_t stream) {
+  if (batch_set_smem_attr<kFp8, kNT>() != 0) return 2;
+  const int tiles = (p.N + kW4TileRows - 1) / kW4TileRows;
+  const int grid = (tiles + L.tiles_per_cluster - 1) / L.tiles_per_cluster * L.cluster;
+  VB_CUDA(launch_pdl_cluster(gemv_batch_kernel<kFp8, kNT>, dim3(grid), dim3(kThreads),
+                             static_cast<size_t>(L.total), stream, dim3(L.cluster, 1, 1), p, w_scale, w_zero, L));
+  return 0;
+}
+
+int gemv_batch(const GemvBatchArgs& p, const void* w_scale, const uint8_t* w_zero, bool fp8, cudaStream_t stream) {
+  const char* name = fp8 ? "gemv_batch_fp8" : "gemv_batch_w4a16";
+  const int unit = fp8 ? 16 : kW4Group;
+  VB_CHECK(p.M >= 1 && p.M <= kBatchMaxRows, "%s: M=%d outside 1..%d", name, p.M, kBatchMaxRows);
+  VB_CHECK(p.N > 0 && p.K > 0 && p.K % unit == 0, "%s: bad shape N=%d K=%d (K %% %d == 0)", name, p.N, p.K, unit);
+  VB_CHECK(!(p.flags & ~3), "%s: unknown flags 0x%x", name, p.flags);
+  VB_CHECK(!(p.flags & 1) || p.N % 2 == 0, "%s: swiglu needs even N", name);
+  VB_CHECK(w_scale != nullptr && (fp8 || w_zero != nullptr),
+           fp8 ? "%s: w_scale is required" : "%s: group scales and zero points are required", name);
+  VB_CHECK(p.x != nullptr && p.w != nullptr && p.y != nullptr, "%s: x, w and y are required", name);
+  const int n_out = (p.flags & 1) ? p.N / 2 : p.N;
+  VB_CHECK(!(reinterpret_cast<uintptr_t>(p.w) & 15) && !(reinterpret_cast<uintptr_t>(p.x) & 15) &&
+               !(reinterpret_cast<uintptr_t>(p.y) & 15) &&
+               !(p.residual && (reinterpret_cast<uintptr_t>(p.residual) & 15)),
+           "%s: w, x, y and residual must be 16-byte aligned", name);
+  VB_CHECK(p.ldx % 8 == 0 && p.ldy % 8 == 0 && (!p.residual || p.ld_res % 8 == 0),
+           "%s: row strides must be 16-byte multiples (ldx=%lld ldy=%lld ld_res=%lld)", name,
+           static_cast<long long>(p.ldx), static_cast<long long>(p.ldy), static_cast<long long>(p.ld_res));
+  VB_CHECK((p.M == 1 || p.ldx >= p.K) && (p.M == 1 || p.ldy >= n_out) && (!p.residual || p.M == 1 || p.ld_res >= p.N),
+           "%s: row strides shorter than a row", name);
+  BatchLayout L;
+  VB_CHECK(batch_partition(p.N, p.K, fp8, L) == 0, "%s: N=%d K=%d does not fit the TMA rings", name, p.N, p.K);
+  const int nt = p.M > 8 ? 2 : 1;
+  if (fp8) return nt == 1 ? gemv_batch_launch<true, 1>(p, w_scale, w_zero, L, stream)
+                          : gemv_batch_launch<true, 2>(p, w_scale, w_zero, L, stream);
+  return nt == 1 ? gemv_batch_launch<false, 1>(p, w_scale, w_zero, L, stream)
+                 : gemv_batch_launch<false, 2>(p, w_scale, w_zero, L, stream);
+}
+
 }  // namespace
 
 // returns 0 on launch, -1 if the shape does not fit this kernel (caller falls back to the LSU kernel)
@@ -647,6 +1099,28 @@ int gemv_tma_w4a16(const GemvParams& p, const __nv_bfloat16* w_gscale, const uin
   const int rc = gemv_w4_launch(p, w_gscale, w_zero, stream);
   VB_CHECK(rc >= 0, "gemv_w4a16: N=%d K=%d does not fit the TMA ring", p.N, p.K);
   return rc;
+}
+
+// batched forms: this kernel or an error, never a fallback
+int gemv_batch_fp8(const GemvBatchArgs& p, const float* w_scale, cudaStream_t stream) {
+  return gemv_batch(p, w_scale, nullptr, true, stream);
+}
+int gemv_batch_w4a16(const GemvBatchArgs& p, const __nv_bfloat16* w_gscale, const uint8_t* w_zero,
+                     cudaStream_t stream) {
+  return gemv_batch(p, w_gscale, w_zero, false, stream);
+}
+int gemv_batch_partition(int N, int K, int fp8, int32_t* out) {
+  VB_CHECK(out != nullptr && N > 0 && K > 0 && K % (fp8 ? 16 : kW4Group) == 0, "gemv_batch_partition: bad shape");
+  BatchLayout L;
+  VB_CHECK(batch_partition(N, K, fp8 != 0, L) == 0, "gemv_batch_partition: N=%d K=%d does not fit", N, K);
+  const int tiles = (N + kW4TileRows - 1) / kW4TileRows;
+  out[0] = L.cluster;
+  out[1] = (tiles + L.tiles_per_cluster - 1) / L.tiles_per_cluster * L.cluster;
+  out[2] = L.tiles_per_cluster;
+  out[3] = L.parts;
+  out[4] = batch_max_active_clusters(L.cluster);
+  out[5] = L.total;
+  return 0;
 }
 
 }  // namespace vb

@@ -149,6 +149,23 @@ int gemv_tma_fp8(const GemvParams& p, cudaStream_t stream);   // e4m3 weights, K
 // 4-bit weights packed by quantize_w4_groups (vila_b200/model/qwen2.py), bf16 scales and uint8 zero
 // points [N, K / 128]; K % 128 == 0
 int gemv_tma_w4a16(const GemvParams& p, const __nv_bfloat16* w_gscale, const uint8_t* w_zero, cudaStream_t stream);
+// M <= 16 activation rows against the same quantized copies (gemv_batch_kernel): y[m] = epilogue(W x[m])
+struct GemvBatchArgs {
+  const __nv_bfloat16* x;         // [M, ldx]
+  int64_t ldx;
+  const void* w;                  // e4m3 [N, K], or the packed 4-bit codes
+  const __nv_bfloat16* bias;      // [N] or null
+  const __nv_bfloat16* residual;  // [M, ld_res] or null; may alias y
+  int64_t ld_res;
+  __nv_bfloat16* y;               // [M, ldy]: N (or N/2 with SwiGLU) values per row
+  int64_t ldy;
+  int M, N, K, flags;             // flags: bit0 SwiGLU, bit1 static weights
+};
+int gemv_batch_fp8(const GemvBatchArgs& p, const float* w_scale, cudaStream_t stream);
+int gemv_batch_w4a16(const GemvBatchArgs& p, const __nv_bfloat16* w_gscale, const uint8_t* w_zero,
+                     cudaStream_t stream);
+// out: {cluster size, CTAs, tiles per cluster, k-parts per slice, max active clusters, dynamic smem bytes}
+int gemv_batch_partition(int N, int K, int fp8, int32_t* out);
 // token = argmax key; token_hist[step++] = token; position++; key = 0; x_next = embed_table[token]
 int argmax_finalize(unsigned long long* key, int32_t* token_out, int32_t* token_hist,
                     int32_t* step_counter, int32_t* position, const __nv_bfloat16* embed_table,

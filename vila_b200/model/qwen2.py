@@ -440,10 +440,11 @@ class Qwen2ForCausalLM(nn.Module):
                   NVILA-8B 3.96 GB per token.  Every linear K must be a multiple of 128 (ValueError
                   before anything is quantized).
         The copies are plain attributes: state_dict() and save_pretrained do not change, and switching
-        modes frees the previous ones.  What stays bf16 in every mode: the prefill (prompt K/V and last
-        hidden state), the vision tower and projector, BatchedDecoder / generate_batch, the eager sampling
-        / logits-processor path and the embedding gather.  Every call drops the cached decoder (its graphs
-        bake in weight pointers)."""
+        modes frees the previous ones.  The continuous-batching engine (serving.BatchedDecoder /
+        generate_batch, built after this call) runs the same copies with vila_gemv_batch_fp8 /
+        vila_gemv_batch_w4a16.  What stays bf16 in every mode: the prefill (prompt K/V and last hidden
+        state), the vision tower and projector, the eager sampling / logits-processor path and the embedding
+        gather.  Every call drops the cached decoder (its graphs bake in weight pointers)."""
         if fmt not in ("bf16", "fp8", "w4a16"):
             raise ValueError(f"decode weights must be 'bf16', 'fp8' or 'w4a16', got {fmt!r}")
         if fmt == "w4a16":

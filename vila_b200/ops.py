@@ -11,7 +11,7 @@ from typing import Optional, Sequence
 import torch
 
 from . import _lib
-from ._lib import DecodeAttnParams, DecodeAttnSplitParams, FmhaParams, GemvParams, check
+from ._lib import DecodeAttnParams, DecodeAttnSplitParams, FmhaParams, GemvBatchParams, GemvParams, check
 
 ACT_NONE, ACT_GELU_TANH, ACT_GELU_ERF, ACT_SILU = 0, 1, 2, 3
 
@@ -372,6 +372,86 @@ def gemv(x: torch.Tensor, w: torch.Tensor, *, bias=None, norm_w=None, norm_eps: 
     else:
         check(_lib.load().vila_gemv(C.byref(p), _stream()), "vila_gemv")
     return out
+
+
+GEMV_BATCH_MAX_M = 16  # activation rows per vila_gemv_batch_* launch
+
+
+def gemv_batch(x: torch.Tensor, w: torch.Tensor, *, w_scale: torch.Tensor, w_zero: Optional[torch.Tensor] = None,
+               bias: Optional[torch.Tensor] = None, residual: Optional[torch.Tensor] = None, swiglu: bool = False,
+               out: Optional[torch.Tensor] = None, static_w: bool = False) -> torch.Tensor:
+    """y[m] = epilogue(W x[m]) for the rows of x [M, K] on quantized weights, every weight byte read once per
+    group of 16 rows: w torch.float8_e4m3fn [N, K] with w_scale fp32 [N] (vila_gemv_batch_fp8), or the
+    packed 4-bit codes of quantize_w4_groups with w_scale bf16 [N, K/128] and w_zero uint8 [N, K/128]
+    (vila_gemv_batch_w4a16).  Epilogue: bias, residual [M, N] (may be `out`: added in place) or SwiGLU on
+    interleaved rows (out [M, N/2]).  M > 16 runs one launch per 16 rows; a row's result depends on that
+    row alone, so it is the same for any M.  bf16 weights are refused: their batches run ops.linear."""
+    fp8 = w.dtype == torch.float8_e4m3fn
+    w4 = w.dtype == torch.uint8
+    if not (fp8 or w4):
+        raise ValueError(f"gemv_batch: weights must be float8_e4m3fn or packed 4-bit (uint8), got {w.dtype}; "
+                         "bf16 batches run ops.linear")
+    if w_scale is None:
+        raise ValueError("gemv_batch: w_scale is required")
+    if w4:
+        if w_zero is None:
+            raise ValueError("gemv_batch: packed 4-bit weights need w_scale (bf16 [N, K/128]) and w_zero (uint8 [N, K/128])")
+        if w_scale.dim() != 2 or w_zero.shape != w_scale.shape or not (w_scale.is_contiguous() and w_zero.is_contiguous()):
+            raise ValueError(f"gemv_batch: w_scale and w_zero must be contiguous [N, K/128] tensors of one shape, got "
+                             f"{tuple(w_scale.shape)} and {tuple(w_zero.shape)}")
+        N, K = w_scale.shape[0], w_scale.shape[1] * 128
+        if w.shape != ((N + 15) // 16, 8 * K) or not w.is_contiguous():
+            raise ValueError(f"gemv_batch: packed 4-bit weights of [{N}, {K}] must be a contiguous uint8 "
+                             f"[{(N + 15) // 16}, {8 * K}] tensor, got {tuple(w.shape)}")
+    else:
+        if w_zero is not None:
+            raise ValueError("gemv_batch: w_zero is only meaningful with packed 4-bit (uint8) weights")
+        N, K = w.shape
+        if w_scale.shape != (N,) or not w_scale.is_contiguous() or not w.is_contiguous():
+            raise ValueError(f"gemv_batch: e4m3 weights need a contiguous fp32 w_scale [{N}], got {tuple(w_scale.shape)}")
+    if x.dim() != 2 or x.shape[1] != K or x.stride(1) != 1:
+        raise ValueError(f"gemv_batch: x must be [M, {K}] with unit column stride, got {tuple(x.shape)}")
+    if swiglu and residual is not None:
+        raise ValueError("gemv_batch: residual and swiglu do not combine")
+    M = x.shape[0]
+    n_out = N // 2 if swiglu else N
+    if out is None:  # rows padded to a 16-byte multiple: the kernel takes such row strides only
+        out = torch.empty((M, (n_out + 7) // 8 * 8), dtype=torch.bfloat16, device=x.device)[:, :n_out]
+    else:
+        if out.shape != (M, n_out) or out.stride(1) != 1:
+            raise ValueError(f"gemv_batch: out must be [{M}, {n_out}] with unit column stride, got {tuple(out.shape)}")
+    if residual is not None:
+        if residual.shape != (M, N) or residual.stride(1) != 1:
+            raise ValueError(f"gemv_batch: residual must be [{M}, {N}] with unit column stride, got {tuple(residual.shape)}")
+    if bias is not None:
+        if bias.shape != (N,) or not bias.is_contiguous():
+            raise ValueError(f"gemv_batch: bias must be a contiguous [{N}] tensor, got {tuple(bias.shape)}")
+    for t, name, dt in ((x, "x", torch.bfloat16), (w, "w", w.dtype), (out, "out", torch.bfloat16),
+                        (w_scale, "w_scale", torch.bfloat16 if w4 else torch.float32), (w_zero, "w_zero", torch.uint8),
+                        (residual, "residual", torch.bfloat16), (bias, "bias", torch.bfloat16)):
+        if t is not None:
+            _chk(t, name, dt)
+    lib = _lib.load()
+    for m0 in range(0, M, GEMV_BATCH_MAX_M):
+        m1 = min(M, m0 + GEMV_BATCH_MAX_M)
+        p = GemvBatchParams()
+        p.x, p.ldx, p.w, p.bias = x[m0].data_ptr(), x.stride(0), _p(w), _p(bias)
+        p.residual = None if residual is None else residual[m0].data_ptr()
+        p.ld_res = 0 if residual is None else residual.stride(0)
+        p.y, p.ldy = out[m0].data_ptr(), out.stride(0)
+        p.M, p.N, p.K, p.flags = m1 - m0, N, K, (1 if swiglu else 0) | (2 if static_w else 0)
+        if fp8:
+            check(lib.vila_gemv_batch_fp8(C.byref(p), _p(w_scale), _stream()), "vila_gemv_batch_fp8")
+        else:
+            check(lib.vila_gemv_batch_w4a16(C.byref(p), _p(w_scale), _p(w_zero), _stream()), "vila_gemv_batch_w4a16")
+    return out
+
+
+def gemv_batch_partition(N: int, K: int, fp8: bool) -> dict:
+    """the partition vila_gemv_batch_* use for (N, K) on the current device (vila_gemv_batch_partition)"""
+    out = (C.c_int32 * 6)()
+    check(_lib.load().vila_gemv_batch_partition(N, K, 1 if fp8 else 0, out), "vila_gemv_batch_partition")
+    return dict(zip(("cluster", "ctas", "tiles_per_cluster", "parts", "max_active_clusters", "smem_bytes"), out))
 
 
 def argmax_finalize(key: torch.Tensor, token_out: torch.Tensor, token_hist=None, step_counter=None,

@@ -238,8 +238,8 @@ def main() -> None:
     ap.add_argument("--slots", type=int, default=8)
     ap.add_argument("--decode-weights", choices=("bf16", "fp8", "w4a16"), default="bf16",
                     help="weights of the single-stream greedy decoder (fp8: e4m3 with per-row scales; w4a16: "
-                         "4-bit with group-128 scales and zero points, lm_head e4m3; prefill and the batching "
-                         "engine stay bf16)")
+                         "4-bit with group-128 scales and zero points, lm_head e4m3), and of the engine that "
+                         "batches queued requests; the prefill stays bf16)")
     args = ap.parse_args()
     model = llava.load(args.model_path, decode_weights=args.decode_weights)
     uvicorn.run(create_app(model, get_model_name_from_path(args.model_path), args.slots), host=args.host,

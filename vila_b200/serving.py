@@ -18,7 +18,10 @@ tokens per byte by B.  Here:
   * slots longer than HEAD_KERNEL_TOKENS (video, dynamic-S2) are attended by the batched split-KV
     kernel (`vila_decode_attention_split_batch`) in the same step; which kernel serves a slot follows
     only from that slot's own length, so a request's ids never depend on its neighbours;
-  * finished slots (EOS / budget) are harvested and refilled between graph replays.
+  * finished slots (EOS / budget) are harvested and refilled between graph replays;
+  * in the LLM's "fp8" / "w4a16" decode-weight modes (Qwen2ForCausalLM.set_decode_weights) the step's
+    GEMMs run `vila_gemv_batch_*` on the quantized copies (up to 16 slots per launch, every weight byte
+    read once per launch) and each slot's first token comes from the e4m3 lm_head; the prefill stays bf16.
 """
 from __future__ import annotations
 
@@ -118,12 +121,20 @@ class BatchedDecoder:
     Pages are handed out on demand (PageAllocator): a slot holds ceil(tokens / 128) pages, grows page by
     page while it decodes and returns them when it is released, so `total_pages` can be smaller than
     slots * pages_per_slot (long and short requests share the pool).  The page-table rows live on the
-    device and are read by the kernels at every launch: changing them needs no graph re-capture."""
+    device and are read by the kernels at every launch: changing them needs no graph re-capture.
+
+    The decoder streams the weights of the LLM's decode-weight mode at construction (`decode_weights`):
+    "bf16" runs the wgmma GEMMs on the parameters; "fp8" and "w4a16" run ops.gemv_batch on the copies
+    set_decode_weights made, which the decoder holds (the captured graphs bake in their pointers)."""
 
     def __init__(self, llm, slots: int = 8, max_tokens_per_slot: int = 2048, max_new: int = 1024,
                  total_pages: Optional[int] = None):
         cfg = llm.config
         self.llm, self.slots = llm, slots
+        self.decode_weights = getattr(llm, "decode_weights", "bf16")
+        # None unless in that mode.  Held here: the graphs bake in their pointers
+        self.fp8 = llm._fp8_weights if self.decode_weights == "fp8" else None
+        self.w4 = llm._w4_weights if self.decode_weights == "w4a16" else None
         dev, dt = llm.device, llm.dtype
         Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
         assert D == 128, "batched decode attention is specialised for head_dim 128"
@@ -176,7 +187,11 @@ class BatchedDecoder:
         self._ensure_pages(slot, S + 1)
         cache = _SlotCache(self.pool, self.page_tables[slot])
         hid = llm.prefill_hidden(inputs_embeds, cache)
-        logits = llm.logits_from_hidden(hid[-1:])
+        if self.decode_weights == "bf16":
+            logits = llm.logits_from_hidden(hid[-1:])
+        else:  # the mode's lm_head, as GraphDecoder.start
+            h = ops.rmsnorm(hid[-1:].contiguous(), llm.model.norm.weight, llm.config.rms_norm_eps)
+            logits = ops.gemv_batch(h, **self._weights(None))
         tok = torch.argmax(logits[0].float())
         self.tokens[slot] = tok
         self.hist[slot, 0] = tok
@@ -201,6 +216,17 @@ class BatchedDecoder:
             self.page_tables[slot, first:first + need] = torch.tensor(new, dtype=torch.int32,
                                                                       device=self.page_tables.device)
 
+    def _weights(self, li: Optional[int]):
+        """quantized modes: (qkv, o, gate/up, down) of layer li, or lm_head for li None, each a dict of
+        ops.gemv_batch's weight arguments"""
+        q = self.w4 if self.w4 is not None else self.fp8
+        if li is None:
+            return dict(w=q.lm_head[0], w_scale=q.lm_head[1])
+        f = q.layers[li]
+        if self.w4 is not None:
+            return tuple(dict(w=p, w_scale=s, w_zero=z) for p, s, z in (f.qkv, f.o, f.gu, f.down))
+        return tuple(dict(w=w, w_scale=s) for w, s in (f.qkv, f.o, f.gu, f.down))
+
     # ---- one decode step for every active slot ----------------------------------------------------
     def _step(self, num_splits: Optional[int]) -> None:
         llm, cfg = self.llm, self.llm.config
@@ -212,9 +238,14 @@ class BatchedDecoder:
             long = self.positions >= HEAD_KERNEL_TOKENS
             pos_head.copy_(self.positions).masked_fill_(long, -1)
             self.pos_split.copy_(self.positions).masked_fill_(~long, -1)
+        quant = self.decode_weights != "bf16"
         for li, layer in enumerate(llm.model.layers):
             h = ops.rmsnorm(x, layer.input_layernorm.weight, cfg.rms_norm_eps)
-            qkv = ops.linear(h, layer._qkv_w, layer._qkv_b, static_w=True)
+            if quant:
+                w_qkv, w_o, w_gu, w_down = self._weights(li)
+                qkv = ops.gemv_batch(h, bias=layer._qkv_b, static_w=True, **w_qkv)
+            else:
+                qkv = ops.linear(h, layer._qkv_w, layer._qkv_b, static_w=True)
             ops.decode_attention_batch(qkv, pos_head, self.pool[li, 0], self.pool[li, 1],
                                        self.page_tables, self.attn, llm.inv_freq, Hq, Hkv, D, D ** -0.5)
             if num_splits is not None:
@@ -222,12 +253,21 @@ class BatchedDecoder:
                                                  self.page_tables, self.attn, self.o_partial, self.lse,
                                                  self.counters, llm.inv_freq, Hq, Hkv, D, num_splits,
                                                  SPLIT_TOKENS, D ** -0.5)
-            ops.linear(self.attn, layer.self_attn.o_proj.weight, residual=x, out=x, static_w=True)
-            h = ops.rmsnorm(x, layer.post_attention_layernorm.weight, cfg.rms_norm_eps)
-            a = ops.linear(h, layer._gu_w, swiglu=True, static_w=True)
-            ops.linear(a, layer.mlp.down_proj.weight, residual=x, out=x, static_w=True)
+            if quant:
+                ops.gemv_batch(self.attn, residual=x, out=x, static_w=True, **w_o)
+                h = ops.rmsnorm(x, layer.post_attention_layernorm.weight, cfg.rms_norm_eps)
+                a = ops.gemv_batch(h, swiglu=True, static_w=True, **w_gu)
+                ops.gemv_batch(a, residual=x, out=x, static_w=True, **w_down)
+            else:
+                ops.linear(self.attn, layer.self_attn.o_proj.weight, residual=x, out=x, static_w=True)
+                h = ops.rmsnorm(x, layer.post_attention_layernorm.weight, cfg.rms_norm_eps)
+                a = ops.linear(h, layer._gu_w, swiglu=True, static_w=True)
+                ops.linear(a, layer.mlp.down_proj.weight, residual=x, out=x, static_w=True)
         h = ops.rmsnorm(x.clone(), llm.model.norm.weight, cfg.rms_norm_eps)
-        logits = ops.linear(h, llm.lm_head.weight, static_w=True)
+        if quant:
+            logits = ops.gemv_batch(h, static_w=True, **self._weights(None))
+        else:
+            logits = ops.linear(h, llm.lm_head.weight, static_w=True)
         active = self.positions >= 0
         tok = torch.argmax(logits.float(), dim=-1)
         self.tokens.copy_(torch.where(active, tok, self.tokens))
@@ -283,7 +323,13 @@ def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eo
     """Greedy-decode `prompts` (list of inputs_embeds [S_i, hidden]) with continuous batching: at most
     `slots` requests in flight; a finished request (EOS or max_new_tokens) frees its slot for the next
     one in the queue.  Returns the new ids per request (EOS included), in request order.
-    max_tokens_per_slot None: the slot and the pool are sized from the requests (slot_geometry)."""
+    max_tokens_per_slot None: the slot and the pool are sized from the requests (slot_geometry).
+    The decoder runs the LLM's current decode-weight mode; a passed-in `decoder` of another mode is a
+    ValueError."""
+    mode = getattr(llm, "decode_weights", "bf16")
+    if decoder is not None and getattr(decoder, "decode_weights", "bf16") != mode:
+        raise ValueError(f"decoder streams {getattr(decoder, 'decode_weights', 'bf16')!r} weights, the LLM is in "
+                         f"{mode!r} mode: build the decoder after set_decode_weights")
     if decoder is None:
         max_tokens_per_slot, pool_pages = slot_geometry([p.shape[0] for p in prompts], max_new_tokens,
                                                         check_every, slots, max_tokens_per_slot)
