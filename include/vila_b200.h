@@ -319,6 +319,48 @@ int vila_decode_attention_split_batch(const vila_decode_attn_split_params* p, in
                                       int out_stride, int pt_stride, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Opt-in FP8 KV cache of the batched engine.  Format: codes e4m3 [L, 2, P, 128, Hkv, 128] (the bf16 pool's
+ * layout with 1-byte elements, K after RoPE) and fp32 scales [L, 2, P, 128, Hkv], one per row of 128 values:
+ *   amax = max|x|, inv = 448 / amax (fp32), code = e4m3(rn, satfinite)(x * inv), scale = amax / 448;
+ *   amax == 0: codes and scale 0.  The dequantised value is float(code) * scale.
+ * Both entry points replace DynamicCache.update + flash-attn decode (in-tree copy
+ * llava/eval/vision_niah_vila/zigzag_ring_attn/modeling_qwen2.py:99-160,262-310) for this format.
+ * ------------------------------------------------------------------------------------------- */
+/* Rows [0, S) of every layer's K and V of a bf16 cache src [L, 2, src_tokens, Hkv, 128] (a prefill's staging
+ * cache with identity pages) -> dst codes [L, 2, dst_pages, 128, Hkv, 128] and dst_scale [L, 2, dst_pages, 128,
+ * Hkv], token t going to page page_table[t / 128] (pt_len entries, device int32).  One launch.  head_dim 128;
+ * src / dst 16-byte aligned. */
+int vila_kv_quantize_fp8(const void* src, int64_t src_tokens, void* dst, float* dst_scale, int64_t dst_pages,
+                         const int32_t* page_table, int pt_len, int L, int Hkv, int D, int S, void* stream);
+/* One decode step of `batch` sequences over one shared e4m3 pool (this layer's k_pool / v_pool [P, 128, Hkv, 128],
+ * k_scale / v_scale [P, 128, Hkv]).  Sequence b uses qkv + b*qkv_stride (bf16, pre-RoPE, not modified),
+ * out + b*out_stride, position[b] (< 0: idle, skipped) and the page-table row page_table + b*pt_stride.  Per
+ * sequence: RoPE of q and of the new k, the new k / v row quantised and appended at position[b], attention over
+ * [0, position[b]] on the dequantised rows (the new row as later steps will read it).  Grid (num_splits, Hkv,
+ * batch): split j covers tokens [j*split_tokens, (j+1)*split_tokens) (split_tokens a multiple of 128, <= 2048;
+ * num_splits * split_tokens and pt_stride * 128 must exceed every position), split CTAs past a sequence's length
+ * exit at once and the last CTA of a (sequence, KV head) combines the splits that hold tokens in index order.  A
+ * sequence's output and appended bytes depend on that sequence only (not on num_splits or the other rows).
+ * ws >= batch*Hkv*num_splits*G*(D+2) floats; counters batch*Hkv ints, zero before the first launch
+ * (self-cleaning).  head_dim 128, G = Hq / Hkv <= 16. */
+typedef struct vila_decode_attn_fp8_params {
+  const void* qkv;
+  const int32_t* position;
+  void* k_pool;
+  void* v_pool;
+  float* k_scale;
+  float* v_scale;
+  const int32_t* page_table;
+  void* out;
+  float* ws;
+  int32_t* counters;
+  const float* inv_freq;
+  int32_t Hq, Hkv, D, batch, qkv_stride, out_stride, pt_stride, num_splits, split_tokens;
+  float scale;
+} vila_decode_attn_fp8_params;
+int vila_decode_attention_fp8_batch(const vila_decode_attn_fp8_params* p, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * vila_decode_mega — n_tokens greedy decode steps of the whole LLM in ONE persistent launch
  * (one CTA per SM, weights streamed through per-warp TMA rings that run ahead across layer and token
  * boundaries, grid barriers between phases).  Replaces the per-token HF generate loop

@@ -64,6 +64,17 @@ class DecodeAttnSplitParams(C.Structure):
     ]
 
 
+class DecodeAttnFp8Params(C.Structure):
+    _fields_ = [
+        ("qkv", c_void_p), ("position", c_void_p), ("k_pool", c_void_p), ("v_pool", c_void_p),
+        ("k_scale", c_void_p), ("v_scale", c_void_p), ("page_table", c_void_p), ("out", c_void_p),
+        ("ws", c_void_p), ("counters", c_void_p), ("inv_freq", c_void_p),
+        ("Hq", C.c_int32), ("Hkv", C.c_int32), ("D", C.c_int32), ("batch", C.c_int32), ("qkv_stride", C.c_int32),
+        ("out_stride", C.c_int32), ("pt_stride", C.c_int32), ("num_splits", C.c_int32),
+        ("split_tokens", C.c_int32), ("scale", c_float),
+    ]
+
+
 class MegaParams(C.Structure):
     _fields_ = [
         ("layers", c_void_p), ("num_layers", C.c_int32),
@@ -120,6 +131,9 @@ SIGNATURES = {
     "vila_decode_attention_batch": [C.POINTER(DecodeAttnParams), c_int, c_int, c_int, c_int, c_int, c_void_p],
     "vila_decode_attention_split": [C.POINTER(DecodeAttnSplitParams), c_void_p],
     "vila_decode_attention_split_batch": [C.POINTER(DecodeAttnSplitParams), c_int, c_int, c_int, c_int, c_void_p],
+    "vila_kv_quantize_fp8": [c_void_p, c_i64, c_void_p, c_void_p, c_i64, c_void_p, c_int, c_int, c_int, c_int,
+                             c_int, c_void_p],
+    "vila_decode_attention_fp8_batch": [C.POINTER(DecodeAttnFp8Params), c_void_p],
     "vila_decode_mega": [C.POINTER(MegaParams), c_void_p],
 }
 _RESTYPES = {"vila_last_error": C.c_char_p}

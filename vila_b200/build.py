@@ -28,6 +28,7 @@ SOURCES = [
     "decode.cu",
     "gemv_tma.cu",
     "decode_mega.cu",
+    "kv_fp8.cu",
 ]
 HEADERS = ["common.cuh", "wgmma.cuh", "kernels.h", "../../include/vila_b200.h"]
 

@@ -377,6 +377,36 @@ int vila_decode_attention_split_batch(const vila_decode_attn_split_params* p, in
   return vb::decode_attention_split_batch(d, batch, qkv_stride, out_stride, pt_stride, st(stream));
 }
 
+// DynamicCache.update + flash-attn decode (modeling_qwen2.py:99-160,262-310) over an e4m3 KV pool
+int vila_kv_quantize_fp8(const void* src, int64_t src_tokens, void* dst, float* dst_scale, int64_t dst_pages,
+                         const int32_t* page_table, int pt_len, int L, int Hkv, int D, int S, void* stream) {
+  VB_REQUIRE_DEVICE();
+  return vb::kv_quantize_fp8(cb(src), src_tokens, static_cast<uint8_t*>(dst), dst_scale, dst_pages, page_table,
+                             pt_len, L, Hkv, D, S, st(stream));
+}
+
+int vila_decode_attention_fp8_batch(const vila_decode_attn_fp8_params* p, void* stream) {
+  VB_REQUIRE_DEVICE();
+  VB_CHECK(p != nullptr, "vila_decode_attention_fp8_batch: params are required");
+  vb::DecodeAttnFp8Params d;
+  d.qkv = cb(p->qkv);
+  d.position = p->position;
+  d.k_pool = static_cast<uint8_t*>(p->k_pool);
+  d.v_pool = static_cast<uint8_t*>(p->v_pool);
+  d.k_scale = p->k_scale;
+  d.v_scale = p->v_scale;
+  d.page_table = p->page_table;
+  d.out = mb(p->out);
+  d.ws = p->ws;
+  d.counters = p->counters;
+  d.inv_freq = p->inv_freq;
+  d.Hq = p->Hq; d.Hkv = p->Hkv; d.D = p->D; d.batch = p->batch;
+  d.qkv_stride = p->qkv_stride; d.out_stride = p->out_stride; d.pt_stride = p->pt_stride;
+  d.num_splits = p->num_splits; d.split_tokens = p->split_tokens;
+  d.scale = p->scale;
+  return vb::decode_attention_fp8_batch(d, st(stream));
+}
+
 int vila_decode_mega(const vila_mega_params* p, void* stream) {
   VB_REQUIRE_DEVICE();
   static_assert(sizeof(vila_mega_layer) == sizeof(vb::MegaLayer), "layer struct mismatch");

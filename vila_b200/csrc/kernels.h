@@ -212,6 +212,28 @@ int decode_attention_split(const DecodeAttnSplitParams& p, cudaStream_t stream);
 int decode_attention_split_batch(const DecodeAttnSplitParams& p, int batch, int qkv_stride, int out_stride,
                                  int pt_stride, cudaStream_t stream);
 
+// ---- opt-in e4m3 KV cache of the batched engine (kv_fp8.cu) -------------------------------------
+// rows [0, S) of every layer's K and V of a bf16 staging cache [L, 2, src_tokens, Hkv, 128] -> e4m3 codes
+// [L, 2, dst_pages, 128, Hkv, 128] and fp32 scales [L, 2, dst_pages, 128, Hkv] through one page-table row
+int kv_quantize_fp8(const __nv_bfloat16* src, int64_t src_tokens, uint8_t* dst, float* dst_scale, int64_t dst_pages,
+                    const int32_t* page_table, int pt_len, int L, int Hkv, int D, int S, cudaStream_t stream);
+struct DecodeAttnFp8Params {
+  const __nv_bfloat16* qkv;    // [batch, qkv_stride] pre-RoPE, current token (not modified)
+  const int32_t* position;     // [batch] position of the new token == tokens cached (< 0: idle slot)
+  uint8_t* k_pool;             // this layer's e4m3 K pages [P, 128, Hkv, 128]
+  uint8_t* v_pool;
+  float* k_scale;              // [P, 128, Hkv]
+  float* v_scale;
+  const int32_t* page_table;   // [batch, pt_stride]
+  __nv_bfloat16* out;          // [batch, out_stride]
+  float* ws;                   // >= batch * Hkv * num_splits * G * (D + 2) floats
+  int32_t* counters;           // [batch * Hkv], zero before the first launch (self-cleaning)
+  const float* inv_freq;       // [D/2]
+  int Hq, Hkv, D, batch, qkv_stride, out_stride, pt_stride, num_splits, split_tokens;
+  float scale;
+};
+int decode_attention_fp8_batch(const DecodeAttnFp8Params& p, cudaStream_t stream);
+
 // ---- persistent decode mega-kernel (decode_mega.cu) -------------------------------------------
 struct MegaLayer {  // device-resident array, one entry per decoder layer
   const __nv_bfloat16* qkv_w;   // [(Hq+2Hkv)*128, hidden]

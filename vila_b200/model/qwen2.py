@@ -148,6 +148,22 @@ def quantize_e4m3_rows(w: torch.Tensor, rows_per_chunk: int = 16384):
     return q, s
 
 
+def quantize_kv_e4m3(x: torch.Tensor):
+    """The FP8 KV cache's rule (kv_cache="fp8" of serving.BatchedDecoder; the kernels of csrc/kv_fp8.cu apply the
+    same one), one fp32 scale per row of the last dim:
+        amax = max|x|;  inv = 448 / amax (fp32);  code = (x.float() * inv).clamp(-448, 448) -> e4m3 (round to
+        nearest even);  scale = amax / 448;  a row with amax == 0 gets all-zero codes and scale 0.
+    The dequantised value is float(code) * scale.  -> (codes float8_e4m3fn, like x; scales fp32 x.shape[:-1])"""
+    xf = x.float()
+    amax = xf.abs().amax(dim=-1)
+    nz = amax > 0
+    lim = torch.full_like(amax, E4M3_MAX)  # tensor / tensor: IEEE division (a Python scalar would go through
+    inv = torch.where(nz, lim / amax, torch.zeros_like(amax))  # a rounded reciprocal)
+    codes = (xf * inv[..., None]).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn)
+    codes.view(torch.uint8).masked_fill_(~nz[..., None], 0)  # no negative zeros in an all-zero row
+    return codes, amax / lim
+
+
 W4_GROUP = 128  # consecutive k of one row sharing a scale and a zero point
 W4_TILE = 16    # rows per packed tile (the m of the kernel's mma.sync m16n8k16)
 

@@ -11,7 +11,8 @@ from typing import Optional, Sequence
 import torch
 
 from . import _lib
-from ._lib import DecodeAttnParams, DecodeAttnSplitParams, FmhaParams, GemvBatchParams, GemvParams, check
+from ._lib import (DecodeAttnFp8Params, DecodeAttnParams, DecodeAttnSplitParams, FmhaParams, GemvBatchParams,
+                   GemvParams, check)
 
 ACT_NONE, ACT_GELU_TANH, ACT_GELU_ERF, ACT_SILU = 0, 1, 2, 3
 
@@ -539,3 +540,84 @@ def decode_attention_split_batch(qkv: torch.Tensor, positions: torch.Tensor, k_p
     check(_lib.load().vila_decode_attention_split_batch(C.byref(p), B, qkv.stride(0), out.stride(0),
                                                         page_tables.stride(0), _stream()),
           "vila_decode_attention_split_batch")
+
+
+def _need(cond: bool, msg: str) -> None:
+    if not cond:
+        raise ValueError(msg)
+
+
+def kv_quantize_fp8(src: torch.Tensor, dst: torch.Tensor, dst_scale: torch.Tensor, page_row: torch.Tensor,
+                    S: int) -> None:
+    """Rows [0, S) of every layer's K and V of a bf16 cache src [L, 2, pages, 128, Hkv, 128] (identity pages: a
+    prefill's staging cache) -> the e4m3 pool dst [L, 2, P, 128, Hkv, 128] and its fp32 scales dst_scale
+    [L, 2, P, 128, Hkv], token t going to page page_row[t // 128] (vila_kv_quantize_fp8, one launch).  The rule is
+    quantize_kv_e4m3's (vila_b200/model/qwen2.py)."""
+    _need(src.dim() == 6 and src.shape[1] == 2 and src.shape[3] == 128 and src.shape[5] == 128 and src.is_contiguous(),
+          f"kv_quantize_fp8: src must be a contiguous [L, 2, pages, 128, Hkv, 128] cache, got {tuple(src.shape)}")
+    L, _, ps, _, Hkv, D = src.shape
+    _need(dst.dim() == 6 and dst.shape[:2] == (L, 2) and dst.shape[3:] == (128, Hkv, D) and dst.is_contiguous(),
+          f"kv_quantize_fp8: dst must be a contiguous [{L}, 2, P, 128, {Hkv}, {D}] pool, got {tuple(dst.shape)}")
+    _need(dst_scale.shape == dst.shape[:5] and dst_scale.is_contiguous(),
+          f"kv_quantize_fp8: dst_scale must be a contiguous {tuple(dst.shape[:5])} tensor, got {tuple(dst_scale.shape)}")
+    _need(page_row.dim() == 1 and page_row.is_contiguous(), "kv_quantize_fp8: page_row must be a contiguous 1-D row")
+    _need(0 <= S <= ps * 128 and (S + 127) // 128 <= page_row.numel(),
+          f"kv_quantize_fp8: S={S} exceeds the source ({ps * 128} tokens) or the page row ({page_row.numel()} pages)")
+    for t, name, dt in ((src, "src", torch.bfloat16), (dst, "dst", torch.float8_e4m3fn),
+                        (dst_scale, "dst_scale", torch.float32), (page_row, "page_row", torch.int32)):
+        _need(t.dtype == dt, f"kv_quantize_fp8: {name} must be {dt}, got {t.dtype}")
+    for t, name in ((src, "src"), (dst, "dst"), (dst_scale, "dst_scale"), (page_row, "page_row")):
+        _chk(t, name, t.dtype)
+    check(_lib.load().vila_kv_quantize_fp8(_p(src), ps * 128, _p(dst), _p(dst_scale), dst.shape[2], _p(page_row),
+                                           page_row.numel(), L, Hkv, D, S, _stream()), "vila_kv_quantize_fp8")
+
+
+def decode_attention_fp8_batch(qkv: torch.Tensor, positions: torch.Tensor, k_pool: torch.Tensor,
+                               v_pool: torch.Tensor, k_scale: torch.Tensor, v_scale: torch.Tensor,
+                               page_tables: torch.Tensor, out: torch.Tensor, ws: torch.Tensor, counters: torch.Tensor,
+                               inv_freq: torch.Tensor, Hq: int, Hkv: int, num_splits: int, split_tokens: int,
+                               scale: float) -> None:
+    """One decode step of B sequences over one shared e4m3 pool (vila_decode_attention_fp8_batch): qkv
+    [B, (Hq+2Hkv)*128] bf16 pre-RoPE (not modified), positions int32 [B] (< 0: idle slot), k_pool / v_pool e4m3
+    [P, 128, Hkv, 128] with k_scale / v_scale fp32 [P, 128, Hkv], page_tables int32 [B, pages], out [B, Hq*128].
+    RoPE, e4m3 append of the new row at positions[b], attention over [0, positions[b]]; split j covers tokens
+    [j*split_tokens, (j+1)*split_tokens) and num_splits * split_tokens must exceed every position.  Work buffers:
+    ws fp32 >= B*Hq*num_splits*130, counters int32 [B*Hkv] (zeroed once, self-cleaning)."""
+    D = 128
+    _need(Hq >= 1 and Hkv >= 1 and Hq % Hkv == 0 and Hq // Hkv <= 16,
+          f"decode_attention_fp8_batch: Hq / Hkv must be an integer <= 16 (Hq={Hq}, Hkv={Hkv})")
+    _need(qkv.dim() == 2 and qkv.shape[1] == (Hq + 2 * Hkv) * D and qkv.stride(1) == 1,
+          f"decode_attention_fp8_batch: qkv must be [B, {(Hq + 2 * Hkv) * D}] with unit column stride "
+          f"(head_dim 128), got {tuple(qkv.shape)}")
+    B = qkv.shape[0]
+    _need(out.shape == (B, Hq * D) and out.stride(1) == 1,
+          f"decode_attention_fp8_batch: out must be [{B}, {Hq * D}], got {tuple(out.shape)}")
+    _need(positions.numel() == B and positions.is_contiguous(), f"decode_attention_fp8_batch: positions must be [{B}]")
+    _need(page_tables.dim() == 2 and page_tables.shape[0] == B and page_tables.stride(1) == 1,
+          f"decode_attention_fp8_batch: page_tables must be [{B}, pages], got {tuple(page_tables.shape)}")
+    for pool, sc, name in ((k_pool, k_scale, "k"), (v_pool, v_scale, "v")):
+        _need(pool.dim() == 4 and pool.shape[1:] == (128, Hkv, D) and pool.is_contiguous(),
+              f"decode_attention_fp8_batch: {name}_pool must be a contiguous [P, 128, {Hkv}, 128] pool, "
+              f"got {tuple(pool.shape)}")
+        _need(sc.shape == pool.shape[:3] and sc.is_contiguous(),
+              f"decode_attention_fp8_batch: {name}_scale must be a contiguous {tuple(pool.shape[:3])} tensor")
+    _need(split_tokens >= 128 and split_tokens % 128 == 0 and split_tokens <= 2048 and num_splits >= 1,
+          f"decode_attention_fp8_batch: bad split configuration ({num_splits} x {split_tokens})")
+    _need(ws.numel() >= B * Hq * num_splits * (D + 2) and counters.numel() >= B * Hkv,
+          "decode_attention_fp8_batch: ws needs B*Hq*num_splits*130 floats and counters B*Hkv ints")
+    for t, name, dt in ((qkv, "qkv", torch.bfloat16), (out, "out", torch.bfloat16), (positions, "positions", torch.int32),
+                        (page_tables, "page_tables", torch.int32), (k_pool, "k_pool", torch.float8_e4m3fn),
+                        (v_pool, "v_pool", torch.float8_e4m3fn), (k_scale, "k_scale", torch.float32),
+                        (v_scale, "v_scale", torch.float32), (ws, "ws", torch.float32),
+                        (counters, "counters", torch.int32), (inv_freq, "inv_freq", torch.float32)):
+        _need(t.dtype == dt, f"decode_attention_fp8_batch: {name} must be {dt}, got {t.dtype}")
+    for t in (qkv, out, positions, page_tables, k_pool, v_pool, k_scale, v_scale, ws, counters, inv_freq):
+        _chk(t, "every tensor", t.dtype)
+    p = DecodeAttnFp8Params()
+    p.qkv, p.position, p.k_pool, p.v_pool = _p(qkv), _p(positions), _p(k_pool), _p(v_pool)
+    p.k_scale, p.v_scale, p.page_table, p.out = _p(k_scale), _p(v_scale), _p(page_tables), _p(out)
+    p.ws, p.counters, p.inv_freq = _p(ws), _p(counters), _p(inv_freq)
+    p.Hq, p.Hkv, p.D, p.batch = Hq, Hkv, D, B
+    p.qkv_stride, p.out_stride, p.pt_stride = qkv.stride(0), out.stride(0), page_tables.stride(0)
+    p.num_splits, p.split_tokens, p.scale = num_splits, split_tokens, scale
+    check(_lib.load().vila_decode_attention_fp8_batch(C.byref(p), _stream()), "vila_decode_attention_fp8_batch")

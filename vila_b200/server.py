@@ -140,8 +140,9 @@ class Engine:
     """One model, one asyncio lock (the GPU is a single queue): streaming requests hold the lock while
     their generator runs; non-streaming requests waiting for it are batched together."""
 
-    def __init__(self, model, model_name: str, slots: int = 8):
+    def __init__(self, model, model_name: str, slots: int = 8, kv_cache: str = "bf16"):
         self.model, self.model_name, self.slots = model, model_name, slots
+        self.kv_cache = kv_cache
         self.lock = asyncio.Lock()
         self.pending: List[Any] = []
 
@@ -180,8 +181,10 @@ class Engine:
         if len(reqs) == 1 or not hasattr(m, "generate_batch"):
             return [m.generate_content(build_prompt(r.messages), generation_config=self._gen_config(r)) for r in reqs]
         prepared = [m._prepare_content(build_prompt(r.messages)) for r in reqs]
+        # the default is not passed: a model whose generate_batch predates the kv_cache argument keeps working
+        kw = {} if self.kv_cache == "bf16" else {"kv_cache": self.kv_cache}
         ids = m.generate_batch([{"input_ids": i, "media": md, "media_config": mc} for i, md, mc in prepared],
-                               max_new_tokens=max(r.max_tokens or 512 for r in reqs), slots=self.slots)
+                               max_new_tokens=max(r.max_tokens or 512 for r in reqs), slots=self.slots, **kw)
         outs = []
         for r, g in zip(reqs, ids):
             outs.append(m.tokenizer.decode(g[:r.max_tokens or 512], skip_special_tokens=True).strip())
@@ -203,11 +206,11 @@ class Engine:
             yield "data: [DONE]\n\n"
 
 
-def create_app(model, model_name: str, slots: int = 8):
+def create_app(model, model_name: str, slots: int = 8, kv_cache: str = "bf16"):
     from fastapi import FastAPI
     from fastapi.responses import JSONResponse, StreamingResponse
     app = FastAPI()
-    engine = Engine(model, model_name, slots)
+    engine = Engine(model, model_name, slots, kv_cache)
     app.state.engine = engine
 
     @app.get("/")
@@ -240,10 +243,13 @@ def main() -> None:
                     help="weights of the single-stream greedy decoder (fp8: e4m3 with per-row scales; w4a16: "
                          "4-bit with group-128 scales and zero points, lm_head e4m3), and of the engine that "
                          "batches queued requests; the prefill stays bf16)")
+    ap.add_argument("--kv-cache", choices=("bf16", "fp8"), default="bf16",
+                    help="K/V format of the engine that batches queued requests (fp8: e4m3 with one fp32 scale "
+                         "per token and KV head, about half the bytes; the single-stream decoder stays bf16)")
     args = ap.parse_args()
     model = llava.load(args.model_path, decode_weights=args.decode_weights)
-    uvicorn.run(create_app(model, get_model_name_from_path(args.model_path), args.slots), host=args.host,
-                port=args.port)
+    uvicorn.run(create_app(model, get_model_name_from_path(args.model_path), args.slots, args.kv_cache),
+                host=args.host, port=args.port)
 
 
 if __name__ == "__main__":

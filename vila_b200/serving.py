@@ -21,7 +21,11 @@ tokens per byte by B.  Here:
   * finished slots (EOS / budget) are harvested and refilled between graph replays;
   * in the LLM's "fp8" / "w4a16" decode-weight modes (Qwen2ForCausalLM.set_decode_weights) the step's
     GEMMs run `vila_gemv_batch_*` on the quantized copies (up to 16 slots per launch, every weight byte
-    read once per launch) and each slot's first token comes from the e4m3 lm_head; the prefill stays bf16.
+    read once per launch) and each slot's first token comes from the e4m3 lm_head; the prefill stays bf16;
+  * with kv_cache="fp8" the pool holds e4m3 codes plus one fp32 scale per (token, KV head) row
+    (quantize_kv_e4m3): a prompt is prefilled into a bf16 staging cache of one slot and converted into the
+    slot's pages by vila_kv_quantize_fp8, and every slot, whatever its length, is attended by
+    vila_decode_attention_fp8_batch (RoPE, e4m3 append and split-KV attention in one launch per layer).
 """
 from __future__ import annotations
 
@@ -47,6 +51,22 @@ HEAD_KERNEL_TOKENS = 16 * PAGE
 SPLIT_TOKENS = 1024
 SPLIT_LADDER = (8, 16, 32, 68)
 MAX_SLOT_TOKENS = SPLIT_LADDER[-1] * SPLIT_TOKENS  # 69,632: a 256-frame LongVILA request + 1K new tokens
+
+KV_CACHE_FORMATS = ("bf16", "fp8")
+# FP8 KV: split j covers tokens [j*FP8_SPLIT_TOKENS, (j+1)*FP8_SPLIT_TOKENS) for every slot length, so a slot's
+# result does not depend on the ladder entry; the ladder (tokens covered) sizes the splits launched from the
+# longest active slot.  DESIGN.md §4 has the measurements behind the split size.
+FP8_SPLIT_TOKENS = 512
+FP8_LADDER_TOKENS = (2048, 8192, 16384, 32768, MAX_SLOT_TOKENS)
+
+
+def fp8_attention_config(longest: int) -> int:
+    """splits launched by an fp8-KV decode step whose longest active slot holds `longest` tokens: those of the
+    smallest ladder entry covering it"""
+    for n in FP8_LADDER_TOKENS:
+        if n >= longest:
+            return (n + FP8_SPLIT_TOKENS - 1) // FP8_SPLIT_TOKENS
+    raise ValueError(f"a slot of {longest} tokens exceeds the engine's limit ({MAX_SLOT_TOKENS})")
 
 
 def attention_config(longest: int) -> Optional[int]:
@@ -125,10 +145,17 @@ class BatchedDecoder:
 
     The decoder streams the weights of the LLM's decode-weight mode at construction (`decode_weights`):
     "bf16" runs the wgmma GEMMs on the parameters; "fp8" and "w4a16" run ops.gemv_batch on the copies
-    set_decode_weights made, which the decoder holds (the captured graphs bake in their pointers)."""
+    set_decode_weights made, which the decoder holds (the captured graphs bake in their pointers).
+
+    kv_cache "bf16" (default) keeps bf16 K/V in `pool`; "fp8" keeps e4m3 codes in `pool` and one fp32 scale per
+    (layer, K|V, token, KV head) row in `pool_scale` (0.516x the bytes for head_dim 128), plus a bf16 staging
+    cache of one slot (`staging`) that admit() prefills into."""
 
     def __init__(self, llm, slots: int = 8, max_tokens_per_slot: int = 2048, max_new: int = 1024,
-                 total_pages: Optional[int] = None):
+                 total_pages: Optional[int] = None, kv_cache: str = "bf16"):
+        if kv_cache not in KV_CACHE_FORMATS:
+            raise ValueError(f"kv_cache must be one of {KV_CACHE_FORMATS}, got {kv_cache!r}")
+        self.kv_cache = kv_cache
         cfg = llm.config
         self.llm, self.slots = llm, slots
         self.decode_weights = getattr(llm, "decode_weights", "bf16")
@@ -142,7 +169,10 @@ class BatchedDecoder:
         assert self.pages_per_slot * PAGE <= MAX_SLOT_TOKENS, \
             f"slots of up to {MAX_SLOT_TOKENS} tokens (asked for {max_tokens_per_slot})"
         P = total_pages if total_pages is not None else slots * self.pages_per_slot
-        self.pool = torch.zeros(cfg.num_hidden_layers, 2, P, PAGE, Hkv, D, device=dev, dtype=dt)
+        L = cfg.num_hidden_layers
+        fp8 = kv_cache == "fp8"
+        self.pool = torch.zeros(L, 2, P, PAGE, Hkv, D, device=dev, dtype=torch.float8_e4m3fn if fp8 else dt)
+        self.pool_scale = torch.zeros(L, 2, P, PAGE, Hkv, device=dev, dtype=torch.float32) if fp8 else None
         self.allocator = PageAllocator(P)
         self.slot_pages: List[List[int]] = [[] for _ in range(slots)]
         # unassigned entries point at page 0; they are never dereferenced (tokens beyond a slot's length)
@@ -161,7 +191,17 @@ class BatchedDecoder:
             if self.pages_per_slot * PAGE > (SPLIT_LADDER[i - 1] * SPLIT_TOKENS if i else HEAD_KERNEL_TOKENS)]
         self.graphs: Dict[Optional[int], torch.cuda.CUDAGraph] = {}  # configuration -> step graph
         self.config: Optional[int] = None  # configuration of the last run()
-        if len(self.configs) > 1:
+        if fp8:
+            # one slot of bf16 K/V with an identity page table: the prefill (and its FMHA over earlier chunks)
+            # runs unchanged on it; configurations are split counts of the fp8 attention kernel
+            self.staging = torch.zeros(L, 2, self.pages_per_slot, PAGE, Hkv, D, device=dev, dtype=dt)
+            self.staging_pages = torch.arange(self.pages_per_slot, dtype=torch.int32, device=dev)
+            tokens = self.pages_per_slot * PAGE
+            self.configs = [fp8_attention_config(n) for i, n in enumerate(FP8_LADDER_TOKENS)
+                            if i == 0 or tokens > FP8_LADDER_TOKENS[i - 1]]
+            self.ws = torch.zeros(slots * Hq * self.configs[-1] * (D + 2), device=dev, dtype=torch.float32)
+            self.counters = torch.zeros(slots * Hkv, device=dev, dtype=torch.int32)
+        elif len(self.configs) > 1:
             n_max = self.configs[-1]
             # per-step copies of `positions` that hide the long slots from the head kernel and the short
             # ones from the split-KV kernel, and the split-KV work buffers (shared by all layers)
@@ -173,9 +213,11 @@ class BatchedDecoder:
 
     @property
     def launches_per_step(self) -> int:
-        """library kernels of one step in the configuration of the last run(): 7 per layer (9 with the
-        split-KV kernel: RoPE/append and attention added) + final RMSNorm and lm_head"""
-        return (7 if self.config is None else 9) * self.llm.config.num_hidden_layers + 2
+        """library kernels of one step in the configuration of the last run(): 7 per layer (9 with the bf16
+        split-KV kernel: RoPE/append and attention added; always 7 with the fp8 KV cache) + final RMSNorm and
+        lm_head"""
+        per_layer = 7 if self.config is None or self.kv_cache == "fp8" else 9
+        return per_layer * self.llm.config.num_hidden_layers + 2
 
     # ---- admission ------------------------------------------------------------------------------
     @torch.inference_mode()
@@ -185,8 +227,11 @@ class BatchedDecoder:
         S = inputs_embeds.shape[0]
         assert S + 1 <= self.pages_per_slot * PAGE, "prompt longer than a slot"
         self._ensure_pages(slot, S + 1)
-        cache = _SlotCache(self.pool, self.page_tables[slot])
-        hid = llm.prefill_hidden(inputs_embeds, cache)
+        if self.kv_cache == "fp8":  # prefill in bf16, then one conversion into the slot's e4m3 pages
+            hid = llm.prefill_hidden(inputs_embeds, _SlotCache(self.staging, self.staging_pages))
+            ops.kv_quantize_fp8(self.staging, self.pool, self.pool_scale, self.page_tables[slot], S)
+        else:
+            hid = llm.prefill_hidden(inputs_embeds, _SlotCache(self.pool, self.page_tables[slot]))
         if self.decode_weights == "bf16":
             logits = llm.logits_from_hidden(hid[-1:])
         else:  # the mode's lm_head, as GraphDecoder.start
@@ -233,7 +278,8 @@ class BatchedDecoder:
         Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
         x = self.x
         pos_head = self.positions
-        if num_splits is not None:  # slot length pos + 1 picks the kernel (idle slots stay -1 in both)
+        fp8_kv = self.kv_cache == "fp8"
+        if num_splits is not None and not fp8_kv:  # slot length pos + 1 picks the kernel (idle slots stay -1 in both)
             pos_head = self.pos_head
             long = self.positions >= HEAD_KERNEL_TOKENS
             pos_head.copy_(self.positions).masked_fill_(long, -1)
@@ -246,9 +292,15 @@ class BatchedDecoder:
                 qkv = ops.gemv_batch(h, bias=layer._qkv_b, static_w=True, **w_qkv)
             else:
                 qkv = ops.linear(h, layer._qkv_w, layer._qkv_b, static_w=True)
-            ops.decode_attention_batch(qkv, pos_head, self.pool[li, 0], self.pool[li, 1],
-                                       self.page_tables, self.attn, llm.inv_freq, Hq, Hkv, D, D ** -0.5)
-            if num_splits is not None:
+            if fp8_kv:
+                ops.decode_attention_fp8_batch(qkv, self.positions, self.pool[li, 0], self.pool[li, 1],
+                                               self.pool_scale[li, 0], self.pool_scale[li, 1], self.page_tables,
+                                               self.attn, self.ws, self.counters, llm.inv_freq, Hq, Hkv,
+                                               num_splits, FP8_SPLIT_TOKENS, D ** -0.5)
+            else:
+                ops.decode_attention_batch(qkv, pos_head, self.pool[li, 0], self.pool[li, 1],
+                                           self.page_tables, self.attn, llm.inv_freq, Hq, Hkv, D, D ** -0.5)
+            if num_splits is not None and not fp8_kv:
                 ops.decode_attention_split_batch(qkv, self.pos_split, self.pool[li, 0], self.pool[li, 1],
                                                  self.page_tables, self.attn, self.o_partial, self.lse,
                                                  self.counters, llm.inv_freq, Hq, Hkv, D, num_splits,
@@ -287,7 +339,8 @@ class BatchedDecoder:
                 self._ensure_pages(s_, self._pos_host[s_] + n_tokens + 1)
                 self._pos_host[s_] += n_tokens
                 longest = max(longest, self._pos_host[s_])  # tokens attended by the slot's last step
-        self.config = attention_config(min(longest, self.pages_per_slot * PAGE))
+        longest = min(longest, self.pages_per_slot * PAGE)
+        self.config = fp8_attention_config(longest) if self.kv_cache == "fp8" else attention_config(longest)
         g = self.graphs[self.config]
         for _ in range(n_tokens):
             g.replay()
@@ -319,22 +372,29 @@ class BatchedDecoder:
 @torch.inference_mode()
 def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eos_token_ids: Sequence[int] = (),
                    slots: int = 8, max_tokens_per_slot: Optional[int] = None, check_every: int = 8,
-                   decoder: Optional[BatchedDecoder] = None, total_pages: Optional[int] = None) -> List[List[int]]:
+                   decoder: Optional[BatchedDecoder] = None, total_pages: Optional[int] = None,
+                   kv_cache: str = "bf16") -> List[List[int]]:
     """Greedy-decode `prompts` (list of inputs_embeds [S_i, hidden]) with continuous batching: at most
     `slots` requests in flight; a finished request (EOS or max_new_tokens) frees its slot for the next
     one in the queue.  Returns the new ids per request (EOS included), in request order.
     max_tokens_per_slot None: the slot and the pool are sized from the requests (slot_geometry).
     The decoder runs the LLM's current decode-weight mode; a passed-in `decoder` of another mode is a
+    ValueError.  kv_cache: "bf16" or "fp8" (BatchedDecoder); a passed-in `decoder` of the other KV format is a
     ValueError."""
     mode = getattr(llm, "decode_weights", "bf16")
     if decoder is not None and getattr(decoder, "decode_weights", "bf16") != mode:
         raise ValueError(f"decoder streams {getattr(decoder, 'decode_weights', 'bf16')!r} weights, the LLM is in "
                          f"{mode!r} mode: build the decoder after set_decode_weights")
+    if kv_cache not in KV_CACHE_FORMATS:
+        raise ValueError(f"kv_cache must be one of {KV_CACHE_FORMATS}, got {kv_cache!r}")
+    if decoder is not None and getattr(decoder, "kv_cache", "bf16") != kv_cache:
+        raise ValueError(f"decoder keeps a {getattr(decoder, 'kv_cache', 'bf16')!r} KV cache, {kv_cache!r} was asked for")
     if decoder is None:
         max_tokens_per_slot, pool_pages = slot_geometry([p.shape[0] for p in prompts], max_new_tokens,
                                                         check_every, slots, max_tokens_per_slot)
         decoder = BatchedDecoder(llm, slots, max_tokens_per_slot, max_new=max_new_tokens,
-                                 total_pages=total_pages if total_pages is not None else pool_pages)
+                                 total_pages=total_pages if total_pages is not None else pool_pages,
+                                 kv_cache=kv_cache)
     dec = decoder
     dec.capture()
     cap = dec.pages_per_slot * PAGE
