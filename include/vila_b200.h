@@ -361,6 +361,39 @@ typedef struct vila_decode_attn_fp8_params {
 int vila_decode_attention_fp8_batch(const vila_decode_attn_fp8_params* p, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * vila_sample_batch — the next token of M rows of bf16 logits [M, V] (row stride ld), each with its own
+ * temperature, top-k, top-p, 64-bit seed and token index, drawn on the device.  Replaces HF
+ * TemperatureLogitsWarper / TopKLogitsWarper / TopPLogitsWarper + torch.multinomial in GenerationMixin._sample,
+ * reached from llava_arch.py:823-833.  The rule (vila_b200/sampling.py states it in torch / numpy):
+ *   greedy   inv_temperature == 0 or top_k == 1: the first index of max float(logit) (torch.argmax)
+ *   scaling  s_i = float(logit_i) * inv_temperature (fp32)
+ *   top-k    0 < top_k < V: keep s_i >= the k-th largest s (ties kept)
+ *   top-p    top_p < 1: p_i = exp(s_i - max s), Z = sum of p over the top-k survivors; keep survivor i iff the mass
+ *            of survivors with a strictly larger s is < top_p * Z (the kernel sums floor(p_i * 2^40) in integers)
+ *   draw     argmax over the kept set of s_i + g_i, ties to the lowest index; g_i = -log(-log1p(-u_i)),
+ *            u_i = (x_i + 0.5) * 2^-32, x_i word i % 4 of Philox-4x32-10, key (seed lo, seed hi), counter
+ *            (i / 4, step lo, step hi, 0)
+ * A row with position < 0 is idle: tokens[row] (and n_kept[row]) are left untouched.  n_kept (may be NULL) gets
+ * the size of each row's kept set (1 for greedy rows).  A row's token depends only on its logits, parameters, seed
+ * and step: not on M, on the row index or on the other rows.  Deterministic bits; no float atomics.
+ * 1 <= V <= 327,680, M <= 65535.  One cluster of 8 CTAs per row.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct vila_sample_params {
+  const void* logits;
+  int64_t ld;
+  const float* inv_temperature;
+  const int32_t* top_k;
+  const float* top_p;
+  const int64_t* seed;
+  const int64_t* step;
+  const int32_t* position;
+  int64_t* tokens;
+  int32_t* n_kept;
+  int32_t M, V;
+} vila_sample_params;
+int vila_sample_batch(const vila_sample_params* p, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * vila_decode_mega — n_tokens greedy decode steps of the whole LLM in ONE persistent launch
  * (one CTA per SM, weights streamed through per-warp TMA rings that run ahead across layer and token
  * boundaries, grid barriers between phases).  Replaces the per-token HF generate loop

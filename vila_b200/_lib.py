@@ -75,6 +75,14 @@ class DecodeAttnFp8Params(C.Structure):
     ]
 
 
+class SampleParams(C.Structure):
+    _fields_ = [
+        ("logits", c_void_p), ("ld", c_i64), ("inv_temperature", c_void_p), ("top_k", c_void_p),
+        ("top_p", c_void_p), ("seed", c_void_p), ("step", c_void_p), ("position", c_void_p),
+        ("tokens", c_void_p), ("n_kept", c_void_p), ("M", C.c_int32), ("V", C.c_int32),
+    ]
+
+
 class MegaParams(C.Structure):
     _fields_ = [
         ("layers", c_void_p), ("num_layers", C.c_int32),
@@ -134,6 +142,7 @@ SIGNATURES = {
     "vila_kv_quantize_fp8": [c_void_p, c_i64, c_void_p, c_void_p, c_i64, c_void_p, c_int, c_int, c_int, c_int,
                              c_int, c_void_p],
     "vila_decode_attention_fp8_batch": [C.POINTER(DecodeAttnFp8Params), c_void_p],
+    "vila_sample_batch": [C.POINTER(SampleParams), c_void_p],
     "vila_decode_mega": [C.POINTER(MegaParams), c_void_p],
 }
 _RESTYPES = {"vila_last_error": C.c_char_p}

@@ -29,6 +29,7 @@ SOURCES = [
     "gemv_tma.cu",
     "decode_mega.cu",
     "kv_fp8.cu",
+    "sample.cu",
 ]
 HEADERS = ["common.cuh", "wgmma.cuh", "kernels.h", "../../include/vila_b200.h"]
 

@@ -407,6 +407,25 @@ int vila_decode_attention_fp8_batch(const vila_decode_attn_fp8_params* p, void* 
   return vb::decode_attention_fp8_batch(d, st(stream));
 }
 
+// HF Temperature / TopK / TopP LogitsWarper + torch.multinomial (GenerationMixin._sample)
+int vila_sample_batch(const vila_sample_params* p, void* stream) {
+  VB_REQUIRE_DEVICE();
+  VB_CHECK(p != nullptr, "vila_sample_batch: params are required");
+  vb::SampleParams d;
+  d.logits = cb(p->logits);
+  d.ld = p->ld;
+  d.inv_temperature = p->inv_temperature;
+  d.top_k = p->top_k;
+  d.top_p = p->top_p;
+  d.seed = p->seed;
+  d.step = p->step;
+  d.position = p->position;
+  d.tokens = p->tokens;
+  d.n_kept = p->n_kept;
+  d.M = p->M; d.V = p->V;
+  return vb::sample_batch(d, st(stream));
+}
+
 int vila_decode_mega(const vila_mega_params* p, void* stream) {
   VB_REQUIRE_DEVICE();
   static_assert(sizeof(vila_mega_layer) == sizeof(vb::MegaLayer), "layer struct mismatch");

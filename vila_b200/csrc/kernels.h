@@ -234,6 +234,22 @@ struct DecodeAttnFp8Params {
 };
 int decode_attention_fp8_batch(const DecodeAttnFp8Params& p, cudaStream_t stream);
 
+// ---- temperature / top-k / top-p sampling of the batched engine (sample.cu) ----------------------
+struct SampleParams {
+  const __nv_bfloat16* logits;   // [M, ld]
+  int64_t ld;                    // row stride (elements), >= V
+  const float* inv_temperature;  // [M] 1/T (0: greedy)
+  const int32_t* top_k;          // [M] 0 or >= V: off
+  const float* top_p;            // [M] 1: off
+  const int64_t* seed;           // [M]
+  const int64_t* step;           // [M] index t of the token being drawn
+  const int32_t* position;       // [M] < 0: idle row, tokens[row] untouched
+  int64_t* tokens;               // [M] out
+  int32_t* n_kept;               // [M] out (size of the kept set) or null
+  int M, V;
+};
+int sample_batch(const SampleParams& p, cudaStream_t stream);
+
 // ---- persistent decode mega-kernel (decode_mega.cu) -------------------------------------------
 struct MegaLayer {  // device-resident array, one entry per decoder layer
   const __nv_bfloat16* qkv_w;   // [(Hq+2Hkv)*128, hidden]

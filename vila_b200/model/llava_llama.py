@@ -585,14 +585,15 @@ class LlavaLlamaModel(nn.Module):
     @torch.inference_mode()
     def generate_batch(self, requests: List[Dict[str, Any]], max_new_tokens: int = 128, slots: int = 8,
                        max_tokens_per_slot: Optional[int] = None, eos_token_id=None,
-                       kv_cache: str = "bf16") -> List[List[int]]:
+                       kv_cache: str = "bf16", sampling=None) -> List[List[int]]:
         """Serve several independent requests with continuous batching over one shared paged KV pool
         (vila_b200/serving.py; the reference's servers run them one at a time, serving/server.py:65-73).
         requests: dicts with the `generate` arguments (`input_ids` [1, T], `media`, `media_config`).
         max_tokens_per_slot None: sized from the requests (serving.slot_geometry: 2048 tokens unless a
         request needs more, e.g. video or dynamic-S2 prompts).
         kv_cache: "bf16" (default) or "fp8" (e4m3 K/V with one fp32 scale per token and KV head, serving.py).
-        Greedy decoding; returns the new ids of every request in order."""
+        sampling: None (default) decodes greedily; a serving.SamplingParams, or a list with one per request,
+        samples on the device (serving.generate_batch).  Returns the new ids of every request in order."""
         from ..serving import generate_batch
         prompts = []
         for r in requests:
@@ -602,7 +603,7 @@ class LlavaLlamaModel(nn.Module):
         eos = self.tokenizer.stop_token_ids if eos_token_id is None else (
             [eos_token_id] if isinstance(eos_token_id, int) else list(eos_token_id))
         return generate_batch(self.llm, prompts, max_new_tokens, eos, slots=slots,
-                              max_tokens_per_slot=max_tokens_per_slot, kv_cache=kv_cache)
+                              max_tokens_per_slot=max_tokens_per_slot, kv_cache=kv_cache, sampling=sampling)
 
     @property
     def default_generation_config(self):

@@ -12,7 +12,7 @@ import torch
 
 from . import _lib
 from ._lib import (DecodeAttnFp8Params, DecodeAttnParams, DecodeAttnSplitParams, FmhaParams, GemvBatchParams,
-                   GemvParams, check)
+                   GemvParams, SampleParams, check)
 
 ACT_NONE, ACT_GELU_TANH, ACT_GELU_ERF, ACT_SILU = 0, 1, 2, 3
 
@@ -621,3 +621,42 @@ def decode_attention_fp8_batch(qkv: torch.Tensor, positions: torch.Tensor, k_poo
     p.qkv_stride, p.out_stride, p.pt_stride = qkv.stride(0), out.stride(0), page_tables.stride(0)
     p.num_splits, p.split_tokens, p.scale = num_splits, split_tokens, scale
     check(_lib.load().vila_decode_attention_fp8_batch(C.byref(p), _stream()), "vila_decode_attention_fp8_batch")
+
+
+SAMPLE_MAX_VOCAB = 8 * 40960  # one cluster of 8 CTAs per row, each holding at most 40,960 fp32 scores
+
+
+def sample_batch(logits: torch.Tensor, inv_temperature: torch.Tensor, top_k: torch.Tensor, top_p: torch.Tensor,
+                 seed: torch.Tensor, step: torch.Tensor, positions: torch.Tensor, *, out: torch.Tensor,
+                 n_kept: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The next token of each row of logits [M, V] bf16 (unit column stride, any row stride), drawn on the device by
+    the rule of vila_b200/sampling.py (vila_sample_batch, one launch).  Per row: inv_temperature fp32 (0: greedy),
+    top_k int32 (0: off), top_p fp32 (1: off), seed int64, step int64 (index t of the token), positions int32 (< 0:
+    idle row, out untouched); out int64 [M]; n_kept int32 [M] or None gets the size of each row's kept set.  The
+    parameter values live on the device and are validated where they are set (SamplingParams); the kernel reads
+    inv_temperature <= 0 as greedy and top_k < 0 or >= V as off."""
+    _need(logits.dim() == 2 and logits.stride(1) == 1 and logits.stride(0) >= logits.shape[1],
+          f"sample_batch: logits must be [M, V] with unit column stride, got {tuple(logits.shape)} strides "
+          f"{tuple(logits.stride())}")
+    M, V = logits.shape
+    _need(1 <= M <= 65535 and 1 <= V <= SAMPLE_MAX_VOCAB,
+          f"sample_batch: M={M} must be in 1..65535 and V={V} in 1..{SAMPLE_MAX_VOCAB}")
+    arrays = [(logits, "logits", torch.bfloat16), (inv_temperature, "inv_temperature", torch.float32),
+              (top_k, "top_k", torch.int32), (top_p, "top_p", torch.float32), (seed, "seed", torch.int64),
+              (step, "step", torch.int64), (positions, "positions", torch.int32), (out, "out", torch.int64)]
+    if n_kept is not None:
+        arrays.append((n_kept, "n_kept", torch.int32))
+    for t, name, dt in arrays:
+        _need(t.dtype == dt, f"sample_batch: {name} must be {dt}, got {t.dtype}")
+        if t is not logits:
+            _need(t.dim() == 1 and t.numel() == M and t.is_contiguous(),
+                  f"sample_batch: {name} must be a contiguous [{M}] vector, got {tuple(t.shape)}")
+    for t, name, _ in arrays:
+        _chk(t, name, t.dtype)
+    p = SampleParams()
+    p.logits, p.ld = _p(logits), logits.stride(0)
+    p.inv_temperature, p.top_k, p.top_p = _p(inv_temperature), _p(top_k), _p(top_p)
+    p.seed, p.step, p.position, p.tokens, p.n_kept = _p(seed), _p(step), _p(positions), _p(out), _p(n_kept)
+    p.M, p.V = M, V
+    check(_lib.load().vila_sample_batch(C.byref(p), _stream()), "vila_sample_batch")
+    return out

@@ -5,7 +5,9 @@ Mirrors the request / response shapes of the reference's `serving/server.py` (`C
 `stream` is set, one `chat.completion` object otherwise) on top of `generate_content(prompt, stream=...)`.
 The reference serialises requests with a global lock; here non-streaming requests that arrive while the
 engine is busy are grouped (up to `slots`) and decoded together by `LlavaLlamaModel.generate_batch`
-(continuous batching over the shared paged pool, vila_b200/serving.py).
+(continuous batching over the shared paged pool, vila_b200/serving.py).  With --sample every non-streaming
+request goes through generate_batch with its own temperature, top_p and seed, drawn on the device; streaming
+requests stay on the single-stream greedy decoder.
 
     python -m vila_b200.server --model-path <dir> --port 8000
 """
@@ -62,6 +64,7 @@ class ChatCompletionRequest(BaseModel):
     use_cache: Optional[bool] = True
     num_beams: Optional[int] = 1
     client: Optional[dict] = None
+    seed: Optional[int] = None
 
 
 def load_image(url: str):
@@ -140,9 +143,12 @@ class Engine:
     """One model, one asyncio lock (the GPU is a single queue): streaming requests hold the lock while
     their generator runs; non-streaming requests waiting for it are batched together."""
 
-    def __init__(self, model, model_name: str, slots: int = 8, kv_cache: str = "bf16"):
+    def __init__(self, model, model_name: str, slots: int = 8, kv_cache: str = "bf16", sample: bool = False):
         self.model, self.model_name, self.slots = model, model_name, slots
         self.kv_cache = kv_cache
+        if sample and not hasattr(model, "generate_batch"):
+            raise ValueError("sample=True needs a model with generate_batch (the batched engine draws the tokens)")
+        self.sample = sample  # non-streaming requests: sampled on the batched engine with their own parameters
         self.lock = asyncio.Lock()
         self.pending: List[Any] = []
 
@@ -155,20 +161,23 @@ class Engine:
         if req.model != self.model_name:
             raise ValueError(f"The endpoint is configured to use the model {self.model_name}, "
                              f"but the request model is {req.model}")
+        # checked before the request joins a batch: a bad value fails this request only
+        params = self._sampling(req) if self.sample else None
         loop = asyncio.get_running_loop()
         fut = loop.create_future()
-        self.pending.append((req, fut))
+        self.pending.append((req, fut, params))
         async with self.lock:
             if not fut.done():  # this task drains the queue for everyone that piled up behind the lock
                 batch, self.pending = self.pending[:self.slots], self.pending[self.slots:]
                 try:
-                    texts = await loop.run_in_executor(None, self._run_batch, [r for r, _ in batch])
+                    texts = await loop.run_in_executor(None, self._run_batch, [r for r, _, _ in batch],
+                                                       [p for _, _, p in batch] if self.sample else None)
                 except Exception as e:  # every request of the failed batch gets the error, none is left waiting
-                    for _, f in batch:
+                    for _, f, _ in batch:
                         if not f.done():
                             f.set_exception(e)
                 else:
-                    for (_, f), t in zip(batch, texts):
+                    for (_, f, _), t in zip(batch, texts):
                         if not f.done():
                             f.set_result(t)
         text = await fut
@@ -176,19 +185,29 @@ class Engine:
                 "model": req.model, "index": 0,
                 "choices": [{"message": {"role": "assistant", "content": text}}]}
 
-    def _run_batch(self, reqs: List[ChatCompletionRequest]) -> List[str]:
+    def _run_batch(self, reqs: List[ChatCompletionRequest], sampling: Optional[list] = None) -> List[str]:
+        """sampling: one SamplingParams per request (Engine(sample=True)), or None for greedy decoding"""
         m = self.model
-        if len(reqs) == 1 or not hasattr(m, "generate_batch"):
+        if sampling is None and (len(reqs) == 1 or not hasattr(m, "generate_batch")):
             return [m.generate_content(build_prompt(r.messages), generation_config=self._gen_config(r)) for r in reqs]
         prepared = [m._prepare_content(build_prompt(r.messages)) for r in reqs]
         # the default is not passed: a model whose generate_batch predates the kv_cache argument keeps working
         kw = {} if self.kv_cache == "bf16" else {"kv_cache": self.kv_cache}
+        if sampling is not None:
+            kw["sampling"] = sampling
         ids = m.generate_batch([{"input_ids": i, "media": md, "media_config": mc} for i, md, mc in prepared],
                                max_new_tokens=max(r.max_tokens or 512 for r in reqs), slots=self.slots, **kw)
         outs = []
         for r, g in zip(reqs, ids):
             outs.append(m.tokenizer.decode(g[:r.max_tokens or 512], skip_special_tokens=True).strip())
         return outs
+
+    @staticmethod
+    def _sampling(req: ChatCompletionRequest):
+        """a request's SamplingParams: temperature None or 0 is greedy, top_p None is off; bad values raise"""
+        from .sampling import SamplingParams
+        return SamplingParams(temperature=float(req.temperature or 0.0),
+                              top_p=float(req.top_p) if req.top_p is not None else 1.0, seed=req.seed)
 
     async def stream(self, req: ChatCompletionRequest):
         if req.model != self.model_name:
@@ -206,11 +225,11 @@ class Engine:
             yield "data: [DONE]\n\n"
 
 
-def create_app(model, model_name: str, slots: int = 8, kv_cache: str = "bf16"):
+def create_app(model, model_name: str, slots: int = 8, kv_cache: str = "bf16", sample: bool = False):
     from fastapi import FastAPI
     from fastapi.responses import JSONResponse, StreamingResponse
     app = FastAPI()
-    engine = Engine(model, model_name, slots, kv_cache)
+    engine = Engine(model, model_name, slots, kv_cache, sample)
     app.state.engine = engine
 
     @app.get("/")
@@ -246,9 +265,14 @@ def main() -> None:
     ap.add_argument("--kv-cache", choices=("bf16", "fp8"), default="bf16",
                     help="K/V format of the engine that batches queued requests (fp8: e4m3 with one fp32 scale "
                          "per token and KV head, about half the bytes; the single-stream decoder stays bf16)")
+    ap.add_argument("--sample", action="store_true",
+                    help="sample non-streaming requests with their own temperature, top_p and seed on the batched "
+                         "engine (vila_sample_batch, on the device), even a request that arrives alone; without it "
+                         "every request is decoded greedily.  Streaming requests stay on the single-stream greedy "
+                         "decoder either way")
     args = ap.parse_args()
     model = llava.load(args.model_path, decode_weights=args.decode_weights)
-    uvicorn.run(create_app(model, get_model_name_from_path(args.model_path), args.slots, args.kv_cache),
+    uvicorn.run(create_app(model, get_model_name_from_path(args.model_path), args.slots, args.kv_cache, args.sample),
                 host=args.host, port=args.port)
 
 

@@ -25,16 +25,20 @@ tokens per byte by B.  Here:
   * with kv_cache="fp8" the pool holds e4m3 codes plus one fp32 scale per (token, KV head) row
     (quantize_kv_e4m3): a prompt is prefilled into a bf16 staging cache of one slot and converted into the
     slot's pages by vila_kv_quantize_fp8, and every slot, whatever its length, is attended by
-    vila_decode_attention_fp8_batch (RoPE, e4m3 append and split-KV attention in one launch per layer).
+    vila_decode_attention_fp8_batch (RoPE, e4m3 append and split-KV attention in one launch per layer);
+  * with sampling=True each slot has its own temperature / top-k / top-p / seed (SamplingParams, the rule in
+    vila_b200/sampling.py) in device arrays, and vila_sample_batch replaces the greedy arg-max, in the step graphs
+    and for the first token at admission; a slot's draw depends only on its own logits, seed and token index.
 """
 from __future__ import annotations
 
 from collections import deque
-from typing import Deque, Dict, List, Optional, Sequence, Tuple
+from typing import Deque, Dict, List, Optional, Sequence, Tuple, Union
 
 import torch
 
 from . import ops
+from .sampling import SamplingParams, signed64
 
 PAGE = 128
 
@@ -149,10 +153,14 @@ class BatchedDecoder:
 
     kv_cache "bf16" (default) keeps bf16 K/V in `pool`; "fp8" keeps e4m3 codes in `pool` and one fp32 scale per
     (layer, K|V, token, KV head) row in `pool_scale` (0.516x the bytes for head_dim 128), plus a bf16 staging
-    cache of one slot (`staging`) that admit() prefills into."""
+    cache of one slot (`staging`) that admit() prefills into.
+
+    sampling False (default) picks every token greedily with torch.argmax.  True keeps per-slot device arrays of
+    the sampling parameters (admit() writes them) and draws every token with vila_sample_batch, at token index
+    `step_idx` of the slot; a slot admitted without parameters decodes greedily (temperature 0)."""
 
     def __init__(self, llm, slots: int = 8, max_tokens_per_slot: int = 2048, max_new: int = 1024,
-                 total_pages: Optional[int] = None, kv_cache: str = "bf16"):
+                 total_pages: Optional[int] = None, kv_cache: str = "bf16", sampling: bool = False):
         if kv_cache not in KV_CACHE_FORMATS:
             raise ValueError(f"kv_cache must be one of {KV_CACHE_FORMATS}, got {kv_cache!r}")
         self.kv_cache = kv_cache
@@ -185,6 +193,14 @@ class BatchedDecoder:
         self.max_new = max_new
         self.hist = torch.zeros(slots, max_new + 8, dtype=torch.int64, device=dev)
         self.step_idx = torch.zeros(slots, 1, dtype=torch.int64, device=dev)  # per-slot write column
+        self.sampling = bool(sampling)
+        if self.sampling:  # per-slot parameters of vila_sample_batch (admit() writes them)
+            self.inv_temperature = torch.zeros(slots, dtype=torch.float32, device=dev)
+            self.top_k = torch.zeros(slots, dtype=torch.int32, device=dev)
+            self.top_p = torch.ones(slots, dtype=torch.float32, device=dev)
+            self.seed = torch.zeros(slots, dtype=torch.int64, device=dev)
+            self._zero_pos = torch.zeros(1, dtype=torch.int32, device=dev)    # admission: row active, t = 0
+            self._zero_step = torch.zeros(1, dtype=torch.int64, device=dev)
         # attention configurations this slot size can need (attention_config): None, then ladder entries
         self.configs: List[Optional[int]] = [None] + [
             n for i, n in enumerate(SPLIT_LADDER)
@@ -215,15 +231,22 @@ class BatchedDecoder:
     def launches_per_step(self) -> int:
         """library kernels of one step in the configuration of the last run(): 7 per layer (9 with the bf16
         split-KV kernel: RoPE/append and attention added; always 7 with the fp8 KV cache) + final RMSNorm and
-        lm_head"""
+        lm_head (+ vila_sample_batch with sampling)"""
         per_layer = 7 if self.config is None or self.kv_cache == "fp8" else 9
-        return per_layer * self.llm.config.num_hidden_layers + 2
+        return per_layer * self.llm.config.num_hidden_layers + 2 + (1 if self.sampling else 0)
 
     # ---- admission ------------------------------------------------------------------------------
     @torch.inference_mode()
-    def admit(self, slot: int, inputs_embeds: torch.Tensor) -> None:
-        """Prefill `inputs_embeds` [S, hidden] into the slot's pages and seed its decode state."""
+    def admit(self, slot: int, inputs_embeds: torch.Tensor, params: Optional[SamplingParams] = None) -> None:
+        """Prefill `inputs_embeds` [S, hidden] into the slot's pages and seed its decode state.  params: the slot's
+        SamplingParams (sampling decoders only; None is greedy); its seed must be set."""
         llm = self.llm
+        if params is not None and not self.sampling:
+            raise ValueError("admit(params=...) needs a decoder built with sampling=True")
+        if self.sampling:
+            params = params if params is not None else SamplingParams()
+            if params.seed is None and not params.greedy:
+                raise ValueError("admit: a sampled slot needs a seed (generate_batch draws one)")
         S = inputs_embeds.shape[0]
         assert S + 1 <= self.pages_per_slot * PAGE, "prompt longer than a slot"
         self._ensure_pages(slot, S + 1)
@@ -237,11 +260,23 @@ class BatchedDecoder:
         else:  # the mode's lm_head, as GraphDecoder.start
             h = ops.rmsnorm(hid[-1:].contiguous(), llm.model.norm.weight, llm.config.rms_norm_eps)
             logits = ops.gemv_batch(h, **self._weights(None))
-        tok = torch.argmax(logits[0].float())
-        self.tokens[slot] = tok
-        self.hist[slot, 0] = tok
-        self.step_idx[slot, 0] = 1
-        self.x[slot] = llm.model.embed_tokens.weight[tok]
+        if self.sampling:  # token 0 by the same kernel: M = 1, t = 0
+            self.inv_temperature[slot] = params.inv_temperature
+            self.top_k[slot] = params.top_k
+            self.top_p[slot] = params.top_p
+            self.seed[slot] = signed64(params.seed or 0)
+            i = slice(slot, slot + 1)
+            ops.sample_batch(logits[:1], self.inv_temperature[i], self.top_k[i], self.top_p[i], self.seed[i],
+                             self._zero_step, self._zero_pos, out=self.tokens[i])
+            self.hist[slot, 0] = self.tokens[slot]
+            self.step_idx[slot, 0] = 1
+            self.x[i] = llm.model.embed_tokens.weight.index_select(0, self.tokens[i])
+        else:
+            tok = torch.argmax(logits[0].float())
+            self.tokens[slot] = tok
+            self.hist[slot, 0] = tok
+            self.step_idx[slot, 0] = 1
+            self.x[slot] = llm.model.embed_tokens.weight[tok]
         self.positions[slot] = S  # position of the token just chosen == tokens cached so far
         self._pos_host[slot] = S
 
@@ -321,8 +356,12 @@ class BatchedDecoder:
         else:
             logits = ops.linear(h, llm.lm_head.weight, static_w=True)
         active = self.positions >= 0
-        tok = torch.argmax(logits.float(), dim=-1)
-        self.tokens.copy_(torch.where(active, tok, self.tokens))
+        if self.sampling:  # idle slots (position < 0) keep their token
+            ops.sample_batch(logits, self.inv_temperature, self.top_k, self.top_p, self.seed, self.step_idx.view(-1),
+                             self.positions, out=self.tokens)
+        else:
+            tok = torch.argmax(logits.float(), dim=-1)
+            self.tokens.copy_(torch.where(active, tok, self.tokens))
         col = self.step_idx.clamp(max=self.hist.shape[1] - 1)
         self.hist.scatter_(1, col, self.tokens[:, None])
         self.step_idx.add_(active[:, None].to(torch.int64))
@@ -369,18 +408,44 @@ class BatchedDecoder:
         return self.hist[slot, :n].tolist()
 
 
+def sampling_for_requests(sampling: Union[None, SamplingParams, Sequence[SamplingParams]],
+                          n: int) -> Optional[List[SamplingParams]]:
+    """generate_batch's `sampling` -> one SamplingParams per request with every seed set (None stays None).  Missing
+    seeds are drawn from the host torch default generator in request order."""
+    if sampling is None:
+        return None
+    per = [sampling] * n if isinstance(sampling, SamplingParams) else list(sampling)
+    if len(per) != n or not all(isinstance(p, SamplingParams) for p in per):
+        raise ValueError(f"sampling must be a SamplingParams or a list of {n} of them (one per request)")
+    out = []
+    for p in per:
+        if p.seed is None:
+            seed = int(torch.randint(-2 ** 63, 2 ** 63 - 1, (1,), dtype=torch.int64))
+            p = SamplingParams(p.temperature, p.top_k, p.top_p, seed)
+        out.append(p)
+    return out
+
+
 @torch.inference_mode()
 def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eos_token_ids: Sequence[int] = (),
                    slots: int = 8, max_tokens_per_slot: Optional[int] = None, check_every: int = 8,
                    decoder: Optional[BatchedDecoder] = None, total_pages: Optional[int] = None,
-                   kv_cache: str = "bf16") -> List[List[int]]:
-    """Greedy-decode `prompts` (list of inputs_embeds [S_i, hidden]) with continuous batching: at most
+                   kv_cache: str = "bf16",
+                   sampling: Union[None, SamplingParams, Sequence[SamplingParams]] = None) -> List[List[int]]:
+    """Decode `prompts` (list of inputs_embeds [S_i, hidden]) with continuous batching: at most
     `slots` requests in flight; a finished request (EOS or max_new_tokens) frees its slot for the next
     one in the queue.  Returns the new ids per request (EOS included), in request order.
     max_tokens_per_slot None: the slot and the pool are sized from the requests (slot_geometry).
     The decoder runs the LLM's current decode-weight mode; a passed-in `decoder` of another mode is a
     ValueError.  kv_cache: "bf16" or "fp8" (BatchedDecoder); a passed-in `decoder` of the other KV format is a
-    ValueError."""
+    ValueError.
+    sampling None: greedy (the decoder's torch arg-max).  Otherwise one SamplingParams for every request or a list
+    with one per request, drawn on the device (BatchedDecoder(sampling=True)); a seed of None is drawn from the host
+    torch default generator in request order, so torch.manual_seed reproduces a run.  A passed-in greedy decoder
+    with sampling requested is a ValueError; a sampling decoder serves greedy requests as temperature-0 rows."""
+    params = sampling_for_requests(sampling, len(prompts))
+    if params is not None and decoder is not None and not getattr(decoder, "sampling", False):
+        raise ValueError("sampling was requested but the decoder was built with sampling=False")
     mode = getattr(llm, "decode_weights", "bf16")
     if decoder is not None and getattr(decoder, "decode_weights", "bf16") != mode:
         raise ValueError(f"decoder streams {getattr(decoder, 'decode_weights', 'bf16')!r} weights, the LLM is in "
@@ -394,7 +459,7 @@ def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eo
                                                         check_every, slots, max_tokens_per_slot)
         decoder = BatchedDecoder(llm, slots, max_tokens_per_slot, max_new=max_new_tokens,
                                  total_pages=total_pages if total_pages is not None else pool_pages,
-                                 kv_cache=kv_cache)
+                                 kv_cache=kv_cache, sampling=params is not None)
     dec = decoder
     dec.capture()
     cap = dec.pages_per_slot * PAGE
@@ -420,7 +485,10 @@ def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eo
                 if need > dec.allocator.available and owner:
                     break  # wait for a running request to finish and return its pages
                 r = queue.popleft()
-                dec.admit(s, prompts[r])
+                if params is None:
+                    dec.admit(s, prompts[r])
+                else:
+                    dec.admit(s, prompts[r], params[r])
                 owner[s] = r
         dec.run(check_every)
         for s in list(owner):
