@@ -45,7 +45,7 @@ extern "C" {
 #define VILA_FLAG_STATIC_W 2
 
 const char* vila_last_error(void);
-int vila_abi_version(void); /* 2 */
+int vila_abi_version(void); /* 3 */
 /* Register caller-owned, ZERO-INITIALISED device scratch (256-byte aligned) used by vila_linear's
  * stream-K schedule for fp32 partial sums (64 KiB of counters + M*N*4 bytes per call that uses it;
  * calls that do not fit simply use the data-parallel schedule).  The kernels leave it zeroed again.
@@ -392,52 +392,6 @@ typedef struct vila_sample_params {
   int32_t M, V;
 } vila_sample_params;
 int vila_sample_batch(const vila_sample_params* p, void* stream);
-
-/* ---------------------------------------------------------------------------------------------
- * vila_decode_mega — n_tokens greedy decode steps of the whole LLM in ONE persistent launch
- * (one CTA per SM, weights streamed through per-warp TMA rings that run ahead across layer and token
- * boundaries, grid barriers between phases).  Replaces the per-token HF generate loop
- * (llava_arch.py:833 -> GenerationMixin: ~400 launches and one D2H sync per token).
- * `layers` is a DEVICE array of num_layers entries.  `barrier` and `epoch` are device u32 words that
- * must both be zero before the first launch (the kernel keeps them consistent afterwards).
- * Head dim is 128.  The new tokens are appended to hist[*step ...], *position and *step advance.
- * ------------------------------------------------------------------------------------------- */
-typedef struct vila_mega_layer {
-  const void* qkv_w;
-  const void* qkv_b;
-  const void* o_w;
-  const void* gu_w;
-  const void* down_w;
-  const void* ln1_w;
-  const void* ln2_w;
-  void* k_pool;
-  void* v_pool;
-} vila_mega_layer;
-typedef struct vila_mega_params {
-  const vila_mega_layer* layers;
-  int32_t num_layers;
-  const void* final_norm_w;
-  const void* lm_head_w;
-  const void* embed;
-  int32_t hidden, inter, Hq, Hkv, vocab;
-  float eps, scale;
-  const float* inv_freq;
-  const int32_t* page_table;
-  void* x;
-  void* qkv;
-  void* act;
-  float* attn_ws;
-  int32_t* attn_counters; /* Hkv ints, zero before the first launch */
-  unsigned long long* key;
-  int32_t* token;
-  int32_t* hist;
-  int32_t* step;
-  int32_t* position;
-  uint32_t* barrier;
-  uint32_t* epoch;
-  int32_t n_tokens, splits;
-} vila_mega_params;
-int vila_decode_mega(const vila_mega_params* p, void* stream);
 
 #ifdef __cplusplus
 }

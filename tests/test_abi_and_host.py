@@ -26,7 +26,7 @@ def test_library_exports_every_declared_symbol():
     # and every ctypes signature corresponds to a declared function
     for n in _lib.SIGNATURES:
         assert n in names, f"{n} bound in _lib.py but not declared in the header"
-    assert lib.vila_abi_version() == 2
+    assert lib.vila_abi_version() == 3
 
 
 def test_struct_layouts_match_header_field_order():
@@ -34,8 +34,7 @@ def test_struct_layouts_match_header_field_order():
     text = (ROOT / "include" / "vila_b200.h").read_text()
     for cname, cls in (("vila_fmha_params", _lib.FmhaParams), ("vila_gemv_params", _lib.GemvParams),
                        ("vila_decode_attn_params", _lib.DecodeAttnParams),
-                       ("vila_decode_attn_split_params", _lib.DecodeAttnSplitParams),
-                       ("vila_mega_params", _lib.MegaParams)):
+                       ("vila_decode_attn_split_params", _lib.DecodeAttnSplitParams)):
         body = re.search(r"typedef struct %s \{(.*?)\} %s;" % (cname, cname), text, flags=re.S).group(1)
         body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
         fields = []

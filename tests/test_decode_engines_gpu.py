@@ -1,7 +1,7 @@
-"""GPU: the three decode engines step by step against the fp32 oracle, at NVILA's head shapes and on every
+"""GPU: the two decode engines step by step against the fp32 oracle, at NVILA's head shapes and on every
 decode attention path; and the batched decode attention entry point against fp32 attention.
 
-Engines (GraphDecoder, MegaDecoder, serving.BatchedDecoder) are checked by teacher forcing: the engine
+Engines (GraphDecoder, serving.BatchedDecoder) are checked by teacher forcing: the engine
 decodes greedily, then the oracle is fed the engine's OWN ids, so every step stays comparable whatever
 the near-ties.  At every decoded position:
   * the id is a greedy choice of the fp32 oracle, up to 3 bf16 ulps at the logit scale;
@@ -145,7 +145,6 @@ def _check_untouched(before, after, decoded):
 #   head   decode_attn_head_kernel, one sequence             (GraphDecoder, S + n <= 512)
 #   simt   SIMT split-KV kernel, one 8-CTA cluster / KV head  (GraphDecoder, S + n <= 1024)
 #   split  wgmma split-KV + separate combine, pick_splits     (GraphDecoder, longer)
-#   mega   the persistent kernel, 8 splits                    (MegaDecoder)
 #   batch  BatchedDecoder, see _run_batched
 _CONTEXTS = [(250, 24), (760, 24), (3060, 24), (16370, 16)]
 _PATHS = ["head", "simt", "split", "split"]
@@ -156,7 +155,6 @@ def _cases():
     for kind in ("tiny", "8b-shallow", "lite-shallow"):
         n_ctx = 4 if kind == "tiny" else 3  # video length on the tiny model only
         out += [(kind, "graph", path, S, n) for (S, n), path in zip(_CONTEXTS[:n_ctx], _PATHS)]
-        out += [(kind, "mega", "mega", S, n) for S, n in _CONTEXTS[:n_ctx]]
         if kind != "lite-shallow":
             out.append((kind, "batched", "batch", None, 16))
     return out
@@ -177,15 +175,14 @@ def test_engine_teacher_forced(cuda, kind, engine, path, S, n):
 
 
 def _run_single(kind, engine, path, S, n):
-    """GraphDecoder / MegaDecoder: cache_for -> prefill_hidden -> snapshot -> start -> run"""
-    from vila_b200.model import GraphDecoder, MegaDecoder
+    """GraphDecoder: cache_for -> prefill_hidden -> snapshot -> start -> run"""
+    from vila_b200.model import GraphDecoder
     model, o32, o16 = _model(kind)
     llm = model.llm
     emb = _prompt(llm, S, seed=S)
-    dec = (MegaDecoder if engine == "mega" else GraphDecoder)(llm, 128)
+    dec = GraphDecoder(llm, 128)
     cache = dec.cache_for(S + n)
-    got_path = ("mega" if engine == "mega" else "split" if dec.split_tokens
-                else "simt" if dec.num_splits else "head")
+    got_path = "split" if dec.split_tokens else "simt" if dec.num_splits else "head"
     assert got_path == path, f"{engine} at {S + n} tokens runs {got_path}, the case is for {path}"
     hid = llm.prefill_hidden(emb, cache)
     before = cache.pool.clone()

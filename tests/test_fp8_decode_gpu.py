@@ -6,7 +6,7 @@
     the fp32 oracle with the bf16 weights; the first id and every decoded position use an oracle whose LLM
     linear weights and lm_head are the dequantized q * s (embedding and norms unchanged);
   * bf16 decoding, the bf16 weights and state_dict() are unchanged by a round trip through fp8 mode;
-  * the public greedy paths follow the mode, and the persistent mega-kernel refuses it.
+  * the public greedy paths follow the mode.
 """
 import math
 
@@ -298,7 +298,7 @@ def test_bf16_unchanged_by_fp8_mode(cuda, kind):
     assert len(ids_q) == 24
 
 
-def test_public_paths_fp8(cuda, monkeypatch):
+def test_public_paths_fp8(cuda):
     model = _model("tiny")[0]
     llm = model.llm
     emb = _prompt(llm, 200, seed=11)
@@ -310,10 +310,5 @@ def test_public_paths_fp8(cuda, monkeypatch):
             via_stream = [t for chunk in llm.stream_greedy(emb, max_new_tokens=20, chunk_tokens=8) for t in chunk]
             direct, _ = _decode(llm, emb, 20)
         assert via_generate == via_stream == direct
-        monkeypatch.setenv("VILA_B200_DECODER", "mega")
-        with pytest.raises(NotImplementedError):
-            llm.decoder(16)
-        with pytest.raises(NotImplementedError):
-            llm.generate(inputs_embeds=emb[None], max_new_tokens=4, eos_token_id=None)
     finally:
         llm.set_decode_weights("bf16")

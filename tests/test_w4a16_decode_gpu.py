@@ -6,7 +6,7 @@
   * GraphDecoder in w4a16 mode, teacher-forced as tests/test_fp8_decode_gpu.py does: the oracle's layer
     weights are the dequantized 4-bit copies and its lm_head the dequantized e4m3 copy;
   * a bf16 -> w4a16 -> fp8 -> bf16 round trip leaves bf16 decoding, the pool and state_dict() unchanged;
-  * the public greedy paths follow the mode, and the persistent mega-kernel refuses it.
+  * the public greedy paths follow the mode.
 """
 import ctypes as C
 import math
@@ -286,7 +286,7 @@ def test_bf16_unchanged_by_w4a16_and_fp8_modes(cuda, kind):
     assert len(ids_w4) == 24 and len(ids_fp8) == 24
 
 
-def test_public_paths_w4a16(cuda, monkeypatch):
+def test_public_paths_w4a16(cuda):
     model = _model("tiny")[0]
     llm = model.llm
     emb = _prompt(llm, 200, seed=11)
@@ -298,10 +298,5 @@ def test_public_paths_w4a16(cuda, monkeypatch):
             via_stream = [t for chunk in llm.stream_greedy(emb, max_new_tokens=20, chunk_tokens=8) for t in chunk]
             direct, _ = _decode(llm, emb, 20)
         assert via_generate == via_stream == direct
-        monkeypatch.setenv("VILA_B200_DECODER", "mega")
-        with pytest.raises(NotImplementedError):
-            llm.decoder(16)
-        with pytest.raises(NotImplementedError):
-            llm.generate(inputs_embeds=emb[None], max_new_tokens=4, eos_token_id=None)
     finally:
         llm.set_decode_weights("bf16")

@@ -83,20 +83,6 @@ class SampleParams(C.Structure):
     ]
 
 
-class MegaParams(C.Structure):
-    _fields_ = [
-        ("layers", c_void_p), ("num_layers", C.c_int32),
-        ("final_norm_w", c_void_p), ("lm_head_w", c_void_p), ("embed", c_void_p),
-        ("hidden", C.c_int32), ("inter", C.c_int32), ("Hq", C.c_int32), ("Hkv", C.c_int32),
-        ("vocab", C.c_int32), ("eps", c_float), ("scale", c_float),
-        ("inv_freq", c_void_p), ("page_table", c_void_p),
-        ("x", c_void_p), ("qkv", c_void_p), ("act", c_void_p), ("attn_ws", c_void_p), ("attn_counters", c_void_p),
-        ("key", c_void_p), ("token", c_void_p), ("hist", c_void_p), ("step", c_void_p),
-        ("position", c_void_p), ("barrier", c_void_p), ("epoch", c_void_p),
-        ("n_tokens", C.c_int32), ("splits", C.c_int32),
-    ]
-
-
 # name -> argtypes; every function returns int (0 == ok) unless listed in _RESTYPES
 SIGNATURES = {
     "vila_abi_version": [],
@@ -143,7 +129,6 @@ SIGNATURES = {
                              c_int, c_void_p],
     "vila_decode_attention_fp8_batch": [C.POINTER(DecodeAttnFp8Params), c_void_p],
     "vila_sample_batch": [C.POINTER(SampleParams), c_void_p],
-    "vila_decode_mega": [C.POINTER(MegaParams), c_void_p],
 }
 _RESTYPES = {"vila_last_error": C.c_char_p}
 

@@ -27,7 +27,6 @@ SOURCES = [
     "data_movement.cu",
     "decode.cu",
     "gemv_tma.cu",
-    "decode_mega.cu",
     "kv_fp8.cu",
     "sample.cu",
 ]

@@ -42,7 +42,7 @@ static int require_sm90() {
 extern "C" {
 
 const char* vila_last_error(void) { return vb::last_error(); }
-int vila_abi_version(void) { return 2; }
+int vila_abi_version(void) { return 3; }
 
 int vila_set_workspace(void* ptr, uint64_t bytes) { return vb::set_workspace(ptr, (size_t)bytes); }
 
@@ -424,29 +424,6 @@ int vila_sample_batch(const vila_sample_params* p, void* stream) {
   d.n_kept = p->n_kept;
   d.M = p->M; d.V = p->V;
   return vb::sample_batch(d, st(stream));
-}
-
-int vila_decode_mega(const vila_mega_params* p, void* stream) {
-  VB_REQUIRE_DEVICE();
-  static_assert(sizeof(vila_mega_layer) == sizeof(vb::MegaLayer), "layer struct mismatch");
-  vb::MegaParams m;
-  m.layers = reinterpret_cast<const vb::MegaLayer*>(p->layers);
-  m.num_layers = p->num_layers;
-  m.final_norm_w = cb(p->final_norm_w);
-  m.lm_head_w = cb(p->lm_head_w);
-  m.embed = cb(p->embed);
-  m.hidden = p->hidden; m.inter = p->inter; m.Hq = p->Hq; m.Hkv = p->Hkv; m.vocab = p->vocab;
-  m.eps = p->eps; m.scale = p->scale;
-  m.inv_freq = p->inv_freq;
-  m.page_table = p->page_table;
-  m.x = mb(p->x); m.qkv = mb(p->qkv); m.act = mb(p->act);
-  m.attn_ws = p->attn_ws;
-  m.attn_counters = p->attn_counters;
-  m.key = p->key; m.token = p->token; m.hist = p->hist; m.step = p->step; m.position = p->position;
-  m.barrier = p->barrier; m.epoch = p->epoch;
-  m.n_tokens = p->n_tokens; m.splits = p->splits;
-  m.ks_hidden = m.ks_inter = m.ks_attn = m.xs_bytes = 0;
-  return vb::decode_mega(m, st(stream));
 }
 
 }  // extern "C"

@@ -250,46 +250,4 @@ struct SampleParams {
 };
 int sample_batch(const SampleParams& p, cudaStream_t stream);
 
-// ---- persistent decode mega-kernel (decode_mega.cu) -------------------------------------------
-struct MegaLayer {  // device-resident array, one entry per decoder layer
-  const __nv_bfloat16* qkv_w;   // [(Hq+2Hkv)*128, hidden]
-  const __nv_bfloat16* qkv_b;   // [(Hq+2Hkv)*128]
-  const __nv_bfloat16* o_w;     // [hidden, Hq*128]
-  const __nv_bfloat16* gu_w;    // [2*inter, hidden], rows interleaved (gate, up)
-  const __nv_bfloat16* down_w;  // [hidden, inter]
-  const __nv_bfloat16* ln1_w;   // [hidden]
-  const __nv_bfloat16* ln2_w;   // [hidden]
-  __nv_bfloat16* k_pool;        // [P, 128, Hkv, 128]
-  __nv_bfloat16* v_pool;
-};
-struct MegaParams {
-  const MegaLayer* layers;
-  int num_layers;
-  const __nv_bfloat16* final_norm_w;
-  const __nv_bfloat16* lm_head_w;
-  const __nv_bfloat16* embed;
-  int hidden, inter, Hq, Hkv, vocab;
-  float eps, scale;
-  const float* inv_freq;
-  const int32_t* page_table;
-  __nv_bfloat16* x;     // [hidden] residual stream (in: embedding of the current token)
-  __nv_bfloat16* qkv;   // [(Hq+2Hkv)*128]
-  __nv_bfloat16* act;   // [inter]
-  float* attn_ws;       // [Hkv*splits*G*(128+2)]
-  int* attn_counters;   // [Hkv] zero-initialised (self-cleaning)
-  unsigned long long* key;
-  int32_t* token;
-  int32_t* hist;
-  int32_t* step;
-  int32_t* position;
-  unsigned int* barrier;  // grid-barrier counter; barrier == epoch between launches (both start at 0)
-  unsigned int* epoch;
-  int n_tokens, splits;
-  // derived by the launcher
-  int ks_hidden, ks_inter, ks_attn, xs_bytes;
-  long long* debug_times = nullptr;  // optional [phases][6] clock64 stamps (profiling aid)
-  int debug_cta = 0;
-};
-int decode_mega(const MegaParams& p, cudaStream_t stream);
-
 }  // namespace vb

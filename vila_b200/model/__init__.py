@@ -5,7 +5,7 @@ from .llava_llama import (BasicImageEncoder, BasicVideoEncoder, LlavaLlamaModel,
                           TSPVideoEncoder)
 from .modeling_vila import VILAForCausalLM
 from .projector import MultimodalProjector
-from .qwen2 import GraphDecoder, MegaDecoder, PagedKVCache, Qwen2ForCausalLM
+from .qwen2 import GraphDecoder, PagedKVCache, Qwen2ForCausalLM
 from .vision import SiglipVisionModel, SiglipVisionTower
 
 __all__ = [n for n in dir() if not n.startswith("_")]

@@ -493,13 +493,9 @@ class Qwen2ForCausalLM(nn.Module):
         self.decode_weights = fmt
 
     def decoder(self, max_new_tokens: int):
-        """Greedy decode engine: the CUDA graph of per-layer kernels (default) or, with
-        VILA_B200_DECODER=mega, the persistent whole-token mega-kernel."""
-        import os
-        kind = MegaDecoder if os.environ.get("VILA_B200_DECODER", "graph") == "mega" else GraphDecoder
-        if (self._decoder is None or self._decoder.max_new < max_new_tokens
-                or type(self._decoder) is not kind):
-            self._decoder = kind(self, max(max_new_tokens, 128))
+        """Greedy decode engine: the CUDA graph of per-layer kernels, reused while it holds enough tokens."""
+        if self._decoder is None or self._decoder.max_new < max_new_tokens:
+            self._decoder = GraphDecoder(self, max(max_new_tokens, 128))
         return self._decoder
 
     @torch.inference_mode()
@@ -672,7 +668,7 @@ class GraphDecoder:
 
     MAX_SPLITS = 64
 
-    def __init__(self, llm: Qwen2ForCausalLM, max_new: int, num_splits: Optional[int] = None):
+    def __init__(self, llm: Qwen2ForCausalLM, max_new: int):
         self.llm = llm
         cfg = llm.config
         dev, dt = llm.device, llm.dtype
@@ -681,8 +677,7 @@ class GraphDecoder:
         self.fp8 = llm._fp8_weights
         self.w4 = llm._w4_weights
         Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
-        self._fixed_splits = num_splits
-        self.num_splits = 8 if num_splits is None else num_splits
+        self.num_splits = 8
         self.x = torch.zeros(cfg.hidden_size, device=dev, dtype=dt)
         self.qkv = torch.zeros((Hq + 2 * Hkv) * D, device=dev, dtype=dt)
         self.attn = torch.zeros(Hq * D, device=dev, dtype=dt)
@@ -721,8 +716,6 @@ class GraphDecoder:
         (video: 16K-66K tokens = 34-135 MB of K/V per layer) are a bandwidth problem: the wgmma FMHA
         kernel in split-KV mode, one CTA per SM (Hkv * splits <= #SMs), every split a whole number of
         128-token pages and all splits of (nearly) equal length."""
-        if self._fixed_splits is not None:
-            return self._fixed_splits, 0
         if ctx <= 512:
             return 0, 0   # one CTA per query head, no split / combine (decode_attn_head_kernel)
         if ctx <= self.LONG_CTX:
@@ -835,74 +828,3 @@ class GraphDecoder:
     def tokens(self, n: int) -> List[int]:
         return self.hist[:n].tolist()
 
-
-class MegaDecoder(GraphDecoder):
-    """Same contract as GraphDecoder, but `run(n)` is ONE launch of the persistent decode mega-kernel
-    (vila_decode_mega): all layers of n tokens, weights streamed through per-warp TMA rings that run
-    ahead across layer / token boundaries, grid barriers between phases."""
-
-    def __init__(self, llm: Qwen2ForCausalLM, max_new: int, num_splits: int = 8):
-        if llm.decode_weights != "bf16":
-            raise NotImplementedError("the decode mega-kernel streams bf16 weights only: use the graph decoder "
-                                      f"for decode_weights={llm.decode_weights!r}")
-        super().__init__(llm, max_new, num_splits)  # the mega-kernel keeps 8 cluster-free splits
-        cfg = llm.config
-        dev = llm.device
-        Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
-        assert D == 128, "the decode mega-kernel is specialised for head_dim 128"
-        self.barrier = torch.zeros(1, device=dev, dtype=torch.int32)
-        self.epoch = torch.zeros(1, device=dev, dtype=torch.int32)
-        self.attn_ws = torch.zeros(Hkv * num_splits * (Hq // Hkv) * (D + 2), device=dev, dtype=torch.float32)
-        self.layer_table = None
-        self._table_key = None
-
-    @property
-    def launches_per_step(self) -> int:
-        return 1
-
-    def _table(self):
-        cache = self.cache
-        key = cache.pool.data_ptr()
-        if self._table_key != key:
-            rows = []
-            for li, layer in enumerate(self.llm.model.layers):
-                rows.append([layer._qkv_w.data_ptr(), layer._qkv_b.data_ptr(),
-                             layer.self_attn.o_proj.weight.data_ptr(), layer._gu_w.data_ptr(),
-                             layer.mlp.down_proj.weight.data_ptr(), layer.input_layernorm.weight.data_ptr(),
-                             layer.post_attention_layernorm.weight.data_ptr(),
-                             cache.k(li).data_ptr(), cache.v(li).data_ptr()])
-            self.layer_table = torch.tensor(rows, dtype=torch.int64, device=self.llm.device)
-            self._table_key = key
-        return self.layer_table
-
-    def run(self, n_tokens: int) -> None:
-        import ctypes as C
-        from .. import _lib
-        n = n_tokens
-        if self._started == 1:
-            n -= 1
-            self._started = 2
-        if n <= 0:
-            return
-        llm, cfg = self.llm, self.llm.config
-        p = _lib.MegaParams()
-        p.layers = self._table().data_ptr()
-        p.num_layers = cfg.num_hidden_layers
-        p.final_norm_w = llm.model.norm.weight.data_ptr()
-        p.lm_head_w = llm.lm_head.weight.data_ptr()
-        p.embed = llm.model.embed_tokens.weight.data_ptr()
-        p.hidden, p.inter = cfg.hidden_size, cfg.intermediate_size
-        p.Hq, p.Hkv, p.vocab = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.vocab_size
-        p.eps, p.scale = cfg.rms_norm_eps, cfg.head_dim ** -0.5
-        p.inv_freq = llm.inv_freq.data_ptr()
-        p.page_table = self.cache.page_table.data_ptr()
-        p.x, p.qkv, p.act = self.x.data_ptr(), self.qkv.data_ptr(), self.act.data_ptr()
-        p.attn_ws = self.attn_ws.data_ptr()
-        p.attn_counters = self.counters.data_ptr()
-        p.key, p.token, p.hist = self.key.data_ptr(), self.token.data_ptr(), self.hist.data_ptr()
-        p.step, p.position = self.step.data_ptr(), self.position.data_ptr()
-        p.barrier, p.epoch = self.barrier.data_ptr(), self.epoch.data_ptr()
-        p.n_tokens, p.splits = n, self.num_splits
-        _lib.check(_lib.load().vila_decode_mega(C.byref(p), torch.cuda.current_stream().cuda_stream),
-                   "vila_decode_mega")
-        self.cache.length += n
