@@ -2,6 +2,7 @@
 from __future__ import annotations
 
 import json
+import math
 import os
 from typing import Dict, List
 
@@ -219,20 +220,25 @@ class Bf16Errors:
         self._bias_sum = 0.0
         self.n = 0
 
-    def add(self, got: torch.Tensor, ref_final: torch.Tensor, row0: int = 0) -> "Bf16Errors":
+    def add(self, got: torch.Tensor, ref_final: torch.Tensor, row0: int = 0, allow: torch.Tensor = None,
+            row_scale: torch.Tensor = None) -> "Bf16Errors":
+        """allow: per-element allowance that replaces B_RMS * rms(ref row) in check 1 (shape of got);
+        row_scale: per-row scale that replaces rms(ref row) in check 2 (one value per row)."""
         got = got.to(torch.float64).reshape(-1, ref_final.shape[-1])
         ref_final = ref_final.to(torch.float64).reshape(got.shape)
         ref = _rb64(ref_final)
         diff = got - ref
         ulp = bf16_ulp(ref)
         rms = ref.pow(2).mean(dim=1, keepdim=True).sqrt().clamp_min(1e-30)
-        ratio = diff.abs() / (self.A_ULP * ulp + self.B_RMS * rms)
+        extra = self.B_RMS * rms if allow is None else allow.to(torch.float64).reshape(got.shape)
+        ratio = diff.abs() / (self.A_ULP * ulp + extra)
         i = int(ratio.argmax())
         v = ratio.view(-1)[i].item()
         if self.where is None or not v <= self.excess:  # (a NaN sticks)
             self.excess, self.where = v, (row0 + i // got.shape[1], i % got.shape[1])
         self.max_ulps = max(self.max_ulps, (diff.abs() / bf16_ulp(torch.maximum(ref.abs(), rms))).max().item())
-        rows = diff.pow(2).mean(dim=1).sqrt() / rms[:, 0]
+        scale = rms[:, 0] if row_scale is None else row_scale.to(torch.float64).reshape(-1)
+        rows = diff.pow(2).mean(dim=1).sqrt() / scale
         r = int(rows.argmax())
         if self.worst_row_at is None or not rows[r].item() <= self.worst_row:
             self.worst_row, self.worst_row_at = rows[r].item(), row0 + r
@@ -250,7 +256,7 @@ class Bf16Errors:
         if not self.excess <= 1.0:
             out.append(f"element {self.where}: error {self.excess:.2f}x the tolerance")
         if not self.worst_row <= self.ROW_RMS:
-            out.append(f"row {self.worst_row_at}: rms error {self.worst_row:.3e} of the row rms > {self.ROW_RMS:.3e}")
+            out.append(f"row {self.worst_row_at}: rms error {self.worst_row:.3e} x the row scale > {self.ROW_RMS:.3e}")
         if not abs(self.bias) <= self.BIAS_ULP:
             out.append(f"rounding bias {self.bias:+.3f} ulp (|bias| > {self.BIAS_ULP})")
         return out
@@ -262,6 +268,156 @@ class Bf16Errors:
     def check(self, name: str) -> None:
         bad = self.failures()
         assert not bad, f"{name}: " + "; ".join(bad)
+
+
+# ------------------------------------------------------------------------------------------------
+# prefill attention: the fp64 reference, the checker, and the three input families
+# ------------------------------------------------------------------------------------------------
+class AttnErrors(Bf16Errors):
+    """Bf16Errors for one attention output [Sq, Hq, D] against the fp64 reference of attention_reference.
+    A row is one (query, head) pair: rows are numbered query * Hq + head.
+
+    The kernel (fmha_wgmma.cu) computes, per row, o = sum_j bf16(p_j) v_j / l with p_j = exp2(s_j *
+    scale*log2(e) - m) for a running maximum m, l = sum_j p_j summed from the UNROUNDED p_j, and rounds
+    o / l to bf16 once.  Every common factor of p (the stale maxima, the alpha rescales) cancels between
+    the numerator and l, so the only error that does not cancel is the rounding of each p_j to bf16,
+    relative error delta_j with |delta_j| <= 2^-8 (the bf16 unit roundoff; p >= 2^-126 stays normal):
+        e_d = sum_j delta_j p_j v_jd / l,   |e_d| <= 2^-8 * A_d,   A_d = sum_j p_j |v_jd| / l.
+    1. per element:  |got - bf16(ref_final)| <= A_ULP * ulp_bf16(ref) + P_ROUND * A_d
+       A_ULP = 1: the output's own rounding, which may go the other way at a tie once e_d moves the
+         value across it (|got - ref| <= |e_d| + 1 ulp).
+       P_ROUND = 2^-7, twice the bound on e_d: the factor 2 absorbs the fp32 score accumulation, the
+         fp32 products s * scale*log2(e), ex2.approx (relative error ~2^-22) and the fp32 alpha
+         products, each below 2^-11 of p for scores within a few thousand of the row maximum.
+         tests/test_attention_cpu.py checks this on an emulation of that arithmetic.
+    2. per row:  rms_d(got - ref) <= ROW_RMS * sqrt(mean_d(2^-16 * S2_d + ulp_d^2 / 4)),
+       S2_d = sum_j p_j^2 v_jd^2 / l^2.  The delta_j are independent, so e_d has a standard deviation
+       of at most 2^-8 sqrt(S2_d); rounding then adds E[(got - ref)^2] <= e_d^2 + ulp^2 / 4.  The bound
+       falls as attention spreads over more keys (S2 ~ |v|^2 / n_keys), so one leaked or dropped key
+       still shows in a long row where the per-element bound (~ 2^-7 |v|) would not see it.
+       ROW_RMS = 3: elementwise |got - ref| <= |e_d| + ulp_d, so rms(got - ref)^2 <= 2 rms(e)^2 +
+       2 mean(ulp^2), which is within 9 x (2^-16 mean(S2) + mean(ulp^2) / 4) as long as rms(e) stays
+       within 2.1 x its bound 2^-8 sqrt(mean(S2)) (a row of only 72 elements may sample it high).  A row
+       in which every element is one ulp off and e is negligible sits at 2.
+    3. rounding bias: as Bf16Errors.  Truncating P or the output moves every value toward zero by a
+       fraction of an ulp; only the mean sees it."""
+    A_ULP = 1.0
+    P_ROUND = 2.0 ** -7
+    ROW_RMS = 3.0
+
+    def add_attention(self, got: torch.Tensor, ref_final: torch.Tensor, A: torch.Tensor, S2: torch.Tensor,
+                      row0: int = 0) -> "AttnErrors":
+        D = ref_final.shape[-1]
+        ulp = bf16_ulp(_rb64(ref_final.to(torch.float64)))
+        row_scale = (2.0 ** -16 * S2.to(torch.float64) + ulp.pow(2) / 4).reshape(-1, D).mean(dim=1).sqrt()
+        return self.add(got, ref_final, row0, allow=self.P_ROUND * A, row_scale=row_scale)
+
+
+def attention_reference(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, *, causal: bool, scale: float,
+                        budget: int = 1 << 27):
+    """Prefill attention in fp64 on q's device, in blocks of query rows (never Sq x Sk x Hq at once).
+    q [Sq, Hq, D], k / v [Sk, Hkv, D] (the kernel's bf16 inputs: q after RoPE, K/V as stored in the pool,
+    in token order); query head h reads KV head h // (Hq / Hkv); causal: query i sees keys j <= i + Sk - Sq.
+    Yields (r0, r1, ref_final, A, S2), each [r1 - r0, Hq, D] in fp64:
+      ref_final = sum_j p_ij v_jd / l_i,  A = sum_j p_ij |v_jd| / l_i,  S2 = sum_j p_ij^2 v_jd^2 / l_i^2,
+    with p_ij = exp(s_ij - max_j s_ij), s_ij = scale * q_i . k_j, l_i = sum_j p_ij.
+    budget: fp64 elements of one block's scores."""
+    Sq, Hq, D = q.shape
+    Sk, Hkv = k.shape[0], k.shape[1]
+    G, off = Hq // Hkv, Sk - Sq
+    kd = k.to(torch.float64).permute(1, 2, 0)         # [Hkv, D, Sk]
+    vd = v.to(torch.float64).permute(1, 0, 2)[:, None]  # [Hkv, 1, Sk, D]
+    step = max(1, min(Sq, budget // (Hq * Sk)))
+    for r0 in range(0, Sq, step):
+        r1 = min(Sq, r0 + step)
+        n = r1 - r0
+        kv = min(Sk, r1 + off) if causal else Sk
+        qd = q[r0:r1].to(torch.float64).reshape(n, Hkv, G, D).permute(1, 2, 0, 3)  # [Hkv, G, n, D]
+        s = torch.matmul(qd, kd[:, None, :, :kv]).mul_(scale)                      # [Hkv, G, n, kv]
+        if causal:
+            i = torch.arange(r0, r1, device=q.device)[:, None]
+            j = torch.arange(kv, device=q.device)[None, :]
+            s.masked_fill_(j > i + off, float("-inf"))
+        p = s.sub_(s.amax(dim=-1, keepdim=True)).exp_()
+        del s
+        l = p.sum(dim=-1, keepdim=True)
+        vk = vd[:, :, :kv]
+        ref = torch.matmul(p, vk) / l
+        A = torch.matmul(p, vk.abs()) / l
+        S2 = torch.matmul(p.mul_(p), vk * vk) / (l * l)
+        del p
+
+        def out(t):
+            return t.permute(2, 0, 1, 3).reshape(n, Hq, D)
+        yield r0, r1, out(ref), out(A), out(S2)
+
+
+def attention_errors(got: torch.Tensor, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, *, causal: bool,
+                     scale: float, into: AttnErrors = None, row0: int = 0) -> AttnErrors:
+    """AttnErrors of the kernel output got [Sq, Hq, D] against attention_reference(q, k, v), added to
+    `into` (a new AttnErrors by default) with row numbers from row0 (several sequences in one checker)."""
+    e = AttnErrors() if into is None else into
+    Hq = q.shape[1]
+    for r0, r1, ref, A, S2 in attention_reference(q, k, v, causal=causal, scale=scale):
+        e.add_attention(got[r0:r1], ref, A, S2, row0 + r0 * Hq)
+    return e
+
+
+ATTN_FAMILIES = ("random", "sink", "probe")
+SENTINEL_V = 256.0  # V of every garbage key slot: large, finite (the kernel multiplies a masked P = 0 by it)
+PROBE_C = 4.0       # probe: q . k = PROBE_C * (key position - query position) on the position channels
+
+
+def attention_inputs(family: str, q_pos: torch.Tensor, key_pos: torch.Tensor, Hq: int, Hkv: int, D: int,
+                     scale: float, *, sink: torch.Tensor = None, garbage: torch.Tensor = None, seed: int = 0):
+    """q [nq, Hq, D] and k, v [N, Hkv, D] (bf16, on key_pos's device) for queries at global token positions
+    q_pos [nq] and N key slots at positions key_pos [N].  sink [N]: the first key of each sequence;
+    garbage [N]: slots no query may see (past Sk in the last page, unused pages).  Their V is SENTINEL_V.
+      random: scores scale * q.k with standard deviation ~1; three V channels 16x larger.
+      sink:   scores with standard deviation ~3, and the sink keys ~12 above the rest: P spans many
+              binades and the running maximum jumps.
+      probe:  score = scale * PROBE_C * (key position - query position) + noise of deviation ~0.3, so every
+              row is dominated by its last visible keys; garbage slots sit 256 positions past the last
+              real key.  A key leaked past the causal diagonal or the end of the sequence then changes the
+              output by O(1).  The position channels hold exact bf16 integers: key channel 0 = pos // 256,
+              1 = pos % 256, 2 = 3 = 1; query channel 0 = 256 c, 1 = c, 2 = -256 c (qpos // 256),
+              3 = -c (qpos % 256); the noise lives in channels >= 16 (its own k16 wgmma step)."""
+    dev = key_pos.device
+    g = torch.Generator(device=dev).manual_seed(seed)
+    nq, N = q_pos.numel(), key_pos.numel()
+    garbage = torch.zeros(N, dtype=torch.bool, device=dev) if garbage is None else garbage
+    v = torch.randn(N, Hkv, D, device=dev, generator=g)
+    if family == "random":
+        q = torch.randn(nq, Hq, D, device=dev, generator=g)
+        k = torch.randn(N, Hkv, D, device=dev, generator=g) / (scale * math.sqrt(D))
+        v[:, :, [3, D // 2, D - 5]] *= 16.0
+    elif family == "sink":
+        sd = math.sqrt(3.0 / (scale * math.sqrt(D - 1)))
+        q = torch.randn(nq, Hq, D, device=dev, generator=g) * sd
+        k = torch.randn(N, Hkv, D, device=dev, generator=g) * sd
+        q[:, :, 0] = 4.0
+        k[:, :, 0] = 0.0
+        if sink is not None:
+            k[sink, :, 0] = 12.0 / (4.0 * scale)
+    elif family == "probe":
+        sd = math.sqrt(0.3 / (scale * math.sqrt(D - 16)))
+        q = torch.zeros(nq, Hq, D, device=dev)
+        k = torch.zeros(N, Hkv, D, device=dev)
+        q[:, :, 16:] = torch.randn(nq, Hq, D - 16, device=dev, generator=g) * sd
+        k[:, :, 16:] = torch.randn(N, Hkv, D - 16, device=dev, generator=g) * sd
+        kp = torch.where(garbage, key_pos[~garbage].max() + 256, key_pos) if bool((~garbage).any()) else key_pos
+        assert int(kp.max()) < 65536 and int(q_pos.max()) < 65536
+        c = PROBE_C
+        k[:, :, 0] = (kp // 256).to(k.dtype)[:, None]
+        k[:, :, 1] = (kp % 256).to(k.dtype)[:, None]
+        k[:, :, 2:4] = 1.0
+        q[:, :, 0], q[:, :, 1] = 256 * c, c
+        q[:, :, 2] = (-256 * c * (q_pos // 256)).to(q.dtype)[:, None]
+        q[:, :, 3] = (-c * (q_pos % 256)).to(q.dtype)[:, None]
+    else:
+        raise ValueError(family)
+    v[garbage] = SENTINEL_V
+    return q.to(torch.bfloat16), k.to(torch.bfloat16), v.to(torch.bfloat16)
 
 
 def greedy_ids_match(got: List[int], oracle_ids: List[int], oracle_logits: torch.Tensor,
