@@ -393,6 +393,32 @@ typedef struct vila_sample_params {
 } vila_sample_params;
 int vila_sample_batch(const vila_sample_params* p, void* stream);
 
+/* vila_sample_finalize — the single-stream decoder's end of a sampled step, the sampling counterpart of
+ * vila_argmax_finalize.  Replaces the same seam as vila_sample_batch (HF GenerationMixin._sample, reached from
+ * llava_arch.py:823-833) for GraphDecoder.  One row of bf16 logits [V] (the lm_head GEMV's output); inv_temperature,
+ * top_k, top_p and seed are DEVICE scalars (a new request writes them, a captured graph keeps replaying) and the
+ * token index t is *step.  The token is drawn by the rule of vila_sample_batch and is bit-identical to it with
+ * M = 1 on the same row, parameters, seed and t.  Then, as vila_argmax_finalize: *token_out = token,
+ * token_hist[t] = token (token_hist may be NULL), *step = t + 1, *position += 1 (position may be NULL) and
+ * x_next = embed_table[token] (hidden values; both NULL: no copy).  One cluster of 8 CTAs, PDL.
+ * 1 <= V <= 327,680; hidden a multiple of 8; embed_table / x_next 16-byte aligned.  The argument errors are
+ * reported before any device call. */
+typedef struct vila_sample_finalize_params {
+  const void* logits;
+  const float* inv_temperature;
+  const int32_t* top_k;
+  const float* top_p;
+  const int64_t* seed;
+  int32_t* step;
+  int32_t* position;
+  int32_t* token_out;
+  int32_t* token_hist;
+  const void* embed_table;
+  void* x_next;
+  int32_t V, hidden;
+} vila_sample_finalize_params;
+int vila_sample_finalize(const vila_sample_finalize_params* p, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

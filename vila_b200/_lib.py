@@ -83,6 +83,15 @@ class SampleParams(C.Structure):
     ]
 
 
+class SampleFinalizeParams(C.Structure):
+    _fields_ = [
+        ("logits", c_void_p), ("inv_temperature", c_void_p), ("top_k", c_void_p), ("top_p", c_void_p),
+        ("seed", c_void_p), ("step", c_void_p), ("position", c_void_p), ("token_out", c_void_p),
+        ("token_hist", c_void_p), ("embed_table", c_void_p), ("x_next", c_void_p), ("V", C.c_int32),
+        ("hidden", C.c_int32),
+    ]
+
+
 # name -> argtypes; every function returns int (0 == ok) unless listed in _RESTYPES
 SIGNATURES = {
     "vila_abi_version": [],
@@ -129,6 +138,7 @@ SIGNATURES = {
                              c_int, c_void_p],
     "vila_decode_attention_fp8_batch": [C.POINTER(DecodeAttnFp8Params), c_void_p],
     "vila_sample_batch": [C.POINTER(SampleParams), c_void_p],
+    "vila_sample_finalize": [C.POINTER(SampleFinalizeParams), c_void_p],
 }
 _RESTYPES = {"vila_last_error": C.c_char_p}
 

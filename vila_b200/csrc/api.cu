@@ -426,4 +426,25 @@ int vila_sample_batch(const vila_sample_params* p, void* stream) {
   return vb::sample_batch(d, st(stream));
 }
 
+// GenerationMixin._sample's warpers + torch.multinomial for the single-stream graph decoder
+int vila_sample_finalize(const vila_sample_finalize_params* p, void* stream) {
+  VB_CHECK(p != nullptr, "vila_sample_finalize: params are required");
+  vb::SampleFinalizeParams d;
+  d.logits = cb(p->logits);
+  d.inv_temperature = p->inv_temperature;
+  d.top_k = p->top_k;
+  d.top_p = p->top_p;
+  d.seed = p->seed;
+  d.step = p->step;
+  d.position = p->position;
+  d.token_out = p->token_out;
+  d.token_hist = p->token_hist;
+  d.embed_table = cb(p->embed_table);
+  d.x_next = mb(p->x_next);
+  d.V = p->V; d.hidden = p->hidden;
+  if (int rc = vb::sample_finalize_check(d)) return rc;
+  VB_REQUIRE_DEVICE();
+  return vb::sample_finalize(d, st(stream));
+}
+
 }  // extern "C"

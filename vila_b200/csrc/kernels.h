@@ -249,5 +249,24 @@ struct SampleParams {
   int M, V;
 };
 int sample_batch(const SampleParams& p, cudaStream_t stream);
+// the single-stream decoder's end of a sampled step: one row, device-scalar parameters, t = *step; then
+// token_out = token, token_hist[t] = token (if given), step + 1, position + 1 (if given), x_next = embed_table[token]
+// (if given).  Bit-identical to sample_batch with M = 1 on the same row, parameters, seed and t.
+struct SampleFinalizeParams {
+  const __nv_bfloat16* logits;   // [V]
+  const float* inv_temperature;  // device scalars, as sample_batch's per-row arrays
+  const int32_t* top_k;
+  const float* top_p;
+  const int64_t* seed;
+  int32_t* step;                 // t; incremented
+  int32_t* position;             // incremented, or null
+  int32_t* token_out;
+  int32_t* token_hist;           // or null
+  const __nv_bfloat16* embed_table;  // [*, hidden] with x_next, or both null
+  __nv_bfloat16* x_next;
+  int V, hidden;
+};
+int sample_finalize_check(const SampleFinalizeParams& p);  // the argument errors, before any device call
+int sample_finalize(const SampleFinalizeParams& p, cudaStream_t stream);
 
 }  // namespace vb

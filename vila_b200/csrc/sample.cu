@@ -1,4 +1,6 @@
-// Temperature / top-k / top-p sampling of the continuous-batching engine (vila_b200/serving.py, sampling=True).
+// Temperature / top-k / top-p sampling on the device: vila_sample_batch for the continuous-batching engine
+// (vila_b200/serving.py, sampling=True) and vila_sample_finalize for the single-stream graph decoder
+// (GraphDecoder's sampled step, vila_b200/model/qwen2.py).
 //
 // The rule (stated in torch / numpy by vila_b200/sampling.py, which the tests use) for a row of bf16 logits with
 // inv_T, top_k, top_p, a 64-bit seed and the token index t of the request:
@@ -18,6 +20,11 @@
 // not depend on thread order.  Histograms and arg-maxes are merged through DSMEM.  Greedy rows run one max pass,
 // "T only" rows one draw pass.  A row's token depends only on its own logits and parameters.
 //
+// Both kernels run the same selection code (draw_row), templated on the cluster width.  Every quantity it decides on
+// is independent of how the row is cut into slices (integer histograms and masses summed over the whole cluster,
+// exact arg-maxes with ties to the lowest index, Philox counters from the global index), so a wider cluster draws
+// the same token.  sample_finalize_kernel serves one row; its width is kFinCluster.
+//
 // Replaces HF TemperatureLogitsWarper / TopKLogitsWarper / TopPLogitsWarper + torch.multinomial in
 // GenerationMixin._sample, reached from llava_arch.py:823-833.
 #include <math.h>
@@ -30,7 +37,12 @@ namespace {
 
 constexpr int kSampThreads = 256;
 constexpr int kSampWarps = kSampThreads / 32;
-constexpr int kSampCluster = 8;
+constexpr int kSampCluster = 8;   // vila_sample_batch: one 8-CTA cluster per row
+// vila_sample_finalize serves one row, so a wider (non-portable) 16-CTA cluster was timed against 8 on an H100 SXM
+// (700 W) at V = 152,064, back-to-back launches: 16 CTAs won for greedy (5.6 vs 7.6 us) and T only (14.6 vs 25.0 us)
+// but lost for top-p 0.9 (196 vs 167 us) and top-k 50 + top-p 0.9 (327 vs 220 us), where every radix round merges one
+// histogram per CTA through DSMEM.  Top-p is the common request (the server's default is top_p 0.9), so: 8.
+constexpr int kFinCluster = 8;
 constexpr int kSampMaxSlice = 40960;  // fp32 values per CTA: V <= 327,680
 constexpr int kHistBins = 2048;       // radix digits: bits [21, 32), [10, 21), [0, 10)
 constexpr float kMassScale = 1099511627776.f;  // 2^40: fixed-point unit of the top-p masses
@@ -131,10 +143,11 @@ __device__ void cta_argmax(SampleScratch& sc, double v, int i, int slot) {
 }
 
 // cluster arg-max of slot `slot` (after cta_argmax), read from every rank in rank order
+template <int kC>
 __device__ void cluster_argmax(SampleScratch& sc, int slot, double* v, int* i) {
   double bv = ld_dsmem_f64(&sc.cta_v[slot], 0);
   int bi = ld_dsmem_s32(&sc.cta_i[slot], 0);
-  for (uint32_t r = 1; r < kSampCluster; ++r) {
+  for (uint32_t r = 1; r < kC; ++r) {
     const double ov = ld_dsmem_f64(&sc.cta_v[slot], r);
     const int oi = ld_dsmem_s32(&sc.cta_i[slot], r);
     if (better(ov, oi, bv, bi)) bv = ov, bi = oi;
@@ -148,7 +161,8 @@ __device__ void cluster_argmax(SampleScratch& sc, int slot, double* v, int* i) {
 // (bins - 1).  The cluster's histogram is merged and scanned from the top bin down; the first bin whose inclusive
 // sum reaches the target is returned (*bin_out) with the sum strictly above it (*above_out).  target_p > 0
 // replaces the target by clamp(ceil(target_p * total), 1, total), total being this round's whole sum; *target_out
-// gets the target used.  Every thread of every CTA of the cluster calls it.
+// gets the target used.  Every thread of every CTA of the kC-CTA cluster calls it.
+template <int kC>
 __device__ void radix_round(SampleScratch& sc, const float* s_sh, int n_local, int round, bool mass, float m,
                             uint32_t lo_key, uint32_t mask, uint32_t prefix, int shift, int bins,
                             unsigned long long target, double target_p, uint32_t* bin_out,
@@ -174,7 +188,7 @@ __device__ void radix_round(SampleScratch& sc, const float* s_sh, int n_local, i
     vals[j] = 0;
     if (j < per) {
       const int b = bins - 1 - (threadIdx.x * per + j);
-      for (uint32_t r = 0; r < kSampCluster; ++r) vals[j] += ld_dsmem_u64(&h[b], r);
+      for (uint32_t r = 0; r < kC; ++r) vals[j] += ld_dsmem_u64(&h[b], r);
       tot += vals[j];
     }
   }
@@ -218,6 +232,7 @@ __device__ void radix_round(SampleScratch& sc, const float* s_sh, int n_local, i
 }
 
 // Three rounds: the key at which the inclusive (count or mass) sum from the top first reaches the target.
+template <int kC>
 __device__ uint32_t radix_select(SampleScratch& sc, const float* s_sh, int n_local, int* round, bool mass, float m,
                                  uint32_t lo_key, unsigned long long target, double target_p) {
   uint32_t prefix = 0, mask = 0;
@@ -227,7 +242,7 @@ __device__ uint32_t radix_select(SampleScratch& sc, const float* s_sh, int n_loc
     const int bins = r == 2 ? 1024 : 2048;
     uint32_t bin;
     unsigned long long above, used;
-    radix_round(sc, s_sh, n_local, (*round)++, mass, m, lo_key, mask, prefix, shift, bins, target,
+    radix_round<kC>(sc, s_sh, n_local, (*round)++, mass, m, lo_key, mask, prefix, shift, bins, target,
                 r == 0 ? target_p : 0.0, &bin, &above, &used);
     prefix |= bin << shift;
     mask |= static_cast<uint32_t>(bins - 1) << shift;
@@ -236,27 +251,31 @@ __device__ uint32_t radix_select(SampleScratch& sc, const float* s_sh, int n_loc
   return prefix;
 }
 
-__global__ void __launch_bounds__(kSampThreads, 2) sample_kernel(SampleArgs a) {
-  extern __shared__ __align__(16) unsigned char smem[];
-  SampleScratch& sc = *reinterpret_cast<SampleScratch*>(smem);
-  float* s_sh = reinterpret_cast<float*>(smem + ((sizeof(SampleScratch) + 15) & ~size_t(15)));
-  griddep_wait();
-  griddep_launch_dependents();
-  const int row = blockIdx.y;
-  if (a.position[row] < 0) return;  // idle slot: the whole cluster leaves, its token is untouched
+// One row's draw: its logits, parameters, seed and token index t.
+struct RowDraw {
+  const __nv_bfloat16* logits;  // the row
+  int V, slice;                 // slice: values per CTA, a multiple of 4
+  float inv_t;
+  int top_k;
+  float top_p;
+  uint64_t seed, t;
+};
+
+// The rule on one row.  Every thread of every CTA of the kC-CTA cluster calls it.  Returns the slot whose per-CTA
+// arg-maxes decide the token (0: greedy max pass, 1: draw pass); on return they are published by a cluster barrier,
+// so any CTA may merge them with cluster_argmax<kC>.  With count, sc.cta_n holds the CTA's kept count (draw pass).
+template <int kC>
+__device__ int draw_row(SampleScratch& sc, float* s_sh, const RowDraw& d, bool count) {
   const uint32_t rank = cluster_ctarank();
-  const int base = static_cast<int>(rank) * a.slice;
-  const int n_local = max(0, min(a.slice, a.V - base));
-  const float inv_t = a.inv_t[row];
-  const int top_k = a.top_k[row];
-  const float top_p = a.top_p[row];
-  const bool greedy = !(inv_t > 0.f) || top_k == 1;
-  const bool use_k = !greedy && top_k > 1 && top_k < a.V;
-  const bool use_p = !greedy && top_p < 1.f;
-  const float mul = greedy ? 1.f : inv_t;
+  const int base = static_cast<int>(rank) * d.slice;
+  const int n_local = max(0, min(d.slice, d.V - base));
+  const bool greedy = !(d.inv_t > 0.f) || d.top_k == 1;
+  const bool use_k = !greedy && d.top_k > 1 && d.top_k < d.V;
+  const bool use_p = !greedy && d.top_p < 1.f;
+  const float mul = greedy ? 1.f : d.inv_t;
 
   // pass 1: s into shared memory, and the slice's first arg-max
-  const __nv_bfloat16* lrow = a.logits + static_cast<int64_t>(row) * a.ld + base;
+  const __nv_bfloat16* lrow = d.logits + base;
   const bool vec = (reinterpret_cast<uintptr_t>(lrow) & 7) == 0;
   float best = -INFINITY;
   int best_i = INT_MAX;
@@ -281,15 +300,7 @@ __global__ void __launch_bounds__(kSampThreads, 2) sample_kernel(SampleArgs a) {
 
   if (greedy) {
     cta_argmax(sc, best, best_i, 0);
-    if (rank == 0 && threadIdx.x == 0) {
-      double v;
-      int i;
-      cluster_argmax(sc, 0, &v, &i);
-      a.tokens[row] = i;
-      if (a.n_kept) a.n_kept[row] = 1;
-    }
-    cluster_sync_all();  // no CTA leaves while rank 0 reads its shared memory
-    return;
+    return 0;
   }
 
   float m = 0.f;
@@ -297,18 +308,17 @@ __global__ void __launch_bounds__(kSampThreads, 2) sample_kernel(SampleArgs a) {
     cta_argmax(sc, best, best_i, 0);
     double v;
     int i;
-    cluster_argmax(sc, 0, &v, &i);
+    cluster_argmax<kC>(sc, 0, &v, &i);
     m = static_cast<float>(v);
   }
   int round = 0;
   uint32_t lo_key = 0;  // kept: key >= lo_key
-  if (use_k) lo_key = radix_select(sc, s_sh, n_local, &round, false, 0.f, 0u, static_cast<unsigned long long>(top_k), 0.0);
-  if (use_p) lo_key = radix_select(sc, s_sh, n_local, &round, true, m, lo_key, 0ull, static_cast<double>(top_p));
+  if (use_k)
+    lo_key = radix_select<kC>(sc, s_sh, n_local, &round, false, 0.f, 0u, static_cast<unsigned long long>(d.top_k), 0.0);
+  if (use_p) lo_key = radix_select<kC>(sc, s_sh, n_local, &round, true, m, lo_key, 0ull, static_cast<double>(d.top_p));
 
   // pass 2: Gumbel-max over the kept set
-  const uint64_t seed = static_cast<uint64_t>(a.seed[row]);
-  const uint64_t t = static_cast<uint64_t>(a.step[row]);
-  const uint32_t k0 = static_cast<uint32_t>(seed), k1 = static_cast<uint32_t>(seed >> 32);
+  const uint32_t k0 = static_cast<uint32_t>(d.seed), k1 = static_cast<uint32_t>(d.seed >> 32);
   double bv = -INFINITY;
   int bi = INT_MAX;
   unsigned cnt = 0;
@@ -322,9 +332,9 @@ __global__ void __launch_bounds__(kSampThreads, 2) sample_kernel(SampleArgs a) {
       any |= keep[e];
     }
     if (!any) continue;
-    const uint4 x = philox4x32_10(
-        make_uint4(static_cast<uint32_t>((base + j) >> 2), static_cast<uint32_t>(t), static_cast<uint32_t>(t >> 32), 0u),
-        k0, k1);
+    const uint4 x = philox4x32_10(make_uint4(static_cast<uint32_t>((base + j) >> 2), static_cast<uint32_t>(d.t),
+                                             static_cast<uint32_t>(d.t >> 32), 0u),
+                                  k0, k1);
     const uint32_t xs[4] = {x.x, x.y, x.z, x.w};
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
@@ -334,7 +344,7 @@ __global__ void __launch_bounds__(kSampThreads, 2) sample_kernel(SampleArgs a) {
       if (better(v, base + j + e, bv, bi)) bv = v, bi = base + j + e;
     }
   }
-  if (a.n_kept) {
+  if (count) {
     const unsigned wc = __reduce_add_sync(0xffffffffu, cnt);
     if ((threadIdx.x & 31) == 0) sc.warp_sum[threadIdx.x >> 5] = wc;
     __syncthreads();
@@ -345,23 +355,96 @@ __global__ void __launch_bounds__(kSampThreads, 2) sample_kernel(SampleArgs a) {
     }
   }
   cta_argmax(sc, bv, bi, 1);  // its cluster barrier also publishes cta_n
-  if (rank == 0 && threadIdx.x == 0) {
+  return 1;
+}
+
+__global__ void __launch_bounds__(kSampThreads, 2) sample_kernel(SampleArgs a) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  SampleScratch& sc = *reinterpret_cast<SampleScratch*>(smem);
+  float* s_sh = reinterpret_cast<float*>(smem + ((sizeof(SampleScratch) + 15) & ~size_t(15)));
+  griddep_wait();
+  griddep_launch_dependents();
+  const int row = blockIdx.y;
+  if (a.position[row] < 0) return;  // idle slot: the whole cluster leaves, its token is untouched
+  const RowDraw d{a.logits + static_cast<int64_t>(row) * a.ld, a.V, a.slice, a.inv_t[row], a.top_k[row],
+                  a.top_p[row], static_cast<uint64_t>(a.seed[row]), static_cast<uint64_t>(a.step[row])};
+  const int slot = draw_row<kSampCluster>(sc, s_sh, d, a.n_kept != nullptr);
+  if (cluster_ctarank() == 0 && threadIdx.x == 0) {
     double v;
     int i;
-    cluster_argmax(sc, 1, &v, &i);
+    cluster_argmax<kSampCluster>(sc, slot, &v, &i);
     a.tokens[row] = i;
     if (a.n_kept) {
-      unsigned long long c = 0;
-      for (uint32_t r = 0; r < kSampCluster; ++r) c += ld_dsmem_u64(&sc.cta_n, r);
+      unsigned long long c = 1;  // greedy rows keep one value
+      if (slot == 1) {
+        c = 0;
+        for (uint32_t r = 0; r < kSampCluster; ++r) c += ld_dsmem_u64(&sc.cta_n, r);
+      }
       a.n_kept[row] = static_cast<int32_t>(c);
     }
   }
-  cluster_sync_all();
+  cluster_sync_all();  // no CTA leaves while rank 0 reads its shared memory
+}
+
+struct FinalizeArgs {
+  const __nv_bfloat16* logits;
+  const float* inv_t;
+  const int32_t* top_k;
+  const float* top_p;
+  const int64_t* seed;
+  int32_t* step;
+  int32_t* position;
+  int32_t* token_out;
+  int32_t* token_hist;
+  const uint4* embed_table;
+  uint4* x_next;
+  int hidden_vec;  // 16-byte vectors per embedding row
+  int V, slice;
+};
+
+// The decoder's end of step: token = the rule's draw on the logits row at t = *step; token_out = token;
+// token_hist[t] = token; step and position + 1; x_next = embed_table[token], each CTA copying its share.
+template <int kC>
+__global__ void __launch_bounds__(kSampThreads, 2) sample_finalize_kernel(FinalizeArgs a) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  SampleScratch& sc = *reinterpret_cast<SampleScratch*>(smem);
+  float* s_sh = reinterpret_cast<float*>(smem + ((sizeof(SampleScratch) + 15) & ~size_t(15)));
+  __shared__ int tok_s;
+  griddep_wait();
+  griddep_launch_dependents();
+  const int32_t t = *a.step;  // read by every CTA before rank 0 advances it (after the draw's cluster barriers)
+  const RowDraw d{a.logits, a.V, a.slice, *a.inv_t, *a.top_k, *a.top_p, static_cast<uint64_t>(*a.seed),
+                  static_cast<uint64_t>(static_cast<int64_t>(t))};
+  const int slot = draw_row<kC>(sc, s_sh, d, false);
+  if (threadIdx.x == 0) {  // every CTA merges the cluster's arg-maxes itself
+    double v;
+    int i;
+    cluster_argmax<kC>(sc, slot, &v, &i);
+    tok_s = i;
+  }
+  __syncthreads();
+  const int tok = tok_s;
+  const uint32_t rank = cluster_ctarank();
+  if (rank == 0 && threadIdx.x == 0) {
+    *a.token_out = tok;
+    if (a.token_hist) a.token_hist[t] = tok;
+    *a.step = static_cast<int32_t>(static_cast<uint32_t>(t) + 1u);
+    if (a.position) *a.position = *a.position + 1;
+  }
+  if (a.x_next) {
+    const uint4* src = a.embed_table + static_cast<size_t>(tok) * a.hidden_vec;
+    for (int i = static_cast<int>(rank) * kSampThreads + threadIdx.x; i < a.hidden_vec; i += kC * kSampThreads)
+      a.x_next[i] = src[i];
+  }
+  cluster_sync_all();  // no CTA leaves while another reads its shared memory
 }
 
 size_t sample_smem_bytes(int slice) {
   return ((sizeof(SampleScratch) + 15) & ~size_t(15)) + static_cast<size_t>(slice) * sizeof(float);
 }
+
+// values per CTA when a cluster of `cluster` CTAs splits a row of V: a multiple of 4
+int slice_for(int V, int cluster) { return ((V + cluster - 1) / cluster + 3) & ~3; }
 
 }  // namespace
 
@@ -378,7 +461,7 @@ int sample_batch(const SampleParams& p, cudaStream_t stream) {
                (reinterpret_cast<uintptr_t>(p.position) & 3) == 0 && (reinterpret_cast<uintptr_t>(p.tokens) & 7) == 0 &&
                (reinterpret_cast<uintptr_t>(p.n_kept) & 3) == 0,
            "sample_batch: misaligned pointer");
-  const int slice = ((p.V + kSampCluster - 1) / kSampCluster + 3) & ~3;
+  const int slice = slice_for(p.V, kSampCluster);
   SampleArgs a{p.logits, p.ld, p.inv_temperature, p.top_k, p.top_p, p.seed, p.step, p.position, p.tokens, p.n_kept,
                p.V, slice};
   static PerDeviceOnce attr_once;
@@ -387,6 +470,41 @@ int sample_batch(const SampleParams& p, cudaStream_t stream) {
                                  (int)sample_smem_bytes(kSampMaxSlice)));
   VB_CUDA(launch_pdl_cluster(sample_kernel, dim3(kSampCluster, p.M), dim3(kSampThreads), sample_smem_bytes(slice),
                              stream, dim3(kSampCluster, 1, 1), a));
+  return 0;
+}
+
+int sample_finalize_check(const SampleFinalizeParams& p) {
+  VB_CHECK(p.logits && p.inv_temperature && p.top_k && p.top_p && p.seed && p.step && p.token_out,
+           "sample_finalize: logits, the four parameter scalars, step and token_out are required");
+  VB_CHECK(p.V >= 1 && p.V <= kSampCluster * kSampMaxSlice, "sample_finalize: bad vocabulary size V=%d (1..%d)", p.V,
+           kSampCluster * kSampMaxSlice);
+  VB_CHECK((p.embed_table == nullptr) == (p.x_next == nullptr),
+           "sample_finalize: embed_table and x_next go together");
+  VB_CHECK(p.x_next == nullptr || (p.hidden > 0 && p.hidden % 8 == 0),
+           "sample_finalize: hidden=%d must be a positive multiple of 8", p.hidden);
+  VB_CHECK((reinterpret_cast<uintptr_t>(p.logits) & 1) == 0 && (reinterpret_cast<uintptr_t>(p.inv_temperature) & 3) == 0 &&
+               (reinterpret_cast<uintptr_t>(p.top_k) & 3) == 0 && (reinterpret_cast<uintptr_t>(p.top_p) & 3) == 0 &&
+               (reinterpret_cast<uintptr_t>(p.seed) & 7) == 0 && (reinterpret_cast<uintptr_t>(p.step) & 3) == 0 &&
+               (reinterpret_cast<uintptr_t>(p.position) & 3) == 0 && (reinterpret_cast<uintptr_t>(p.token_out) & 3) == 0 &&
+               (reinterpret_cast<uintptr_t>(p.token_hist) & 3) == 0 &&
+               (reinterpret_cast<uintptr_t>(p.embed_table) & 15) == 0 && (reinterpret_cast<uintptr_t>(p.x_next) & 15) == 0,
+           "sample_finalize: misaligned pointer");
+  return 0;
+}
+
+int sample_finalize(const SampleFinalizeParams& p, cudaStream_t stream) {
+  if (int rc = sample_finalize_check(p)) return rc;
+  const int slice = slice_for(p.V, kFinCluster);
+  FinalizeArgs a{p.logits, p.inv_temperature, p.top_k, p.top_p, p.seed, p.step, p.position, p.token_out,
+                 p.token_hist, reinterpret_cast<const uint4*>(p.embed_table), reinterpret_cast<uint4*>(p.x_next),
+                 p.hidden / 8, p.V, slice};
+  auto kern = sample_finalize_kernel<kFinCluster>;
+  static PerDeviceOnce attr_once;
+  if (attr_once.first())
+    VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)sample_smem_bytes(slice_for(kSampCluster * kSampMaxSlice, kFinCluster))));
+  VB_CUDA(launch_pdl_cluster(kern, dim3(kFinCluster), dim3(kSampThreads), sample_smem_bytes(slice), stream,
+                             dim3(kFinCluster, 1, 1), a));
   return 0;
 }
 

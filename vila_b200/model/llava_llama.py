@@ -24,7 +24,7 @@ from torch import nn
 from .. import ops
 from .configuration import LlavaConfig
 from .projector import MultimodalProjector
-from .qwen2 import Qwen2ForCausalLM
+from .qwen2 import Qwen2ForCausalLM, sampling_for_generate
 from .vision import SiglipVisionTower
 
 IGNORE_INDEX = -100
@@ -667,7 +667,9 @@ class LlavaLlamaModel(nn.Module):
         Image tensors must already be normalised; PIL images go through `media.process_image`.
         response_format: xgrammar-constrained decoding (llava_arch.py:846-849).
         stream=True (serving/server.py:259-264 calls it that way): returns an iterator of text
-        chunks; the greedy decode stays on the device and is drained every few tokens."""
+        chunks; the decode stays on the device and is drained every few tokens.  Both forms sample on the
+        device when the generation config sets do_sample (its temperature, top_k, top_p and `seed`), with the
+        same ids for the same seed."""
         if stream:
             return self._generate_content_stream(prompt, generation_config, response_format)
         with torch.inference_mode():
@@ -692,7 +694,8 @@ class LlavaLlamaModel(nn.Module):
             input_ids, media, media_config = self._prepare_content(prompt)
             gc = generation_config or self.default_generation_config
             inputs_embeds, _, _ = self._embed(input_ids, media, media_config, None, None)
-        for ids in self.llm.stream_greedy(inputs_embeds[0], gc, chunk_tokens=chunk_tokens):
+        sampling = sampling_for_generate(gc, 1)[0] if getattr(gc, "do_sample", False) else None
+        for ids in self.llm.stream_tokens(inputs_embeds[0], gc, chunk_tokens=chunk_tokens, sampling=sampling):
             text = self.tokenizer.decode(ids, skip_special_tokens=True)
             if text:
                 yield text

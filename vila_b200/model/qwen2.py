@@ -22,6 +22,7 @@ import torch
 from torch import nn
 
 from .. import ops
+from ..sampling import SamplingParams, signed64
 from .configuration import Qwen2Config
 
 PAGE = 128
@@ -126,6 +127,28 @@ def unsupported_generation_options(generation_config, kwargs) -> List[str]:
         if not any(v is n or (n is not None and v == n) for n in neutral):
             bad.append(f"{name}={v!r}")
     return bad
+
+
+def sampling_for_generate(generation_config, rows: int, temperature=None, top_k=None,
+                          top_p=None) -> List[SamplingParams]:
+    """The SamplingParams of a do_sample generate, one per batch row: temperature / top_k / top_p from the
+    explicit values first, then the generation config (1.0 / 0 / 1.0 when neither sets them; HF's default
+    GenerationConfig has top_k 50).  Every row gets the config's `seed` attribute when it carries one, else a draw
+    from the host torch default generator in row order (serving.sampling_for_requests), so torch.manual_seed
+    reproduces a run.  Out-of-range values are ValueErrors."""
+    from ..serving import sampling_for_requests
+    gc = generation_config
+
+    def pick(name, given, default):
+        if given is not None:
+            return given
+        v = getattr(gc, name, None) if gc is not None else None
+        return default if v is None else v
+
+    params = SamplingParams(temperature=float(pick("temperature", temperature, 1.0)),
+                            top_k=int(pick("top_k", top_k, 0)), top_p=float(pick("top_p", top_p, 1.0)),
+                            seed=getattr(gc, "seed", None) if gc is not None else None)
+    return sampling_for_requests(params, rows)
 
 
 E4M3_MAX = 448.0
@@ -443,8 +466,8 @@ class Qwen2ForCausalLM(nn.Module):
 
     # ---- decode ----
     def set_decode_weights(self, fmt: str) -> None:
-        """Weights the single-stream greedy decoder (GraphDecoder: generate's greedy path, stream_greedy,
-        sequence-parallel greedy generate) streams per token.
+        """Weights the single-stream decoder (GraphDecoder: generate's greedy and sampled paths, stream_tokens /
+        stream_greedy, sequence-parallel greedy generate) streams per token.
           "bf16"  the parameters themselves (default); frees any FP8 copies.
           "fp8"   e4m3 copies with one fp32 scale per output row (quantize_e4m3_rows) of every layer's
                   fused qkv, o_proj, interleaved gate/up and down_proj weights and of lm_head (a tied
@@ -459,8 +482,8 @@ class Qwen2ForCausalLM(nn.Module):
         modes frees the previous ones.  The continuous-batching engine (serving.BatchedDecoder /
         generate_batch, built after this call) runs the same copies with vila_gemv_batch_fp8 /
         vila_gemv_batch_w4a16.  What stays bf16 in every mode: the prefill (prompt K/V and last hidden
-        state), the vision tower and projector, the eager sampling / logits-processor path and the embedding
-        gather.  Every call drops the cached decoder (its graphs bake in weight pointers)."""
+        state), the vision tower and projector, the eager logits-processor path and the embedding gather.
+        Every call drops the cached decoder (its graphs bake in weight pointers)."""
         if fmt not in ("bf16", "fp8", "w4a16"):
             raise ValueError(f"decode weights must be 'bf16', 'fp8' or 'w4a16', got {fmt!r}")
         if fmt == "w4a16":
@@ -493,7 +516,8 @@ class Qwen2ForCausalLM(nn.Module):
         self.decode_weights = fmt
 
     def decoder(self, max_new_tokens: int):
-        """Greedy decode engine: the CUDA graph of per-layer kernels, reused while it holds enough tokens."""
+        """Single-stream decode engine (greedy or sampled): the CUDA graphs of per-layer kernels, reused while it
+        holds enough tokens."""
         if self._decoder is None or self._decoder.max_new < max_new_tokens:
             self._decoder = GraphDecoder(self, max(max_new_tokens, 128))
         return self._decoder
@@ -505,7 +529,11 @@ class Qwen2ForCausalLM(nn.Module):
                  top_p=None, top_k=None, sp_runner=None, **kw) -> torch.Tensor:
         """HF GenerationMixin.generate(inputs_embeds=...) contract: returns ONLY the new ids
         [B, <=max_new_tokens] (pad-filled after EOS).  sp_runner: a sp.SequenceParallelPrefill ->
-        the prompt is prefilled sequence-parallel across its group (greedy, batch size 1)."""
+        the prompt is prefilled sequence-parallel across its group (greedy, batch size 1).
+        do_sample without logits_processor samples on the device in the graph decoder (temperature, top_k, top_p
+        from the kwargs, else the generation config; the rule of vila_b200/sampling.py).  Each row's seed is the
+        config's `seed` attribute when it has one, else a draw from the host torch default generator in row order
+        (torch.manual_seed reproduces a run).  With logits_processor the eager path chooses on the host."""
         gc = generation_config or self.generation_config
         refused = unsupported_generation_options(gc, kw)
         if refused:
@@ -530,6 +558,9 @@ class Qwen2ForCausalLM(nn.Module):
         pad = pick("pad_token_id", pad_token_id, eos_ids[0] if eos_ids else 0)
         if inputs_embeds.dim() == 2:
             inputs_embeds = inputs_embeds[None]
+        per_row = None
+        if sample and not logits_processor and sp_runner is None:
+            per_row = sampling_for_generate(gc, inputs_embeds.shape[0], temperature, top_k, top_p)
         outs = []
         for b in range(inputs_embeds.shape[0]):
             emb = inputs_embeds[b]
@@ -537,7 +568,9 @@ class Qwen2ForCausalLM(nn.Module):
                 emb = emb[attention_mask[b].to(torch.bool)]
             if sp_runner is not None and (sample or logits_processor or inputs_embeds.shape[0] != 1):
                 raise NotImplementedError("sequence-parallel generate: greedy decoding, batch size 1")
-            if sample or logits_processor:
+            if per_row is not None:
+                ids = self._generate_greedy(emb, max_new, eos_ids, sampling=per_row[b])
+            elif sample or logits_processor:
                 ids = self._generate_eager(emb, max_new, eos_ids, sample, logits_processor,
                                            pick("temperature", temperature, 1.0),
                                            pick("top_p", top_p, 1.0), pick("top_k", top_k, 0))
@@ -551,7 +584,9 @@ class Qwen2ForCausalLM(nn.Module):
         return res
 
     def _generate_greedy(self, emb: torch.Tensor, max_new: int, eos_ids: List[int],
-                         check_every: int = 16, sp_runner=None) -> List[int]:
+                         check_every: int = 16, sp_runner=None,
+                         sampling: Optional[SamplingParams] = None) -> List[int]:
+        """The graph decoder's loop: greedy, or sampled on the device with `sampling` (its seed set)."""
         S = emb.shape[0]
         dec = self.decoder(max_new)
         if sp_runner is not None:
@@ -573,7 +608,7 @@ class Qwen2ForCausalLM(nn.Module):
         else:
             cache = dec.cache_for(S + max_new)
             hid = self.prefill_hidden_graphed(emb, cache)
-            dec.start(hid[-1], cache)
+            dec.start(hid[-1], cache, sampling)
         done = 0
         ids: List[int] = []
         while done < max_new:
@@ -592,6 +627,14 @@ class Qwen2ForCausalLM(nn.Module):
         """Greedy decode as a generator of id chunks (serving: `generate_content(stream=True)`): the
         loop stays on the device (CUDA graph); the host drains the token history every `chunk_tokens`
         tokens, which is also where EOS is noticed."""
+        return self.stream_tokens(emb, generation_config, chunk_tokens, max_new_tokens)
+
+    def stream_tokens(self, emb: torch.Tensor, generation_config=None, chunk_tokens: int = 8,
+                      max_new_tokens: Optional[int] = None, sampling: Optional[SamplingParams] = None):
+        """stream_greedy, or with `sampling` (a SamplingParams with its seed set) the same loop sampled on the
+        device: the ids are those of generate(do_sample=True) with the same parameters and seed."""
+        if sampling is not None and not sampling.greedy and sampling.seed is None:
+            raise ValueError("stream_tokens: sampling needs a seed")
         gc = generation_config or self.generation_config
         max_new = max_new_tokens or getattr(gc, "max_new_tokens", None)
         if max_new is None:
@@ -603,7 +646,7 @@ class Qwen2ForCausalLM(nn.Module):
             dec = self.decoder(max_new)
             cache = dec.cache_for(S + max_new)
             hid = self.prefill_hidden_graphed(emb, cache)
-            dec.start(hid[-1], cache)
+            dec.start(hid[-1], cache, sampling)
             done = 0
             while done < max_new:
                 n = min(chunk_tokens, max_new - done)
@@ -655,10 +698,16 @@ class Qwen2ForCausalLM(nn.Module):
 
 
 class GraphDecoder:
-    """Greedy decode loop living entirely on the device: per token 5 launches per layer + lm_head
+    """Decode loop living entirely on the device: per token 5 launches per layer + lm_head
     GEMV(argmax) + finalize (token history, position++, next embedding gather), captured in a CUDA
     graph and replayed without host synchronisation (the reference runs ~400 launches and one D2H
     stopping-criteria sync per token, SURVEY §3.1 HOT LOOP C).
+
+    Sampled decoding (start(..., params) with non-greedy SamplingParams) runs a second graph per
+    configuration, with the same number of launches: lm_head writes the bf16 logits row and
+    vila_sample_finalize draws the token from it (the rule of vila_b200/sampling.py, t = the step counter) in
+    place of argmax_finalize.  Temperature, top-k, top-p and seed are device scalars that start() writes, so a
+    new request's parameters replay the same graph.
 
     The decoder streams the weights of the LLM's decode-weight mode at construction
     (Qwen2ForCausalLM.set_decode_weights): in "fp8" mode every GEMV of start() and of each step, lm_head
@@ -687,6 +736,13 @@ class GraphDecoder:
         self.hist = torch.zeros(max_new + 8, device=dev, dtype=torch.int32)
         self.step = torch.zeros(1, device=dev, dtype=torch.int32)
         self.position = torch.zeros(1, device=dev, dtype=torch.int32)
+        # sampled steps: the lm_head logits row and the request's parameters (device scalars read by the graph)
+        self.logits = torch.zeros(llm.lm_head.weight.shape[0], device=dev, dtype=dt)
+        self.inv_temperature = torch.zeros(1, device=dev, dtype=torch.float32)
+        self.top_k = torch.zeros(1, device=dev, dtype=torch.int32)
+        self.top_p = torch.ones(1, device=dev, dtype=torch.float32)
+        self.seed = torch.zeros(1, device=dev, dtype=torch.int64)
+        self.sampled = False  # mode of the current request (start())
         self.ws = torch.zeros(Hkv * self.MAX_SPLITS * (Hq // Hkv) * (D + 2), device=dev,
                               dtype=torch.float32)
         self.counters = torch.zeros(Hkv, device=dev, dtype=torch.int32)
@@ -696,15 +752,16 @@ class GraphDecoder:
         self.split_tokens = 0  # > 0: the long-context path is active for the current cache
         self.cache: Optional[PagedKVCache] = None
         self.graphs = {}  # (num_splits, split_tokens) -> captured CUDA graph of one decode step (for self.cache)
+        self.sampled_graphs = {}  # the same for sampled steps
 
     @property
     def graph(self):
-        return self.graphs.get((self.num_splits, self.split_tokens))
+        return (self.sampled_graphs if self.sampled else self.graphs).get((self.num_splits, self.split_tokens))
 
     @property
     def launches_per_step(self) -> int:
         """kernels of one decode step: 5 per layer (7 on the long-context path: RoPE/append, split-KV
-        attention, combine) + lm_head GEMV + finalize"""
+        attention, combine) + lm_head GEMV + finalize (argmax or sample), in either mode"""
         return (7 if self.split_tokens else 5) * self.llm.config.num_hidden_layers + 2
 
     LONG_CTX = 1024  # above: the wgmma split-KV path
@@ -738,6 +795,7 @@ class GraphDecoder:
             self.cache = self.llm.new_cache(n_tok, order)
             self._order_key = order_key
             self.graphs = {}
+            self.sampled_graphs = {}
         self.cache.length = 0
         self.num_splits, self.split_tokens = self.pick_splits(self.cache.max_tokens if tokens > self.LONG_CTX
                                                               else tokens)
@@ -765,8 +823,21 @@ class GraphDecoder:
 
     def _lm_head(self):
         cfg = self.llm.config
-        ops.gemv(self.x, norm_w=self.llm.model.norm.weight, norm_eps=cfg.rms_norm_eps, argmax_key=self.key,
-                 write_out=False, static_w=True, **self._weights(None))
+        if self.sampled:
+            ops.gemv(self.x, norm_w=self.llm.model.norm.weight, norm_eps=cfg.rms_norm_eps, out=self.logits,
+                     static_w=True, **self._weights(None))
+        else:
+            ops.gemv(self.x, norm_w=self.llm.model.norm.weight, norm_eps=cfg.rms_norm_eps, argmax_key=self.key,
+                     write_out=False, static_w=True, **self._weights(None))
+
+    def _finalize(self):
+        """the token (arg-max, or the draw in sampled mode) -> history, step++, position++, next x"""
+        emb = self.llm.model.embed_tokens.weight
+        if self.sampled:
+            ops.sample_finalize(self.logits, self.inv_temperature, self.top_k, self.top_p, self.seed, self.step,
+                                self.token, self.hist, self.position, emb, self.x)
+        else:
+            ops.argmax_finalize(self.key, self.token, self.hist, self.step, self.position, emb, self.x)
 
     def _step(self):
         llm, cfg, cache = self.llm, self.llm.config, self.cache
@@ -790,20 +861,27 @@ class GraphDecoder:
                      norm_eps=cfg.rms_norm_eps, swiglu=True, out=self.act, static_w=True, **w_gu)
             ops.gemv(self.act, residual=self.x, out=self.x, static_w=True, **w_down)
         self._lm_head()
-        ops.argmax_finalize(self.key, self.token, self.hist, self.step, self.position,
-                            llm.model.embed_tokens.weight, self.x)
+        self._finalize()
 
-    def start(self, last_hidden: torch.Tensor, cache: PagedKVCache) -> None:
-        """Seed the loop from the prefill: first new token = argmax(lm_head(norm(last_hidden)))."""
+    def start(self, last_hidden: torch.Tensor, cache: PagedKVCache, params: Optional[SamplingParams] = None) -> None:
+        """Seed the loop from the prefill: first new token = argmax(lm_head(norm(last_hidden))), or with
+        non-greedy `params` (seed set) the draw of token index 0 from those logits; the following steps
+        run the matching graph.  params None or greedy: exactly the greedy path."""
         assert cache is self.cache
-        llm = self.llm
+        self.sampled = params is not None and not params.greedy
+        if self.sampled:
+            if params.seed is None:
+                raise ValueError("GraphDecoder.start: sampling needs a seed (serving.sampling_for_requests draws one)")
+            self.inv_temperature.fill_(params.inv_temperature)
+            self.top_k.fill_(min(params.top_k, 2 ** 31 - 1))
+            self.top_p.fill_(params.top_p)
+            self.seed.fill_(signed64(params.seed))
         self.step.zero_()
         self.key.zero_()
         self.position.fill_(cache.length - 1)  # finalize increments -> position of the new token
         self.x.copy_(last_hidden)
         self._lm_head()
-        ops.argmax_finalize(self.key, self.token, self.hist, self.step, self.position,
-                            llm.model.embed_tokens.weight, self.x)
+        self._finalize()
         self._started = 1
 
     def run(self, n_tokens: int) -> None:
@@ -814,13 +892,14 @@ class GraphDecoder:
             self._started = 2
         if n <= 0:
             return
-        g = self.graphs.get((self.num_splits, self.split_tokens))
+        graphs = self.sampled_graphs if self.sampled else self.graphs
+        g = graphs.get((self.num_splits, self.split_tokens))
         if g is None:
             # warm-up launch outside capture is not allowed to change state: capture directly
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
                 self._step()
-            self.graphs[(self.num_splits, self.split_tokens)] = g
+            graphs[(self.num_splits, self.split_tokens)] = g
         for _ in range(n):
             g.replay()
         self.cache.length += n

@@ -12,7 +12,7 @@ import torch
 
 from . import _lib
 from ._lib import (DecodeAttnFp8Params, DecodeAttnParams, DecodeAttnSplitParams, FmhaParams, GemvBatchParams,
-                   GemvParams, SampleParams, check)
+                   GemvParams, SampleFinalizeParams, SampleParams, check)
 
 ACT_NONE, ACT_GELU_TANH, ACT_GELU_ERF, ACT_SILU = 0, 1, 2, 3
 
@@ -660,3 +660,44 @@ def sample_batch(logits: torch.Tensor, inv_temperature: torch.Tensor, top_k: tor
     p.M, p.V = M, V
     check(_lib.load().vila_sample_batch(C.byref(p), _stream()), "vila_sample_batch")
     return out
+
+
+def sample_finalize(logits: torch.Tensor, inv_temperature: torch.Tensor, top_k: torch.Tensor, top_p: torch.Tensor,
+                    seed: torch.Tensor, step: torch.Tensor, token_out: torch.Tensor, token_hist=None, position=None,
+                    embed_table=None, x_next=None) -> None:
+    """The single-stream decoder's end of a sampled step (vila_sample_finalize, one launch): the token of the bf16
+    logits row [V] drawn by the rule of vila_b200/sampling.py with the device scalars inv_temperature fp32,
+    top_k int32, top_p fp32 and seed int64 at token index t = step (int32 [1]); bit-identical to sample_batch with
+    M = 1.  Then token_out (int32 [1]) = token, token_hist[t] = token (int32, optional), step + 1, position + 1
+    (int32 [1], optional) and x_next = embed_table[token] (bf16 [*, hidden] and [hidden], optional, together)."""
+    _need(logits.dim() == 1 and logits.is_contiguous() and 1 <= logits.numel() <= SAMPLE_MAX_VOCAB,
+          f"sample_finalize: logits must be a contiguous [V] row with V in 1..{SAMPLE_MAX_VOCAB}, got "
+          f"{tuple(logits.shape)}")
+    _need((embed_table is None) == (x_next is None), "sample_finalize: embed_table and x_next go together")
+    arrays = [(logits, "logits", torch.bfloat16), (inv_temperature, "inv_temperature", torch.float32),
+              (top_k, "top_k", torch.int32), (top_p, "top_p", torch.float32), (seed, "seed", torch.int64),
+              (step, "step", torch.int32), (token_out, "token_out", torch.int32)]
+    for t, name, dt in ((position, "position", torch.int32), (token_hist, "token_hist", torch.int32),
+                        (embed_table, "embed_table", torch.bfloat16), (x_next, "x_next", torch.bfloat16)):
+        if t is not None:
+            arrays.append((t, name, dt))
+    for t, name, dt in arrays:
+        _need(t.dtype == dt, f"sample_finalize: {name} must be {dt}, got {t.dtype}")
+        if name in ("inv_temperature", "top_k", "top_p", "seed", "step", "token_out", "position"):
+            _need(t.numel() == 1, f"sample_finalize: {name} must be a single value, got {tuple(t.shape)}")
+    hidden = 0
+    if embed_table is not None:
+        hidden = embed_table.shape[-1]
+        _need(embed_table.dim() == 2 and embed_table.is_contiguous() and x_next.numel() == hidden
+              and x_next.is_contiguous(),
+              f"sample_finalize: embed_table must be a contiguous [*, hidden] table and x_next a contiguous [hidden] "
+              f"vector, got {tuple(embed_table.shape)} and {tuple(x_next.shape)}")
+    for t, name, _ in arrays:
+        _chk(t, name, t.dtype)
+    p = SampleFinalizeParams()
+    p.logits, p.inv_temperature, p.top_k, p.top_p, p.seed = (_p(logits), _p(inv_temperature), _p(top_k), _p(top_p),
+                                                             _p(seed))
+    p.step, p.position, p.token_out, p.token_hist = _p(step), _p(position), _p(token_out), _p(token_hist)
+    p.embed_table, p.x_next = _p(embed_table), _p(x_next)
+    p.V, p.hidden = logits.numel(), hidden
+    check(_lib.load().vila_sample_finalize(C.byref(p), _stream()), "vila_sample_finalize")

@@ -5,9 +5,10 @@ Mirrors the request / response shapes of the reference's `serving/server.py` (`C
 `stream` is set, one `chat.completion` object otherwise) on top of `generate_content(prompt, stream=...)`.
 The reference serialises requests with a global lock; here non-streaming requests that arrive while the
 engine is busy are grouped (up to `slots`) and decoded together by `LlavaLlamaModel.generate_batch`
-(continuous batching over the shared paged pool, vila_b200/serving.py).  With --sample every non-streaming
-request goes through generate_batch with its own temperature, top_p and seed, drawn on the device; streaming
-requests stay on the single-stream greedy decoder.
+(continuous batching over the shared paged pool, vila_b200/serving.py).  With --sample every request is sampled
+on the device with its own temperature, top_p and seed: non-streaming ones through generate_batch, streaming ones
+on the single-stream graph decoder (generate_content(stream=True) with a sampling generation config).  Without it
+every request is decoded greedily.
 
     python -m vila_b200.server --model-path <dir> --port 8000
 """
@@ -16,6 +17,7 @@ from __future__ import annotations
 import argparse
 import asyncio
 import base64
+import copy
 import json
 import re
 import time
@@ -148,7 +150,7 @@ class Engine:
         self.kv_cache = kv_cache
         if sample and not hasattr(model, "generate_batch"):
             raise ValueError("sample=True needs a model with generate_batch (the batched engine draws the tokens)")
-        self.sample = sample  # non-streaming requests: sampled on the batched engine with their own parameters
+        self.sample = sample  # every request sampled with its own parameters (batched engine / graph decoder)
         self.lock = asyncio.Lock()
         self.pending: List[Any] = []
 
@@ -209,13 +211,26 @@ class Engine:
         return SamplingParams(temperature=float(req.temperature or 0.0),
                               top_p=float(req.top_p) if req.top_p is not None else 1.0, seed=req.seed)
 
+    def _stream_config(self, req: ChatCompletionRequest):
+        """a streamed request's generation config: a copy of the model's default with the request's max_tokens,
+        and do_sample set explicitly: with --sample the request's temperature, top_p (top_k 0) and seed, else
+        greedy whatever the checkpoint's config says.  Bad values raise."""
+        gc = copy.copy(self.model.default_generation_config)
+        gc.max_new_tokens = req.max_tokens
+        gc.do_sample = False
+        if self.sample:
+            p = self._sampling(req)
+            gc.do_sample = not p.greedy
+            gc.temperature, gc.top_k, gc.top_p, gc.seed = p.temperature, 0, p.top_p, p.seed
+        return gc
+
     async def stream(self, req: ChatCompletionRequest):
         if req.model != self.model_name:
             raise ValueError(f"The endpoint is configured to use the model {self.model_name}, "
                              f"but the request model is {req.model}")
+        gc = self._stream_config(req)  # a bad value fails this request before it takes the lock
         async with self.lock:
-            gen = self.model.generate_content(build_prompt(req.messages), generation_config=self._gen_config(req),
-                                              stream=True)
+            gen = self.model.generate_content(build_prompt(req.messages), generation_config=gc, stream=True)
             for chunk_id, new_text in enumerate(gen):
                 if len(new_text):
                     chunk = {"id": str(chunk_id), "object": "chat.completion.chunk", "created": int(time.time()),
@@ -240,6 +255,7 @@ def create_app(model, model_name: str, slots: int = 8, kv_cache: str = "bf16", s
     async def chat_completions(request: ChatCompletionRequest):
         try:
             if request.stream:
+                engine._stream_config(request)  # bad sampling values: this request's error, before streaming starts
                 return StreamingResponse(engine.stream(request), media_type="text/event-stream")
             return await engine.complete(request)
         except Exception as e:  # the reference answers 500 with the message (server.py:302-306)
@@ -266,10 +282,10 @@ def main() -> None:
                     help="K/V format of the engine that batches queued requests (fp8: e4m3 with one fp32 scale "
                          "per token and KV head, about half the bytes; the single-stream decoder stays bf16)")
     ap.add_argument("--sample", action="store_true",
-                    help="sample non-streaming requests with their own temperature, top_p and seed on the batched "
-                         "engine (vila_sample_batch, on the device), even a request that arrives alone; without it "
-                         "every request is decoded greedily.  Streaming requests stay on the single-stream greedy "
-                         "decoder either way")
+                    help="sample every request with its own temperature, top_p and seed on the device: "
+                         "non-streaming requests on the batched engine (vila_sample_batch), even one that arrives "
+                         "alone, streaming requests on the single-stream graph decoder (vila_sample_finalize); "
+                         "without it every request is decoded greedily")
     args = ap.parse_args()
     model = llava.load(args.model_path, decode_weights=args.decode_weights)
     uvicorn.run(create_app(model, get_model_name_from_path(args.model_path), args.slots, args.kv_cache, args.sample),
