@@ -420,6 +420,164 @@ def attention_inputs(family: str, q_pos: torch.Tensor, key_pos: torch.Tensor, Hq
     return q.to(torch.bfloat16), k.to(torch.bfloat16), v.to(torch.bfloat16)
 
 
+# ------------------------------------------------------------------------------------------------
+# decode attention: one new token at position pos over the keys 0..pos (Sq = 1, non-causal)
+# ------------------------------------------------------------------------------------------------
+DECODE_FAMILIES = ("random", "sink", "leak")
+LEAK_EDGE = 6.0      # leak: score of an edge key above the rest
+LEAK_GARBAGE = 30.0  # leak: score of every garbage slot (>= 16 above every visible key)
+LEAK_Q = 4.0         # leak: the query heads' shared component along u (rotated space)
+
+
+class DecodeInputs:
+    """One decode step's inputs (decode_attention_inputs); every tensor bf16 on the device.
+      qkv     [(Hq + 2 Hkv) D]  the projection row before RoPE: q, k_new, v_new
+      q       [Hq, D]           q after RoPE at pos (HF's bf16 op order), what the reference uses
+      k_new   [Hkv, D]          k_new after RoPE: the K row the kernel must append at pos
+      v_new   [Hkv, D]          the V row it must append (not rotated)
+      k_hist, v_hist [pos, Hkv, D]  the cached keys 0..pos-1 as prefill leaves them (after RoPE)
+      k_garbage [Hkv, D]        K of every slot no query may see; its V is SENTINEL_V"""
+
+    def __init__(self, **kw):
+        self.__dict__.update(kw)
+
+    def keys(self):
+        """K and V of the keys 0..pos in token order: the reference's inputs"""
+        return torch.cat([self.k_hist, self.k_new[None]]), torch.cat([self.v_hist, self.v_new[None]])
+
+
+def _rope_pair(pos: int, D: int, theta: float = 1e6):
+    """bf16 cos / sin of position pos, [1, D] on the CPU: O.rope_cos_sin (what the kernels' sincosf matches)"""
+    return O.rope_cos_sin(torch.tensor([pos]), D, theta, torch.bfloat16)
+
+
+def rope_rotate(x: torch.Tensor, pos: int) -> torch.Tensor:
+    """x [H, D] bf16 rotated to position pos in HF's bf16 op order (O.apply_rope)"""
+    cos, sin = _rope_pair(pos, x.shape[-1])
+    r, _ = O.apply_rope(x.cpu()[:, None], x.cpu()[:, None], cos, sin)
+    return r[:, 0].to(x.device)
+
+
+def _rope_preimage(y: torch.Tensor, pos: int) -> torch.Tensor:
+    """bf16 x whose rotation to pos is close to y (fp32 [H, D]): the inverse rotation in fp64, rounded"""
+    D = y.shape[-1]
+    inv = O.rope_inv_freq(D, 1e6).double()
+    ang = torch.tensor(float(pos), dtype=torch.float32).double() * inv
+    c, s = ang.cos(), ang.sin()
+    y = y.double().cpu()
+    y0, y1 = y[:, :D // 2], y[:, D // 2:]
+    return torch.cat([y0 * c + y1 * s, -y0 * s + y1 * c], dim=1).to(torch.bfloat16)
+
+
+def decode_edges(pos: int, chunks) -> torch.Tensor:
+    """bool [pos + 1]: the keys at the edges of every chunk size in `chunks` (pages, splits), pos - 1 and pos"""
+    t = torch.arange(pos + 1)
+    e = (t == pos) | (t == pos - 1)
+    for c in chunks:
+        e |= (t % c == 0) | (t % c == c - 1)
+    return e
+
+
+def decode_attention_inputs(family: str, pos: int, Hq: int, Hkv: int, D: int, scale: float, seed: int, *,
+                            chunks=(128,), device="cpu") -> DecodeInputs:
+    """The inputs of one decode step at position pos (the new token; keys 0..pos-1 are cached).  q and the
+    new k are drawn after RoPE and mapped back to a bf16 pre-RoPE row, so every family's score pattern holds
+    for the rotated values the kernels see; the history is drawn directly as cached (after RoPE).
+      random: scores with standard deviation ~1; three V channels 16x larger.
+      sink:   key 0 scores ~12 above the rest, which have standard deviation ~3.
+      leak:   the G query heads of a KV group share a component LEAK_Q u (u a unit vector per KV head, the
+              rest of q orthogonal to it); visible keys score with deviation ~0.3, and the edge keys (the
+              new token, pos - 1, the first and last key of every chunk size in `chunks`) LEAK_EDGE above;
+              k_garbage = c u scores LEAK_GARBAGE for every head.  u depends on the shape only, so the
+              slots of one pool share k_garbage (random / sink: any slot's k_garbage will do).  Attending a garbage slot changes the
+              output by O(SENTINEL_V); dropping or double-counting one edge key by O(|v| / edge keys)."""
+    G = Hq // Hkv
+    g = torch.Generator(device=device).manual_seed(seed)
+    gc = torch.Generator().manual_seed(seed)
+    n = pos + 1
+    v = torch.randn(n, Hkv, D, device=device, generator=g)
+    if family == "random":
+        qr = torch.randn(Hq, D, generator=gc)
+        k = torch.randn(n, Hkv, D, device=device, generator=g) / (scale * math.sqrt(D))
+        kg = torch.randn(Hkv, D, generator=gc) / (scale * math.sqrt(D))
+        v[:, :, [3, D // 2, D - 5]] *= 16.0
+    elif family == "sink":
+        sd = math.sqrt(3.0 / (scale * math.sqrt(D - 1)))
+        qr = torch.randn(Hq, D, generator=gc) * sd
+        k = torch.randn(n, Hkv, D, device=device, generator=g) * sd
+        kg = torch.randn(Hkv, D, generator=gc) * sd
+        qr[:, 0] = 4.0
+        k[:, :, 0] = 0.0
+        kg[:, 0] = 0.0
+        k[0, :, 0] = 12.0 / (4.0 * scale)
+    elif family == "leak":
+        u = torch.randn(Hkv, D, generator=torch.Generator().manual_seed(Hkv * D))  # one per shape: slots
+        u /= u.norm(dim=1, keepdim=True)  # sharing a pool share k_garbage
+        nq = torch.randn(Hq, D, generator=gc)
+        uq = u.repeat_interleave(G, dim=0)
+        nq -= (nq * uq).sum(dim=1, keepdim=True) * uq
+        qr = LEAK_Q * uq + nq
+        sd = 0.3 / (scale * math.sqrt(D))
+        k = torch.randn(n, Hkv, D, device=device, generator=g) * sd
+        ud = u.to(device)
+        k -= (k * ud).sum(dim=-1, keepdim=True) * ud
+        edge = decode_edges(pos, chunks).to(device)
+        k[edge] += (LEAK_EDGE / (scale * LEAK_Q)) * ud
+        kg = (LEAK_GARBAGE / (scale * LEAK_Q)) * u
+    else:
+        raise ValueError(family)
+    q_pre = _rope_preimage(qr, pos)
+    k_pre = _rope_preimage(k[pos].float().cpu(), pos)
+    q = rope_rotate(q_pre, pos)
+    k_new = rope_rotate(k_pre, pos)
+    v = v.to(torch.bfloat16)
+    qkv = torch.cat([q_pre.reshape(-1), k_pre.reshape(-1), v[pos].cpu().reshape(-1)]).to(device)
+    inp = DecodeInputs(qkv=qkv, q=q.to(device), k_new=k_new.to(device), v_new=v[pos].clone(),
+                       k_hist=k[:pos].to(torch.bfloat16), v_hist=v[:pos], k_garbage=kg.to(torch.bfloat16).to(device),
+                       pos=pos, family=family)
+    if family == "leak":  # the family's promise, on the values the kernels see
+        kq = inp.keys()[0].double()
+        hk = torch.arange(Hq, device=device) // G
+        s = scale * torch.einsum("hd,thd->ht", q.double().to(device), kq[:, hk])
+        sg = scale * (q.double().to(device) * inp.k_garbage.double()[hk]).sum(dim=1)
+        assert bool((sg >= s.amax(dim=1) + 16.0).all()), "leak: a garbage slot scores too close to a visible key"
+    return inp
+
+
+# The fp8 decode kernel rounds p * vscale once per (token, KV head): that rounding is shared by the G * 128
+# outputs of the group, so when a few keys carry a row the group's outputs move together and the mean signed
+# error is a mean of a few shifts, not of independent roundings (tests/test_decode_attention_cpu.py::
+# test_fp8_sink_bias_is_one_shared_rounding).  Its rounding bias is checked only over contexts of at least this
+# many keys and away from the sink family; the element and row checks apply everywhere.
+FP8_BIAS_MIN_KEYS = 128
+
+
+def check_decode_attention(name: str, got: torch.Tensor, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor,
+                           scale: float, bias: bool = True) -> AttnErrors:
+    """AttnErrors of one decode output got [Hq, D] against the fp64 reference over the keys k, v [pos + 1, Hkv,
+    D] (non-causal) for the rotated q [Hq, D]; recorded like report_rel and asserted (bias False: the element
+    and row checks only)."""
+    e = attention_errors(got.reshape(1, *q.shape[-2:]), q.reshape(1, *q.shape[-2:]), k, v, causal=False,
+                         scale=scale)
+    _record({"name": name, "bias_checked": bias, **e.summary()})
+    bad = [f for f in e.failures() if bias or not f.startswith("rounding bias")]
+    assert not bad, f"{name}: " + "; ".join(bad)
+    return e
+
+
+def scatter_tokens(pool: torch.Tensor, pages, rows: torch.Tensor) -> None:
+    """rows [n, ...] (token t of a sequence) into pool [P, 128, ...] at page pages[t // 128], row t % 128"""
+    n = rows.shape[0]
+    if n == 0:
+        return
+    pages = torch.as_tensor(pages, device=pool.device).long()
+    full = n // 128
+    if full:
+        pool[pages[:full]] = rows[:full * 128].reshape(full, 128, *rows.shape[1:]).to(pool.dtype)
+    if n % 128:
+        pool[pages[full], :n % 128] = rows[full * 128:].to(pool.dtype)
+
+
 def greedy_ids_match(got: List[int], oracle_ids: List[int], oracle_logits: torch.Tensor,
                      margin: float) -> None:
     """Greedy token ids must be identical, except that the comparison stops at the first step where

@@ -4,8 +4,8 @@ import pytest
 import torch
 
 from oracle import vila_oracle as O
-from tests.helpers import greedy_ids_match, oracle_from_state_dict, report_rel
-from tests.test_kernels_gpu import _ops, bf, ref_attention
+from tests.helpers import check_decode_attention, greedy_ids_match, oracle_from_state_dict
+from tests.test_kernels_gpu import _ops, bf
 
 pytestmark = pytest.mark.gpu
 
@@ -95,8 +95,8 @@ def test_decode_attention_split_batch(cuda, Hq, Hkv):
         v_hist = v_pool0[pt[b, t // 128].long(), t % 128]
         k_all = torch.cat([k_hist, kr.transpose(0, 1)], 0).float()
         v_all = torch.cat([v_hist, vn], 0).float()
-        ref = ref_attention(qr.transpose(0, 1)[None].float(), k_all[None], v_all[None], True, D ** -0.5)[0, 0]
-        report_rel(f"decode_attention_split_batch Hq={Hq} ctx={p}", out_buf[b, :Hq * D].view(Hq, D), ref, 1.5e-2)
+        check_decode_attention(f"decode_attention_split_batch Hq={Hq} ctx={p}", out_buf[b, :Hq * D].view(Hq, D),
+                               qr.transpose(0, 1), k_all, v_all, D ** -0.5)
         # bit-identical to the single-sequence kernel with counters and the same split configuration
         kp1, vp1 = k_pool0.clone(), v_pool0.clone()
         out1 = torch.zeros(Hq * D, dtype=torch.bfloat16, device=cuda)

@@ -22,8 +22,8 @@ import pytest
 import torch
 
 from oracle import vila_oracle as O
-from tests.helpers import check_close, oracle_from_state_dict, report_rel
-from tests.test_kernels_gpu import _ops, bf, ref_attention
+from tests.helpers import check_close, check_decode_attention, oracle_from_state_dict
+from tests.test_kernels_gpu import _ops, bf
 
 pytestmark = pytest.mark.gpu
 
@@ -305,8 +305,8 @@ def test_decode_attention_batch(cuda, Hq, Hkv):
         t = torch.arange(p, device=cuda)
         k_all = torch.cat([k0[pt[b, t // PAGE].long(), t % PAGE], kr.transpose(0, 1)], 0).float()
         v_all = torch.cat([v0[pt[b, t // PAGE].long(), t % PAGE], vn], 0).float()
-        ref = ref_attention(qr.transpose(0, 1)[None].float(), k_all[None], v_all[None], True, D ** -0.5)[0, 0]
-        report_rel(f"decode_attention_batch Hq={Hq} Hkv={Hkv} ctx={p}", out[b, :Hq * D].view(Hq, D), ref, 1.5e-2)
+        check_decode_attention(f"decode_attention_batch Hq={Hq} Hkv={Hkv} ctx={p}", out[b, :Hq * D].view(Hq, D),
+                               qr.transpose(0, 1), k_all, v_all, D ** -0.5)
         if p <= 1023:  # the single-sequence entry point runs the same kernel template (8-page rows)
             kp1, vp1 = k0.clone(), v0.clone()
             out1 = torch.zeros(Hq * D, dtype=torch.bfloat16, device=cuda)

@@ -556,7 +556,7 @@ _DECODE_GQA_CASES = [(ctx, s, hq, hkv) for hq, hkv in ((28, 4), (16, 2), (4, 2))
 def test_decode_attention(cuda, ctx, splits, Hq, Hkv):
     """(16448, *) / (65814, *): decode right after a 64-frame / 256-frame video prefill (README.md:69-70
     publishes decode throughput for exactly that), splits as GraphDecoder.pick_splits chooses them."""
-    from tests.helpers import report_rel
+    from tests.helpers import check_decode_attention
     ops = _ops()
     D = 128
     g = torch.Generator(device="cuda").manual_seed(ctx + splits)
@@ -590,8 +590,8 @@ def test_decode_attention(cuda, ctx, splits, Hq, Hkv):
     qr, kr = O.apply_rope(q, kn, cos.to(cuda), sin.to(cuda))
     k_all = torch.cat([k_hist, kr.transpose(0, 1)], 0)
     v_all = torch.cat([v_hist, vn], 0)
-    ref = ref_attention(qr.transpose(0, 1)[None], k_all[None], v_all[None], True, D ** -0.5)[0, 0]
-    report_rel(f"decode_attention Hq={Hq} Hkv={Hkv} ctx={ctx} splits={splits}", out.view(Hq, D), ref, 1.5e-2)
+    check_decode_attention(f"decode_attention Hq={Hq} Hkv={Hkv} ctx={ctx} splits={splits}", out.view(Hq, D),
+                           qr.transpose(0, 1), k_all, v_all, D ** -0.5)
     # KV append happened
     assert torch.equal(k_pool[perm[ctx // 128], ctx % 128], kr.transpose(0, 1)[0])
     assert torch.equal(v_pool[perm[ctx // 128], ctx % 128], vn[0])
@@ -636,7 +636,7 @@ def test_preprocess_tiles_bit_exact_vs_pil(cuda, w, h, mode):
 def test_decode_attention_split_long_context(cuda, ctx, splits, split_tokens):
     """vila_decode_attention_split (RoPE + append, wgmma FMHA in split-KV mode, combine) vs fp32
     attention over the whole context; (1000, 37, 512): most splits are empty."""
-    from tests.helpers import report_rel
+    from tests.helpers import check_decode_attention, report_rel
     ops = _ops()
     Hq, Hkv, D = 28, 4, 128
     assert splits * split_tokens >= ctx + 1
@@ -681,7 +681,8 @@ def test_decode_attention_split_long_context(cuda, ctx, splits, split_tokens):
     k_all = torch.cat([k_hist, kr.transpose(0, 1)], 0)
     v_all = torch.cat([v_hist, vn], 0)
     ref = ref_attention(qr.transpose(0, 1)[None], k_all[None], v_all[None], True, D ** -0.5)[0, 0]
-    report_rel(f"decode_attention_split ctx={ctx} splits={splits}", out.view(Hq, D), ref, 1.5e-2)
+    check_decode_attention(f"decode_attention_split ctx={ctx} splits={splits}", out.view(Hq, D), qr.transpose(0, 1),
+                           k_all, v_all, D ** -0.5)
     assert torch.equal(k_pool[perm[ctx // 128], ctx % 128], kr.transpose(0, 1)[0])
     assert torch.equal(v_pool[perm[ctx // 128], ctx % 128], vn[0])
     # the SIMT split kernel on the same problem agrees (both within bf16 noise of the fp32 reference)

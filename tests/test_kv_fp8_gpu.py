@@ -23,10 +23,10 @@ import torch.nn.functional as F
 from oracle import vila_oracle as O
 from tests import test_fp8_decode_gpu as T8
 from tests import test_w4a16_decode_gpu as T4
-from tests.helpers import _record, report_rel
+from tests.helpers import FP8_BIAS_MIN_KEYS, _record, check_decode_attention
 from tests.test_decode_engines_gpu import _fp32_truth  # noqa: F401  (autouse: the fp32 oracle is really fp32)
 from tests.test_decode_engines_gpu import _check_untouched, _decoded_rows, _prompt
-from tests.test_kernels_gpu import _ops, bf, ref_attention
+from tests.test_kernels_gpu import _ops, bf
 
 pytestmark = pytest.mark.gpu
 
@@ -181,8 +181,8 @@ def test_decode_attention_fp8_batch(cuda, Hq, Hkv):
         q = qkv0[b, :Hq * D].view(1, Hq, D).transpose(0, 1)
         cos, sin = O.rope_cos_sin(torch.tensor([p]), D, 1e6, torch.bfloat16)
         qr, _ = O.apply_rope(q, q[:Hkv], cos.to(cuda), sin.to(cuda))
-        ref = ref_attention(qr.transpose(0, 1)[None].float(), k_all[None], v_all[None], True, D ** -0.5)[0, 0]
-        report_rel(f"decode_attention_fp8_batch Hq={Hq} Hkv={Hkv} ctx={p}", out[b, :Hq * D].view(Hq, D), ref, 1.5e-2)
+        check_decode_attention(f"decode_attention_fp8_batch Hq={Hq} Hkv={Hkv} ctx={p}", out[b, :Hq * D].view(Hq, D),
+                               qr.transpose(0, 1), k_all, v_all, D ** -0.5, bias=p + 1 >= FP8_BIAS_MIN_KEYS)
     assert torch.equal(_u8(kp), touched[0]) and torch.equal(ks, touched[1])    # every other pool byte unchanged
     assert torch.equal(_u8(vp), touched[2]) and torch.equal(vs, touched[3])
 
