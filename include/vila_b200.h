@@ -419,6 +419,22 @@ typedef struct vila_sample_finalize_params {
 } vila_sample_finalize_params;
 int vila_sample_finalize(const vila_sample_finalize_params* p, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * vila_prefix_block_hash — a 128-bit digest of every full 128-row block of a bf16 matrix x [rows, cols] (row
+ * stride ld elements), for prefix caching in the continuous-batching engine: out [rows / 128][2] (uint64).  The
+ * reference has no counterpart: it prefills every request in full (serving/server.py:65-73, llava_arch.py:823-833).
+ * The rule (vila_b200/prefix_cache.py states it in numpy), for block b and lane L in {0, 1}:
+ *   w_j   the j-th 8-byte little-endian word of rows [128b, 128b + 128), read row-major over the cols logical
+ *         columns (the ld padding is not read)
+ *   d_L = sum_j fmix64(fmix64(w_j ^ key_L) + j * 0x9E3779B97F4A7C15) mod 2^64, fmix64 the murmur3 finalizer
+ * Rows past the last full block are not hashed and out is not written past [rows / 128].  Not cryptographic: pick
+ * the keys at random so that colliding blocks cannot be prepared in advance.  cols a multiple of 4, ld a multiple
+ * of 4 and >= cols, x and out 8-byte aligned; the argument errors are reported before any device call.  One CTA
+ * per block, PDL.
+ * ------------------------------------------------------------------------------------------- */
+int vila_prefix_block_hash(const void* x, int64_t ld, int64_t rows, int64_t cols, uint64_t key0, uint64_t key1,
+                           uint64_t* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

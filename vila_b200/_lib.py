@@ -139,6 +139,7 @@ SIGNATURES = {
     "vila_decode_attention_fp8_batch": [C.POINTER(DecodeAttnFp8Params), c_void_p],
     "vila_sample_batch": [C.POINTER(SampleParams), c_void_p],
     "vila_sample_finalize": [C.POINTER(SampleFinalizeParams), c_void_p],
+    "vila_prefix_block_hash": [c_void_p, c_i64, c_i64, c_i64, C.c_uint64, C.c_uint64, c_void_p, c_void_p],
 }
 _RESTYPES = {"vila_last_error": C.c_char_p}
 

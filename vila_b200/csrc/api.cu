@@ -447,4 +447,13 @@ int vila_sample_finalize(const vila_sample_finalize_params* p, void* stream) {
   return vb::sample_finalize(d, st(stream));
 }
 
+// the reference prefills every request in full (serving/server.py:65-73, llava_arch.py:823-833): no seam
+int vila_prefix_block_hash(const void* x, int64_t ld, int64_t rows, int64_t cols, uint64_t key0, uint64_t key1,
+                           uint64_t* out, void* stream) {
+  if (int rc = vb::prefix_block_hash_check(x, ld, rows, cols, out)) return rc;
+  if (rows < 128) return 0;
+  VB_REQUIRE_DEVICE();
+  return vb::prefix_block_hash(x, ld, rows, cols, key0, key1, out, st(stream));
+}
+
 }  // extern "C"

@@ -269,4 +269,12 @@ struct SampleFinalizeParams {
 int sample_finalize_check(const SampleFinalizeParams& p);  // the argument errors, before any device call
 int sample_finalize(const SampleFinalizeParams& p, cudaStream_t stream);
 
+// ---- block digests for prefix caching in the batched engine (prefix_hash.cu) ----------------------------
+// out[b] = (d_0, d_1) of every full 128-row block b of x [rows, cols] bf16 (row stride ld elements); the rule is
+// vila_b200/prefix_cache.py's.  The check reports the argument errors before any device call.
+int prefix_block_hash_check(const void* x, int64_t ld, int64_t rows, int64_t cols, const uint64_t* out);
+int prefix_block_hash(const void* x, int64_t ld, int64_t rows, int64_t cols, uint64_t key0, uint64_t key1,
+                      uint64_t* out, cudaStream_t stream);
+
+
 }  // namespace vb

@@ -14,6 +14,7 @@ llava_arch.py:463,470); dynamic-S2 stitching is one kernel per image.
 from __future__ import annotations
 
 import copy
+import gc
 from collections import defaultdict, deque
 from types import SimpleNamespace
 from typing import Any, Dict, List, Optional, Sequence, Tuple, Union
@@ -585,7 +586,7 @@ class LlavaLlamaModel(nn.Module):
     @torch.inference_mode()
     def generate_batch(self, requests: List[Dict[str, Any]], max_new_tokens: int = 128, slots: int = 8,
                        max_tokens_per_slot: Optional[int] = None, eos_token_id=None,
-                       kv_cache: str = "bf16", sampling=None) -> List[List[int]]:
+                       kv_cache: str = "bf16", sampling=None, prefix_cache: bool = False) -> List[List[int]]:
         """Serve several independent requests with continuous batching over one shared paged KV pool
         (vila_b200/serving.py; the reference's servers run them one at a time, serving/server.py:65-73).
         requests: dicts with the `generate` arguments (`input_ids` [1, T], `media`, `media_config`).
@@ -593,8 +594,16 @@ class LlavaLlamaModel(nn.Module):
         request needs more, e.g. video or dynamic-S2 prompts).
         kv_cache: "bf16" (default) or "fp8" (e4m3 K/V with one fp32 scale per token and KV head, serving.py).
         sampling: None (default) decodes greedily; a serving.SamplingParams, or a list with one per request,
-        samples on the device (serving.generate_batch).  Returns the new ids of every request in order."""
-        from ..serving import generate_batch
+        samples on the device (serving.generate_batch).
+        prefix_cache: True shares the K/V pages of the full 128-token prompt blocks that requests start with (the
+        same video or image, one system prompt), and needs max_tokens_per_slot.  The model keeps the engine it
+        builds (max_new = max_tokens_per_slot), and with it the cached blocks, for later calls with the same slots,
+        max_tokens_per_slot, decode-weight mode, kv_cache and sampling (greedy or not); any other call rebuilds it.
+        Returns the new ids of every request in order."""
+        from ..serving import BatchedDecoder, generate_batch
+        if prefix_cache and max_tokens_per_slot is None:
+            raise ValueError("generate_batch(prefix_cache=True) needs max_tokens_per_slot: the engine and its cached "
+                             "blocks are kept between calls, so its slot size cannot follow the requests")
         prompts = []
         for r in requests:
             emb, _, mask = self._embed(r["input_ids"], r.get("media"), r.get("media_config"), None,
@@ -602,8 +611,22 @@ class LlavaLlamaModel(nn.Module):
             prompts.append(emb[0][mask[0]] if mask is not None else emb[0])
         eos = self.tokenizer.stop_token_ids if eos_token_id is None else (
             [eos_token_id] if isinstance(eos_token_id, int) else list(eos_token_id))
+        decoder = None
+        if prefix_cache:
+            key = (slots, max_tokens_per_slot, getattr(self.llm, "decode_weights", "bf16"), kv_cache,
+                   sampling is not None)
+            kept = getattr(self, "_prefix_engine", None)
+            if kept is None or kept[0] != key:
+                if kept is not None:  # free the old pool and its graphs before the new ones are allocated
+                    kept = self._prefix_engine = None
+                    gc.collect()
+                kept = (key, BatchedDecoder(self.llm, slots, max_tokens_per_slot, max_new=max_tokens_per_slot,
+                                            kv_cache=kv_cache, sampling=sampling is not None, prefix_cache=True))
+                self._prefix_engine = kept
+            decoder = kept[1]
         return generate_batch(self.llm, prompts, max_new_tokens, eos, slots=slots,
-                              max_tokens_per_slot=max_tokens_per_slot, kv_cache=kv_cache, sampling=sampling)
+                              max_tokens_per_slot=max_tokens_per_slot, decoder=decoder, kv_cache=kv_cache,
+                              sampling=sampling, prefix_cache=prefix_cache)
 
     @property
     def default_generation_config(self):

@@ -701,3 +701,21 @@ def sample_finalize(logits: torch.Tensor, inv_temperature: torch.Tensor, top_k: 
     p.embed_table, p.x_next = _p(embed_table), _p(x_next)
     p.V, p.hidden = logits.numel(), hidden
     check(_lib.load().vila_sample_finalize(C.byref(p), _stream()), "vila_sample_finalize")
+
+
+def prefix_block_hash(x: torch.Tensor, key0: int, key1: int) -> torch.Tensor:
+    """The 128-bit digest of every full 128-row block of x [rows, cols] bf16 (unit column stride, any row stride that
+    is a multiple of 4; cols a multiple of 4) under the 64-bit keys key0 / key1, by the rule of
+    vila_b200/prefix_cache.py (vila_prefix_block_hash, one launch).  -> int64 [rows // 128, 2] on x's device, the
+    uint64 digests' bits (.view(torch.uint64) or numpy .view(np.uint64) to read them unsigned)."""
+    _need(x.dim() == 2 and x.stride(1) == 1 and (x.shape[0] <= 1 or x.stride(0) >= x.shape[1]),
+          f"prefix_block_hash: x must be [rows, cols] with unit column stride, got {tuple(x.shape)} strides "
+          f"{tuple(x.stride())}")
+    _need(0 <= key0 < 2 ** 64 and 0 <= key1 < 2 ** 64, "prefix_block_hash: the keys are unsigned 64-bit integers")
+    _chk(x, "x")
+    rows, cols = x.shape
+    out = torch.empty(rows // 128, 2, dtype=torch.int64, device=x.device)
+    ld = x.stride(0) if rows > 1 else cols
+    check(_lib.load().vila_prefix_block_hash(_p(x), ld, rows, cols, key0, key1, _p(out), _stream()),
+          "vila_prefix_block_hash")
+    return out

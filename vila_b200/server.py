@@ -8,7 +8,9 @@ engine is busy are grouped (up to `slots`) and decoded together by `LlavaLlamaMo
 (continuous batching over the shared paged pool, vila_b200/serving.py).  With --sample every request is sampled
 on the device with its own temperature, top_p and seed: non-streaming ones through generate_batch, streaming ones
 on the single-stream graph decoder (generate_content(stream=True) with a sampling generation config).  Without it
-every request is decoded greedily.
+every request is decoded greedily.  With --prefix-cache every non-streaming request goes to the batched engine, which
+the model keeps between batches together with the K/V pages of the prompt blocks it has seen: a request that starts
+like an earlier one (another question about the same video or image) prefills only what follows the shared blocks.
 
     python -m vila_b200.server --model-path <dir> --port 8000
 """
@@ -145,12 +147,18 @@ class Engine:
     """One model, one asyncio lock (the GPU is a single queue): streaming requests hold the lock while
     their generator runs; non-streaming requests waiting for it are batched together."""
 
-    def __init__(self, model, model_name: str, slots: int = 8, kv_cache: str = "bf16", sample: bool = False):
+    def __init__(self, model, model_name: str, slots: int = 8, kv_cache: str = "bf16", sample: bool = False, *,
+                 prefix_cache: bool = False, max_tokens_per_slot: int = 20480):
         self.model, self.model_name, self.slots = model, model_name, slots
         self.kv_cache = kv_cache
         if sample and not hasattr(model, "generate_batch"):
             raise ValueError("sample=True needs a model with generate_batch (the batched engine draws the tokens)")
+        if prefix_cache and not hasattr(model, "generate_batch"):
+            raise ValueError("prefix_cache=True needs a model with generate_batch (the batched engine caches prompts)")
+        if prefix_cache and kv_cache == "fp8":
+            raise ValueError("prefix caching is not supported with the fp8 KV cache")
         self.sample = sample  # every request sampled with its own parameters (batched engine / graph decoder)
+        self.prefix_cache, self.max_tokens_per_slot = prefix_cache, max_tokens_per_slot
         self.lock = asyncio.Lock()
         self.pending: List[Any] = []
 
@@ -190,13 +198,15 @@ class Engine:
     def _run_batch(self, reqs: List[ChatCompletionRequest], sampling: Optional[list] = None) -> List[str]:
         """sampling: one SamplingParams per request (Engine(sample=True)), or None for greedy decoding"""
         m = self.model
-        if sampling is None and (len(reqs) == 1 or not hasattr(m, "generate_batch")):
+        if sampling is None and not self.prefix_cache and (len(reqs) == 1 or not hasattr(m, "generate_batch")):
             return [m.generate_content(build_prompt(r.messages), generation_config=self._gen_config(r)) for r in reqs]
         prepared = [m._prepare_content(build_prompt(r.messages)) for r in reqs]
         # the default is not passed: a model whose generate_batch predates the kv_cache argument keeps working
         kw = {} if self.kv_cache == "bf16" else {"kv_cache": self.kv_cache}
         if sampling is not None:
             kw["sampling"] = sampling
+        if self.prefix_cache:
+            kw.update(prefix_cache=True, max_tokens_per_slot=self.max_tokens_per_slot)
         ids = m.generate_batch([{"input_ids": i, "media": md, "media_config": mc} for i, md, mc in prepared],
                                max_new_tokens=max(r.max_tokens or 512 for r in reqs), slots=self.slots, **kw)
         outs = []
@@ -240,11 +250,13 @@ class Engine:
             yield "data: [DONE]\n\n"
 
 
-def create_app(model, model_name: str, slots: int = 8, kv_cache: str = "bf16", sample: bool = False):
+def create_app(model, model_name: str, slots: int = 8, kv_cache: str = "bf16", sample: bool = False, *,
+               prefix_cache: bool = False, max_tokens_per_slot: int = 20480):
     from fastapi import FastAPI
     from fastapi.responses import JSONResponse, StreamingResponse
     app = FastAPI()
-    engine = Engine(model, model_name, slots, kv_cache, sample)
+    engine = Engine(model, model_name, slots, kv_cache, sample, prefix_cache=prefix_cache,
+                    max_tokens_per_slot=max_tokens_per_slot)
     app.state.engine = engine
 
     @app.get("/")
@@ -286,9 +298,21 @@ def main() -> None:
                          "non-streaming requests on the batched engine (vila_sample_batch), even one that arrives "
                          "alone, streaming requests on the single-stream graph decoder (vila_sample_finalize); "
                          "without it every request is decoded greedily")
+    ap.add_argument("--prefix-cache", action="store_true",
+                    help="send every non-streaming request, even one that arrives alone, to the batched engine and "
+                         "keep that engine between batches with the K/V pages of the full 128-token prompt blocks it "
+                         "has seen, so that a request starting like an earlier one (another question about the same "
+                         "video or image) prefills only what follows.  The kept pool is slots x "
+                         "--max-tokens-per-slot x the K/V bytes per token (57,344 B for NVILA-8B: 9.4 GB at 8 x "
+                         "20,480).  Not with --kv-cache fp8; streaming requests are unchanged")
+    ap.add_argument("--max-tokens-per-slot", type=int, default=20480,
+                    help="tokens per slot of the kept engine of --prefix-cache (prompt + new tokens + 8)")
     args = ap.parse_args()
+    if args.prefix_cache and args.kv_cache == "fp8":
+        ap.error("--prefix-cache is not supported with --kv-cache fp8")
     model = llava.load(args.model_path, decode_weights=args.decode_weights)
-    uvicorn.run(create_app(model, get_model_name_from_path(args.model_path), args.slots, args.kv_cache, args.sample),
+    uvicorn.run(create_app(model, get_model_name_from_path(args.model_path), args.slots, args.kv_cache, args.sample,
+                           prefix_cache=args.prefix_cache, max_tokens_per_slot=args.max_tokens_per_slot),
                 host=args.host, port=args.port)
 
 

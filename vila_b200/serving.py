@@ -28,16 +28,24 @@ tokens per byte by B.  Here:
     vila_decode_attention_fp8_batch (RoPE, e4m3 append and split-KV attention in one launch per layer);
   * with sampling=True each slot has its own temperature / top-k / top-p / seed (SamplingParams, the rule in
     vila_b200/sampling.py) in device arrays, and vila_sample_batch replaces the greedy arg-max, in the step graphs
-    and for the first token at admission; a slot's draw depends only on its own logits, seed and token index.
+    and for the first token at admission; a slot's draw depends only on its own logits, seed and token index;
+  * with prefix_cache=True (vila_b200/prefix_cache.py) the full 128-token blocks of every admitted prompt are digested
+    on the device (vila_prefix_block_hash) and kept in a trie of cached pages: a later prompt that starts with the same
+    blocks at the same positions takes those pages into its page-table row and prefills only its suffix.  Full prompt
+    pages are never written after the prefill (decode appends at positions >= S), so sharing needs no copy.  A hit
+    request's ids equal those of a chunked prefill of its suffix over the donor's prefix pages; they may differ from
+    its uncached ids, since the donor's prefill may have run its GEMMs at another M.
 """
 from __future__ import annotations
 
 from collections import deque
 from typing import Deque, Dict, List, Optional, Sequence, Tuple, Union
 
+import numpy as np
 import torch
 
 from . import ops
+from .prefix_cache import PrefixPages, random_keys
 from .sampling import SamplingParams, signed64
 
 PAGE = 128
@@ -157,13 +165,25 @@ class BatchedDecoder:
 
     sampling False (default) picks every token greedily with torch.argmax.  True keeps per-slot device arrays of
     the sampling parameters (admit() writes them) and draws every token with vila_sample_batch, at token index
-    `step_idx` of the slot; a slot admitted without parameters decodes greedily (temperature 0)."""
+    `step_idx` of the slot; a slot admitted without parameters decodes greedily (temperature 0).
+
+    prefix_cache False (default) prefills every prompt in full.  True shares the pages of full 128-token prompt blocks
+    between requests whose prompts start alike (vila_b200/prefix_cache.py): `allocator` is then a PrefixPages,
+    admit() prefills only the part of the prompt past the cached blocks, released blocks stay findable until their
+    pages are needed, `prefix_stats` counts the work saved and clear_prefix_cache() drops the unused blocks.  The
+    fp8 KV cache is not supported with it (its admission prefills into a bf16 staging cache, which would need the
+    prefix in bf16)."""
 
     def __init__(self, llm, slots: int = 8, max_tokens_per_slot: int = 2048, max_new: int = 1024,
-                 total_pages: Optional[int] = None, kv_cache: str = "bf16", sampling: bool = False):
+                 total_pages: Optional[int] = None, kv_cache: str = "bf16", sampling: bool = False,
+                 prefix_cache: bool = False):
         if kv_cache not in KV_CACHE_FORMATS:
             raise ValueError(f"kv_cache must be one of {KV_CACHE_FORMATS}, got {kv_cache!r}")
+        if prefix_cache and kv_cache == "fp8":
+            raise ValueError("prefix_cache=True is not supported with kv_cache='fp8': the fp8 admission prefills into "
+                             "a bf16 staging cache, which would need the cached prefix in bf16")
         self.kv_cache = kv_cache
+        self.prefix_cache = bool(prefix_cache)
         cfg = llm.config
         self.llm, self.slots = llm, slots
         self.decode_weights = getattr(llm, "decode_weights", "bf16")
@@ -181,7 +201,9 @@ class BatchedDecoder:
         fp8 = kv_cache == "fp8"
         self.pool = torch.zeros(L, 2, P, PAGE, Hkv, D, device=dev, dtype=torch.float8_e4m3fn if fp8 else dt)
         self.pool_scale = torch.zeros(L, 2, P, PAGE, Hkv, device=dev, dtype=torch.float32) if fp8 else None
-        self.allocator = PageAllocator(P)
+        self.allocator = PrefixPages(P) if self.prefix_cache else PageAllocator(P)
+        if self.prefix_cache:
+            self.prefix_keys = random_keys()
         self.slot_pages: List[List[int]] = [[] for _ in range(slots)]
         # unassigned entries point at page 0; they are never dereferenced (tokens beyond a slot's length)
         self.page_tables = torch.zeros(slots, self.pages_per_slot, dtype=torch.int32, device=dev)
@@ -235,12 +257,44 @@ class BatchedDecoder:
         per_layer = 7 if self.config is None or self.kv_cache == "fp8" else 9
         return per_layer * self.llm.config.num_hidden_layers + 2 + (1 if self.sampling else 0)
 
+    # ---- prefix cache ---------------------------------------------------------------------------
+    def prefix_digests(self, inputs_embeds: torch.Tensor) -> np.ndarray:
+        """uint64 [S // 128, 2]: the digests of the prompt's full blocks under this decoder's keys (one
+        vila_prefix_block_hash launch and one copy to the host)"""
+        return ops.prefix_block_hash(inputs_embeds, *self.prefix_keys).cpu().numpy().view(np.uint64)
+
+    def prefix_hits(self, digests: np.ndarray, S: int) -> List[int]:
+        """cached pages an S-token prompt with these digests would take: at most (S - 1) // 128 blocks, so that at
+        least one token is prefilled (it gives the first token) and the slot never writes into a shared page"""
+        return self.allocator.match(digests, (S - 1) // PAGE)
+
+    def _need_prefix_cache(self, what: str) -> None:
+        if not self.prefix_cache:
+            raise ValueError(f"{what} needs a decoder built with prefix_cache=True")
+
+    @property
+    def prefix_stats(self) -> Dict[str, int]:
+        """lookups (admissions), hit_blocks / hit_tokens served from the cache, prefilled_tokens, cached_blocks (now)
+        and evictions"""
+        self._need_prefix_cache("prefix_stats")
+        return dict(self.allocator.stats, cached_blocks=self.allocator.cached_blocks)
+
+    def clear_prefix_cache(self) -> int:
+        """drop every cached block that no live slot holds -> blocks dropped"""
+        self._need_prefix_cache("clear_prefix_cache()")
+        return self.allocator.clear()
+
     # ---- admission ------------------------------------------------------------------------------
     @torch.inference_mode()
-    def admit(self, slot: int, inputs_embeds: torch.Tensor, params: Optional[SamplingParams] = None) -> None:
+    def admit(self, slot: int, inputs_embeds: torch.Tensor, params: Optional[SamplingParams] = None, *,
+              digests: Optional[np.ndarray] = None) -> None:
         """Prefill `inputs_embeds` [S, hidden] into the slot's pages and seed its decode state.  params: the slot's
-        SamplingParams (sampling decoders only; None is greedy); its seed must be set."""
-        llm = self.llm
+        SamplingParams (sampling decoders only; None is greedy); its seed must be set.  digests: prefix_digests of
+        the prompt, if the caller has them already (prefix-caching decoders).
+
+        A prefix-caching decoder admits into an idle slot only (released, or never used), and if the admission raises
+        it releases the slot again: the hit blocks are unpinned and the pages it took are returned, so a failed request
+        leaves no page half-owned and no block registered over K/V that was not written."""
         if params is not None and not self.sampling:
             raise ValueError("admit(params=...) needs a decoder built with sampling=True")
         if self.sampling:
@@ -249,12 +303,44 @@ class BatchedDecoder:
                 raise ValueError("admit: a sampled slot needs a seed (generate_batch draws one)")
         S = inputs_embeds.shape[0]
         assert S + 1 <= self.pages_per_slot * PAGE, "prompt longer than a slot"
+        if not self.prefix_cache:
+            self._fill(slot, inputs_embeds, params, 0, None)
+            return
+        if self.slot_pages[slot] or self._pos_host[slot] >= 0:
+            raise ValueError(f"admit: slot {slot} is still in use: release() it first")
+        if digests is None:
+            digests = self.prefix_digests(inputs_embeds)
+        hits = self.prefix_hits(digests, S)
+        self.allocator.pin(hits)  # before any allocation: the hit pages cannot be evicted under this request
+        self.slot_pages[slot] = list(hits)
+        try:
+            if hits:
+                self.page_tables[slot, :len(hits)] = torch.tensor(hits, dtype=torch.int32,
+                                                                  device=self.page_tables.device)
+            self._fill(slot, inputs_embeds, params, PAGE * len(hits), digests)
+        except BaseException:
+            self.release(slot)
+            raise
+        self.allocator.stats["prefilled_tokens"] += S - PAGE * len(hits)
+
+    def _fill(self, slot: int, inputs_embeds: torch.Tensor, params: Optional[SamplingParams], p0: int,
+              digests: Optional[np.ndarray]) -> None:
+        """admit()'s work once the slot's first p0 // 128 pages hold the cached prefix: pages for the rest, the prefill
+        of inputs_embeds[p0:], registration of the new full blocks (prefix caching) and the first token"""
+        llm = self.llm
+        S = inputs_embeds.shape[0]
         self._ensure_pages(slot, S + 1)
         if self.kv_cache == "fp8":  # prefill in bf16, then one conversion into the slot's e4m3 pages
             hid = llm.prefill_hidden(inputs_embeds, _SlotCache(self.staging, self.staging_pages))
             ops.kv_quantize_fp8(self.staging, self.pool, self.pool_scale, self.page_tables[slot], S)
+        elif p0:
+            cache = _SlotCache(self.pool, self.page_tables[slot])
+            cache.length = p0
+            hid = llm.prefill_hidden(inputs_embeds[p0:], cache)
         else:
             hid = llm.prefill_hidden(inputs_embeds, _SlotCache(self.pool, self.page_tables[slot]))
+        if self.prefix_cache:
+            self.allocator.register(digests, self.slot_pages[slot], p0 // PAGE)
         if self.decode_weights == "bf16":
             logits = llm.logits_from_hidden(hid[-1:])
         else:  # the mode's lm_head, as GraphDecoder.start
@@ -431,7 +517,8 @@ def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eo
                    slots: int = 8, max_tokens_per_slot: Optional[int] = None, check_every: int = 8,
                    decoder: Optional[BatchedDecoder] = None, total_pages: Optional[int] = None,
                    kv_cache: str = "bf16",
-                   sampling: Union[None, SamplingParams, Sequence[SamplingParams]] = None) -> List[List[int]]:
+                   sampling: Union[None, SamplingParams, Sequence[SamplingParams]] = None,
+                   prefix_cache: bool = False) -> List[List[int]]:
     """Decode `prompts` (list of inputs_embeds [S_i, hidden]) with continuous batching: at most
     `slots` requests in flight; a finished request (EOS or max_new_tokens) frees its slot for the next
     one in the queue.  Returns the new ids per request (EOS included), in request order.
@@ -442,8 +529,18 @@ def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eo
     sampling None: greedy (the decoder's torch arg-max).  Otherwise one SamplingParams for every request or a list
     with one per request, drawn on the device (BatchedDecoder(sampling=True)); a seed of None is drawn from the host
     torch default generator in request order, so torch.manual_seed reproduces a run.  A passed-in greedy decoder
-    with sampling requested is a ValueError; a sampling decoder serves greedy requests as temperature-0 rows."""
+    with sampling requested is a ValueError; a sampling decoder serves greedy requests as temperature-0 rows.
+    prefix_cache True: requests share the pages of the full prompt blocks they start with (BatchedDecoder); a request
+    is admitted when the pool can hold the pages it must newly take, ceil((S + max_new_tokens + check_every) / 128)
+    minus its cached blocks, out of the free and evictable pages other than its own cached blocks.  A passed-in
+    `decoder` with the other setting, or whose max_new is below max_new_tokens, is a ValueError."""
     params = sampling_for_requests(sampling, len(prompts))
+    if decoder is not None and getattr(decoder, "prefix_cache", False) != bool(prefix_cache):
+        raise ValueError(f"decoder was built with prefix_cache={getattr(decoder, 'prefix_cache', False)}, "
+                         f"prefix_cache={bool(prefix_cache)} was asked for")
+    if decoder is not None and max_new_tokens > getattr(decoder, "max_new", max_new_tokens):
+        raise ValueError(f"max_new_tokens={max_new_tokens} exceeds the decoder's max_new={decoder.max_new}: its "
+                         f"history would stop short of the budget")
     if params is not None and decoder is not None and not getattr(decoder, "sampling", False):
         raise ValueError("sampling was requested but the decoder was built with sampling=False")
     mode = getattr(llm, "decode_weights", "bf16")
@@ -459,7 +556,7 @@ def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eo
                                                         check_every, slots, max_tokens_per_slot)
         decoder = BatchedDecoder(llm, slots, max_tokens_per_slot, max_new=max_new_tokens,
                                  total_pages=total_pages if total_pages is not None else pool_pages,
-                                 kv_cache=kv_cache, sampling=params is not None)
+                                 kv_cache=kv_cache, sampling=params is not None, prefix_cache=prefix_cache)
     dec = decoder
     dec.capture()
     cap = dec.pages_per_slot * PAGE
@@ -477,23 +574,41 @@ def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eo
                 return ids[:i + 1]
         return ids[:max_new_tokens] if len(ids) >= max_new_tokens else None
 
-    while queue or owner:
+    try:
+        digests: Dict[int, np.ndarray] = {}  # request -> prefix_digests, computed once while it heads the queue
+        while queue or owner:
+            for s in range(dec.slots):
+                if s not in owner and queue:
+                    # admit only when the pool can hold the prompt and the request's whole budget
+                    head = prompts[queue[0]]
+                    need = (head.shape[0] + max_new_tokens + check_every + PAGE - 1) // PAGE
+                    available = dec.allocator.available
+                    if prefix_cache:  # cached blocks are not taken again; pinning makes them unavailable
+                        if queue[0] not in digests:
+                            digests[queue[0]] = dec.prefix_digests(head)
+                        hits = dec.prefix_hits(digests[queue[0]], head.shape[0])
+                        need -= len(hits)
+                        available -= dec.allocator.evictable_among(hits)
+                    if need > available and owner:
+                        break  # wait for a running request to finish and return its pages
+                    r = queue.popleft()
+                    kw = {"digests": digests.pop(r)} if prefix_cache else {}
+                    if params is None:
+                        dec.admit(s, prompts[r], **kw)
+                    else:
+                        dec.admit(s, prompts[r], params[r], **kw)
+                    owner[s] = r
+            dec.run(check_every)
+            for s in list(owner):
+                done = harvest(s, dec.generated(s))
+                if done is not None:
+                    out[owner.pop(s)] = done
+                    dec.release(s)
+    except BaseException:
+        # a failed request fails the call, but a decoder that outlives it (a kept prefix-caching engine) must not keep
+        # this call's slots: every slot that was admitted, or was being admitted, is released
         for s in range(dec.slots):
-            if s not in owner and queue:
-                # admit only when the pool can hold the prompt and the request's whole budget
-                need = (prompts[queue[0]].shape[0] + max_new_tokens + check_every + PAGE - 1) // PAGE
-                if need > dec.allocator.available and owner:
-                    break  # wait for a running request to finish and return its pages
-                r = queue.popleft()
-                if params is None:
-                    dec.admit(s, prompts[r])
-                else:
-                    dec.admit(s, prompts[r], params[r])
-                owner[s] = r
-        dec.run(check_every)
-        for s in list(owner):
-            done = harvest(s, dec.generated(s))
-            if done is not None:
-                out[owner.pop(s)] = done
+            if s in owner or getattr(dec, "slot_pages", [[]] * dec.slots)[s]:
                 dec.release(s)
+        raise
     return [o or [] for o in out]
