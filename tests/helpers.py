@@ -590,3 +590,421 @@ def greedy_ids_match(got: List[int], oracle_ids: List[int], oracle_logits: torch
         gap = (top2[0] - top2[1]).item()
         assert gap < margin, f"token {i}: got {a}, oracle {b}, oracle top-2 margin {gap:.4f} >= {margin}"
         return
+
+
+# ------------------------------------------------------------------------------------------------
+# decode GEMV: mirrors of the launch plans, independent quantizers, the fp64 reference and GemvErrors
+# ------------------------------------------------------------------------------------------------
+W4_GROUP = 128
+W4_TILE = 16
+
+
+def gemv_tma_plan(N: int, K: int, fp8: bool, swiglu: bool, norm: bool, sms: int):
+    """gemv_tma_launch's choice (gemv_tma.cu) for the bf16 (fp8=False) or e4m3 TMA-ring kernel: a dict with
+    rows_per_block, grid, ksplit, chunk_elems and stages, or None where the launcher returns -1 (bf16: the
+    register-staged kernel runs instead)."""
+    max_stages, eb = (12, 1) if fp8 else (6, 2)
+    align = 16 // eb
+    rpb = _cdiv(N, sms)
+    if swiglu and rpb % 2:
+        rpb += 1
+    x1 = _cdiv(K * 2, 128) * 128
+    xb = x1 * (2 if norm else 1)
+    scb = rpb * 4 if fp8 else 0
+    bars = (8 * max_stages + 2) * 8
+    ksplit = -1
+    for ks in range(1, 129):
+        if K % ks:
+            continue
+        ce = K // ks
+        if ce % align:
+            continue
+        cb = ce * eb
+        if cb > 8192:
+            continue
+        if cb < 512:
+            break
+        acc = _cdiv(rpb * ks * 4 + scb, 128) * 128
+        st = min(max_stages, (220 * 1024 - xb - acc - bars - 256) // (8 * cb))
+        if st < 3:
+            continue
+        ksplit = ks
+        if rpb * ks >= 6 * 8:
+            break
+    if ksplit < 0:
+        return None
+    ce = K // ksplit
+    ring_off = _cdiv(xb + rpb * ksplit * 4 + scb, 128) * 128
+    st = min(max_stages, (220 * 1024 - ring_off - bars - 256) // (8 * ce * eb))
+    if st < 2:
+        return None
+    return dict(rows_per_block=rpb, grid=_cdiv(N, rpb), ksplit=ksplit, chunk_elems=ce, stages=st)
+
+
+def gemv_reg_plan(N: int, K: int, swiglu: bool, sms: int) -> dict:
+    """gemv_bf16's register-staged kernel (decode.cu, variant 1): rows per block, k-parts, 256-k chunks per part"""
+    rpb = _cdiv(N, sms)
+    if swiglu and rpb % 2:
+        rpb += 1
+    nchunks = _cdiv(K // 8, 32)
+    ks = 1
+    while rpb * ks < 3 * 8 and ks * 2 <= nchunks and ks < 16:
+        ks *= 2
+    return dict(rows_per_block=rpb, grid=_cdiv(N, rpb), ksplit=ks, chunks_per_part=_cdiv(nchunks, ks))
+
+
+def gemv_w4_plan(N: int, K: int, norm: bool, sms: int):
+    """gemv_w4_launch's choice for the single-stream W4A16 kernel: tiles_per_block, rows_per_block, grid,
+    ksplit, chunk_groups, stages (None: the launcher refuses the shape)"""
+    tiles = _cdiv(N, W4_TILE)
+    tpb = _cdiv(tiles, sms)
+    rpb = tpb * W4_TILE
+    G = K // W4_GROUP
+    x1 = _cdiv(K * 2, 128) * 128
+    xb = x1 * (2 if norm else 1)
+    gp = _cdiv(rpb * G * 3, 128) * 128
+    bars = (8 * 12 + 2) * 8
+    ksplit = -1
+    for ks in range(1, G + 1):
+        if G % ks:
+            continue
+        cb = G // ks * 1024
+        if cb > 8192:
+            continue
+        acc = _cdiv(rpb * ks * 4, 128) * 128
+        if (220 * 1024 - xb - acc - gp - bars - 256) // (8 * cb) < 3:
+            continue
+        ksplit = ks
+        if tpb * ks >= 6 * 8:
+            break
+    if ksplit < 0:
+        return None
+    cg = G // ksplit
+    ring_off = xb + _cdiv(rpb * ksplit * 4, 128) * 128 + gp
+    st = min(12, (220 * 1024 - ring_off - bars - 256) // (8 * cg * 1024))
+    return dict(tiles_per_block=tpb, rows_per_block=rpb, grid=_cdiv(tiles, tpb), ksplit=ksplit, chunk_groups=cg,
+                stages=st)
+
+
+def batch_partition(N: int, K: int, fp8: bool, sms: int, max_active_clusters=None):
+    """batch_partition (gemv_tma.cu) for gemv_batch_*: max_active_clusters(cluster) is what
+    cudaOccupancyMaxActiveClusters reports for that cluster size (default: sms // cluster).  -> dict with
+    cluster, ctas, tiles_per_cluster, unit, units, max_units, parts, stages, slices [(u0, nu)] and, per slice,
+    its k-parts [(pu0, pu)] as part_range cuts them; None where the launcher refuses the shape."""
+    active = max_active_clusters or (lambda cl: sms // cl)
+    tiles = _cdiv(N, W4_TILE)
+    unit = 16 if fp8 else W4_GROUP
+    units = K // unit
+
+    def x_pitch(cl):
+        return _cdiv(_cdiv(units, cl) * unit * 2, 128) * 128 + 16
+
+    def tpc(cl):
+        a = active(cl)
+        n = max(1, min(sms // cl, a if a > 0 else sms // cl))
+        return _cdiv(tiles, n)
+
+    cluster = 0
+    cl = 1
+    while cl <= 8:
+        if units < 4 * cl:
+            break
+        xb = 16 * x_pitch(cl)
+        pb = tpc(cl) * W4_TILE * 16 * 4 if cl > 1 else 0
+        if xb + pb <= 100 * 1024:
+            cluster = cl
+            break
+        cl *= 2
+    if cluster == 0:
+        if 16 * x_pitch(1) > 120 * 1024:
+            return None
+        cluster = 1
+    t = tpc(cluster)
+    max_units = _cdiv(units, cluster)
+    rows = t * W4_TILE
+    part_off = 16 * x_pitch(cluster)
+    gs_off = part_off + (rows * 16 * 4 if cluster > 1 else 0)
+    gz_off = gs_off + (rows * 4 if fp8 else rows * max_units * 2)
+    ring_off = _cdiv(gz_off + (0 if fp8 else rows * max_units), 128) * 128
+    bars = (8 * 12 + 1) * 8
+    max_chunk = 32 if fp8 else 8
+    parts, stages = _cdiv(max_units, max_chunk), 0
+    while parts <= max_units:
+        chunk = _cdiv(max_units, parts)
+        slot = 16 * (_cdiv(chunk * unit, 128) * 128 + 64) if fp8 else chunk * 1024
+        stages = min(12, (220 * 1024 - ring_off - bars) // (8 * slot))
+        if stages >= 3:
+            break
+        parts += 1
+    if parts > max_units or stages < 3:
+        return None
+    slices = [(r * units // cluster, (r + 1) * units // cluster - r * units // cluster) for r in range(cluster)]
+    kparts = [[(q * nu // parts, (q + 1) * nu // parts - q * nu // parts) for q in range(parts)] for _, nu in slices]
+    return dict(cluster=cluster, ctas=_cdiv(tiles, t) * cluster, tiles_per_cluster=t, unit=unit, units=units,
+                max_units=max_units, parts=parts, stages=stages, slices=slices, kparts=kparts)
+
+
+def gemv_depth(kind: str, K: int, plan: dict) -> int:
+    """The deepest fp32 summation chain of one output (additions a product passes through before the epilogue,
+    the epilogue's scale and bias included), for GemvErrors' accumulation term.  An mma.sync step is counted
+    as 16 additions; kind: "tma-bf16", "tma-fp8", "reg-bf16", "w4", "batch-fp8", "batch-w4"."""
+    if kind in ("tma-bf16", "tma-fp8"):
+        per_vec = 16 if kind == "tma-fp8" else 8
+        vecs = plan["chunk_elems"] * (1 if kind == "tma-fp8" else 2) // 16
+        return per_vec * _cdiv(vecs, 64) + 1 + 5 + plan["ksplit"] + 2
+    if kind == "reg-bf16":
+        return 8 * plan["chunks_per_part"] + 5 + plan["ksplit"] + 2
+    if kind == "w4":
+        return 4 * 16 + 1 + plan["chunk_groups"] + plan["ksplit"] + 2
+    if kind == "batch-w4":
+        return 4 * 16 + 1 + plan["max_units"] + plan["cluster"] + 2
+    if kind == "batch-fp8":
+        chunk = _cdiv(plan["max_units"], plan["parts"]) * plan["unit"]
+        return 4 * 16 * _cdiv(chunk, 128) + 1 + plan["parts"] + plan["cluster"] + 2
+    raise ValueError(kind)
+
+
+# --- the quantizers, re-derived from their docstrings and gemv_tma.cu's layout comment -------------------------
+def _bf16_rne(t: torch.Tensor) -> torch.Tensor:
+    """fp32 -> the nearest bf16 (ties to even), returned as fp32; finite inputs"""
+    u = t.to(torch.float32).contiguous().view(torch.int32).to(torch.int64)
+    u = (u + 0x7FFF + ((u >> 16) & 1)) & ~0xFFFF
+    return u.to(torch.int32).view(torch.float32)  # int64 -> int32 wraps the sign bit back
+
+
+def e4m3_values() -> torch.Tensor:
+    """the value of each e4m3fn code 0..255 (fp64; 0x7f and 0xff are NaN): sign, 4 exponent bits (bias 7),
+    3 mantissa bits; exponent 0 is subnormal (m / 8 * 2^-6)"""
+    c = torch.arange(256, dtype=torch.int64)
+    e, m = (c >> 3) & 15, (c & 7).to(torch.float64)
+    mag = torch.where(e == 0, m / 8 * 2.0 ** -6, (1 + m / 8) * torch.pow(2.0, (e - 7).to(torch.float64)))
+    mag = torch.where((c & 127) == 127, torch.full_like(mag, float("nan")), mag)
+    return torch.where(c >= 128, -mag, mag)
+
+
+def e4m3_encode(t: torch.Tensor) -> torch.Tensor:
+    """fp32 values with |t| <= 464 -> e4m3fn codes (uint8), round to nearest, ties to the even code (the
+    even mantissa); the sign bit follows t's sign, so a negative value that rounds to 0 is -0 (0x80)"""
+    pos = e4m3_values()[:127].to(t.device)  # codes 0..126: 0 .. 448, increasing
+    a = t.to(torch.float64).abs()
+    assert bool((a <= 464).all()), "e4m3_encode: |t| > 464 overflows"
+    hi = torch.searchsorted(pos, a).clamp(max=126)
+    lo = (hi - 1).clamp(min=0)
+    dlo, dhi = a - pos[lo], pos[hi] - a
+    code = torch.where(dlo < dhi, lo, torch.where(dhi < dlo, hi, torch.where(lo % 2 == 0, lo, hi)))
+    code = torch.where(a > 448, torch.full_like(code, 126), code)
+    return (code | (torch.signbit(t).to(torch.int64) << 7)).to(torch.uint8)
+
+
+REF_ROWS = 4096  # rows per chunk of the reference quantizers: an lm_head's fp64 temporaries stay ~100 MB each
+
+
+def ref_quantize_e4m3_rows(w: torch.Tensor):
+    """quantize_e4m3_rows' docstring: s_n = amax_n / 448 in fp32 (1 for an all-zero row), code =
+    e4m3(W / s_n) with the division in fp32.  -> (codes uint8 [N, K], s fp32 [N]), in chunks of rows"""
+    N = w.shape[0]
+    codes = torch.empty(w.shape, dtype=torch.uint8, device=w.device)
+    s = torch.empty(N, dtype=torch.float32, device=w.device)
+    for r0 in range(0, N, REF_ROWS):
+        wf = w[r0:r0 + REF_ROWS].to(torch.float32)
+        amax = wf.abs().amax(dim=1)
+        sc = torch.where(amax > 0, amax / torch.tensor(448.0, device=w.device), torch.ones_like(amax))
+        codes[r0:r0 + REF_ROWS] = e4m3_encode(wf / sc[:, None])
+        s[r0:r0 + REF_ROWS] = sc
+    return codes, s
+
+
+def ref_quantize_w4(w: torch.Tensor):
+    """quantize_w4_groups' docstring, per row and group of 128 k in fp32: lo = min(0, min w), hi = max(0, max w),
+    s = bf16((hi - lo) / 15) or 1, z = clamp(rint(-lo / s), 0, 15), q = clamp(rint(w / s) + z, 0, 15) (rint:
+    half to even).  -> (codes uint8 [N, K], s fp32 [N, G] (bf16 values), z uint8 [N, G]), in chunks of rows"""
+    N, K = w.shape
+    G = K // W4_GROUP
+    q = torch.empty(N, K, dtype=torch.uint8, device=w.device)
+    s = torch.empty(N, G, dtype=torch.float32, device=w.device)
+    z = torch.empty(N, G, dtype=torch.uint8, device=w.device)
+    for r0 in range(0, N, REF_ROWS):
+        wf = w[r0:r0 + REF_ROWS].to(torch.float32).reshape(-1, G, W4_GROUP)
+        lo = wf.amin(dim=2).clamp(max=0)
+        hi = wf.amax(dim=2).clamp(min=0)
+        sc = _bf16_rne((hi - lo) / torch.tensor(15.0, device=w.device))
+        sc = torch.where(sc == 0, torch.ones_like(sc), sc)
+        zp = torch.round(-lo / sc).clamp(0, 15)  # torch.round: half to even
+        q[r0:r0 + REF_ROWS] = (torch.round(wf / sc[..., None]) + zp[..., None]).clamp(0, 15).reshape(-1, K)
+        s[r0:r0 + REF_ROWS], z[r0:r0 + REF_ROWS] = sc, zp.to(torch.uint8)
+    return q, s, z
+
+
+# nibble p of a packed u32 (bits 4p .. 4p+3): (row offset 0 / 8 within the lane's pair g, g + 8; k offset from k0)
+W4_NIBBLES = ((0, 0), (8, 0), (0, 2), (8, 2), (0, 1), (8, 1), (0, 3), (8, 3))
+
+
+def ref_w4_pack(q: torch.Tensor) -> torch.Tensor:
+    """codes uint8 [N, K] -> the packed bytes [ceil(N/16), 8 K] as gemv_tma.cu's comment above w4_pair lays them
+    out: rows in tiles of 16 (padded with zero codes), per tile [K/64 blocks][32 lanes][4 u32], lane = 4 g + c,
+    u32 j of block b holding rows g, g + 8 at k0 = b + 16 c + 4 j .. k0 + 3, nibble p as W4_NIBBLES; u32s little
+    endian; in chunks of tiles"""
+    N, K = q.shape
+    T = _cdiv(N, W4_TILE)
+    out = torch.empty(T, 8 * K, dtype=torch.uint8, device=q.device)
+    step = REF_ROWS // W4_TILE
+    for t0 in range(0, T, step):
+        t1 = min(T, t0 + step)
+        qp = torch.zeros((t1 - t0) * W4_TILE, K, dtype=torch.int64, device=q.device)
+        rows = q[t0 * W4_TILE:t1 * W4_TILE]
+        qp[:rows.shape[0]] = rows.to(torch.int64)
+        t = qp.view(t1 - t0, W4_TILE, K // 64, 4, 4, 4)  # [tile, row, b, c, j, kk]
+        word = torch.zeros(t1 - t0, K // 64, 8, 4, 4, dtype=torch.int64, device=q.device)  # [tile, b, g, c, j]
+        for p, (dr, dk) in enumerate(W4_NIBBLES):
+            word |= t[:, dr:dr + 8, :, :, :, dk].permute(0, 2, 1, 3, 4) << (4 * p)
+        by = torch.stack([(word >> (8 * i)) & 255 for i in range(4)], dim=-1)  # [tile, b, g, c, j, byte]
+        out[t0:t1] = by.reshape(t1 - t0, 8 * K).to(torch.uint8)
+    return out
+
+
+def ref_w4_unpack(packed: torch.Tensor, N: int, K: int) -> torch.Tensor:
+    """the inverse of ref_w4_pack (the same layout read back): codes uint8 [N, K]"""
+    T = packed.shape[0]
+    by = packed.to(torch.int64).view(T, K // 64, 8, 4, 4, 4)
+    word = by[..., 0] | (by[..., 1] << 8) | (by[..., 2] << 16) | (by[..., 3] << 24)  # [tile, b, g, c, j]
+    q = torch.zeros(T, W4_TILE, K // 64, 4, 4, 4, dtype=torch.int64, device=packed.device)
+    for p, (dr, dk) in enumerate(W4_NIBBLES):
+        q[:, dr:dr + 8, :, :, :, dk] = ((word >> (4 * p)) & 15).permute(0, 2, 1, 3, 4)
+    return q.reshape(T * W4_TILE, K)[:N].to(torch.uint8)
+
+
+# --- the reference and the checker ---------------------------------------------------------------------------
+def gemv_xn(x: torch.Tensor, norm_w=None, eps: float = 1e-6) -> torch.Tensor:
+    """x as the GEMV multiplies it: bf16(bf16(x * rstd) * norm_w) with rstd in fp32 (the fused RMSNorm
+    prologue), or x itself"""
+    return x if norm_w is None else O.rms_norm(x, norm_w, eps)
+
+
+def gemv_reference(x: torch.Tensor, w, N: int, *, block_rows: int = 8192, need_E: bool = True):
+    """x [M, K] (bf16, already as the kernel multiplies it); w(r0, r1) -> the weight rows r0..r1 in fp64, or
+    an [N, K] tensor.  -> (P, A, E) fp64 [M, N]: P = x W^T, A = |x| |W|^T (what bounds the fp32 accumulation),
+    E = max_k |W_nk x_mk| (one flipped element of x; left unset without need_E).  Row blocks: no full fp64
+    copy of a large W."""
+    rows = w if callable(w) else (lambda r0, r1: w[r0:r1].to(torch.float64))
+    xd = x.to(torch.float64)
+    M = xd.shape[0]
+    P = torch.empty(M, N, dtype=torch.float64, device=x.device)
+    A, E = torch.empty_like(P), torch.empty_like(P)
+    xa = xd.abs()
+    for r0 in range(0, N, block_rows):
+        r1 = min(N, r0 + block_rows)
+        wb = rows(r0, r1)
+        P[:, r0:r1] = xd @ wb.t()
+        wa = wb.abs()
+        A[:, r0:r1] = xa @ wa.t()
+        for m in range(M if need_E else 0):
+            E[m, r0:r1] = (wa * xa[m]).amax(dim=1)
+        del wb, wa
+    return P, A, E
+
+
+class GemvErrors(Bf16Errors):
+    """Bf16Errors for a decode GEMV output [M, N or N/2] with a per-element allowance derived from the kernel's
+    arithmetic, in place of the blanket B_RMS * rms(row).  From gemv_reference's P, A, E and the depth d of the
+    deepest fp32 summation chain (gemv_depth):
+      e_P = ACC * d * A  +  ACC * |bias|  [+ NORM_FLIP * E with the fused RMSNorm]
+    bounds how far the kernel's fp32 value before the epilogue may lie from P (+ bias):
+      * fp32 accumulation: recursive summation of products that enter a chain of d additions errs by at most
+        d * u * sum|products| (u = 2^-24 with round to nearest).  ACC = 2^-23 = 2u: the tensor cores' fp32
+        accumulation inside an mma.sync is not round-to-nearest (it may truncate), which at most doubles u.
+        The chain counts lane terms, the warp tree (5), the k-parts, the cluster ranks, the fp32 row or group
+        scale and the bias add (bounded by u |bias|, the ACC |bias| term).
+      * the fused RMSNorm: the kernel's rstd (rsqrtf of a differently ordered fp32 sum) is not torch's, so
+        an element of bf16(x * rstd) near a rounding tie may round the other way: one ulp, <= 2^-7 of the
+        element, moves P by <= 2^-7 max_k |W_nk x_nk| (NORM_FLIP = 2^-7; the later * norm_w is exact in fp32).
+    Every other operation is an exact fp32 product of bf16 / e4m3 / 4-bit values.  Then, per epilogue:
+      1. per element:  |got - bf16(ref_final)| <= A_ULP * ulp(ref) + allow,  A_ULP = 1, the final rounding
+         (e_P may carry the value across a rounding tie), and allow =
+         * plain, bias, arg-max:  e_P;
+         * residual:  e_P + ulp(bf16(P + bias)): the rounded product before the add may flip (it may cancel
+           against the residual, so this does not scale with the output);
+         * SwiGLU, g = bf16(P_gate), u = bf16(P_up), s = bf16(silu(g)), out = bf16(s u):
+           |g' - g| <= e_g + ulp(g),  |u' - u| <= e_u + ulp(u) = du,  |s' - s| <= 1.1 |g' - g| + ulp(s) = ds
+           (|silu'| <= 1.1), so allow = ds (|u| + du) + |s| du.
+       At K = 18944, d * ACC * A is ~1e-3 of an output's rms, far below its ulp: the element check is as tight as
+       the output's own rounding.  One wrong (row, group) zero point or scale moves its output by s * (sum of the
+       group's x), which is under one ulp for about a quarter of the groups; tests/test_gemv_cpu.py measures 73 %
+       of such faults rejected (57 to 62 % when a residual as large as the output is added).
+    2. per row and 3. rounding bias: as Bf16Errors (ROW_RMS = 2^-7 of the row rms, |bias| <= 0.1 ulp)."""
+    A_ULP = 1.0
+    ACC = 2.0 ** -23
+    NORM_FLIP = 2.0 ** -7
+
+    @classmethod
+    def allowance(cls, P, A, E, *, depth: int, bias=None, residual=False, swiglu=False, norm=False):
+        """-> (ref_final without the residual's values, allow): see the class docstring"""
+        t = P if bias is None else P + bias.to(torch.float64)
+        e = cls.ACC * depth * A
+        if bias is not None:
+            e = e + cls.ACC * bias.to(torch.float64).abs()
+        if norm:
+            e = e + cls.NORM_FLIP * E
+        if swiglu:
+            g, u = _rb64(t[:, 0::2]), _rb64(t[:, 1::2])
+            s = _rb64(torch.nn.functional.silu(g))
+            du = e[:, 1::2] + bf16_ulp(u)
+            ds = 1.1 * (e[:, 0::2] + bf16_ulp(g)) + bf16_ulp(s)
+            return ds * (u.abs() + du) + s.abs() * du
+        if residual:
+            return e + bf16_ulp(_rb64(t))
+        return e
+
+    def add_gemv(self, got, P, A, E, *, depth: int, bias=None, residual=None, swiglu=False, norm=False,
+                 row0: int = 0) -> "GemvErrors":
+        """got [M, N or N/2] against (P, A, E) of gemv_reference; residual [M, N] (the values before the add)"""
+        allow = self.allowance(P, A, E, depth=depth, bias=bias, residual=residual is not None, swiglu=swiglu,
+                               norm=norm)
+        ref_final = linear_reference(P, bias=bias, residual=residual, swiglu=swiglu)
+        return self.add(got, ref_final, row0, allow=allow)
+
+
+def gemv_plan(fmt: str, N: int, K: int, fusion: str, sms: int, *, variant: int = 0, batched: bool = False):
+    """-> (plan, depth, regime label) of the kernel that runs (fmt, N, K, fusion) on `sms` SMs: the single-stream
+    bf16 (variant 0: TMA ring, else register-staged), e4m3 or W4A16 kernel, or (batched) gemv_batch_*"""
+    swiglu, norm = "swiglu" in fusion, "norm" in fusion
+    if batched:
+        p = batch_partition(N, K, fmt == "fp8", sms)
+        kind = "batch-fp8" if fmt == "fp8" else "batch-w4"
+        return p, gemv_depth(kind, K, p), f"cluster {p['cluster']} x {p['tiles_per_cluster']} tiles, {p['parts']} parts"
+    if fmt == "w4a16":
+        p = gemv_w4_plan(N, K, norm, sms)
+        return p, gemv_depth("w4", K, p), f"w4 ksplit {p['ksplit']} x {p['chunk_groups']} groups, {p['tiles_per_block']} tiles/block"
+    p = gemv_tma_plan(N, K, fmt == "fp8", swiglu, norm, sms) if variant == 0 else None
+    if p is None:
+        assert fmt == "bf16", (fmt, N, K)
+        p = gemv_reg_plan(N, K, swiglu, sms)
+        return p, gemv_depth("reg-bf16", K, p), f"register-staged ksplit {p['ksplit']}"
+    kind = "tma-fp8" if fmt == "fp8" else "tma-bf16"
+    return p, gemv_depth(kind, K, p), f"tma ksplit {p['ksplit']}, {p['rows_per_block']} rows/block, {p['stages']} stages"
+
+
+def check_gemv(name: str, got: torch.Tensor, x: torch.Tensor, w, N: int, *, depth: int, norm_w=None, eps=1e-6,
+               bias=None, residual=None, swiglu=False, record: dict = None) -> GemvErrors:
+    """GemvErrors of a GEMV output got [M, N or N/2] for the input rows x [M, K] (before the fused RMSNorm with
+    norm_w) and the weight rows w (gemv_reference), recorded like report_rel; the caller asserts e.failures()"""
+    x = x.reshape(-1, x.shape[-1])
+    P, A, E = gemv_reference(gemv_xn(x, norm_w, eps), w, N, need_E=norm_w is not None)
+    e = GemvErrors().add_gemv(got.reshape(P.shape[0], -1), P, A, E, depth=depth, bias=bias,
+                              residual=None if residual is None else residual.reshape(P.shape[0], -1),
+                              swiglu=swiglu, norm=norm_w is not None)
+    _record({"name": name, **(record or {}), **e.summary()})
+    return e
+
+
+def e4m3_rows(codes: torch.Tensor, s: torch.Tensor):
+    """weight rows in fp64 of ref_quantize_e4m3_rows' (codes, s), for gemv_reference"""
+    vals = e4m3_values().to(codes.device)
+    return lambda r0, r1: vals[codes[r0:r1].long()] * s[r0:r1, None].to(torch.float64)
+
+
+def w4_rows(q: torch.Tensor, s: torch.Tensor, z: torch.Tensor):
+    """weight rows (q - z) * s in fp64 of ref_quantize_w4's (q, s, z), for gemv_reference"""
+    def rows(r0, r1):
+        zz = z[r0:r1].to(torch.float64).repeat_interleave(W4_GROUP, 1)
+        return (q[r0:r1].to(torch.float64) - zz) * s[r0:r1].to(torch.float64).repeat_interleave(W4_GROUP, 1)
+    return rows

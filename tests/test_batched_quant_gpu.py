@@ -1,6 +1,7 @@
 """GPU: the continuous-batching engine on the opt-in FP8 and W4A16 decode weights.
 
-  * vila_gemv_batch_fp8 / vila_gemv_batch_w4a16 against fp32 math on the dequantized copies, at every layer
+  * vila_gemv_batch_fp8 / vila_gemv_batch_w4a16 against the fp64 reference on the dequantized copies
+    (tests.helpers.GemvErrors), at every layer
     shape of NVILA-8B, NVILA-Lite-3B and the tiny test model in both formats, the e4m3 lm_heads and an
     N = 1003 case, for M in {1, 5, 8, 16, 20} with their fusions;
   * row independence: every output row is bit-identical to the same row run alone (M = 1) and to a run in
@@ -16,14 +17,13 @@ import math
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 from tests import test_fp8_decode_gpu as T8
 from tests import test_w4a16_decode_gpu as T4
-from tests.helpers import report_rel
+from tests.helpers import check_gemv, gemv_plan
 from tests.test_decode_engines_gpu import _fp32_truth  # noqa: F401  (autouse: the fp32 oracle is really fp32)
 from tests.test_decode_engines_gpu import _check_untouched, _decoded_rows, _prompt
-from tests.test_fp8_decode_gpu import _check_fp8_sequence, rb
+from tests.test_fp8_decode_gpu import _check_fp8_sequence
 from tests.test_kernels_gpu import _ops, bf
 
 pytestmark = pytest.mark.gpu
@@ -49,7 +49,8 @@ M_VALUES = (1, 5, 8, 16, 20)
 
 
 def _weights(fmt, N, K, seed):
-    """-> (dict of gemv_batch weight arguments, dequantized fp32 [N, K])"""
+    """-> (dict of gemv_batch weight arguments, the dequantized weights: fp32 [N, K] (W4A16, exact), or fp64 rows
+    of q * s (e4m3) for gemv_reference)"""
     g = torch.Generator(device="cuda").manual_seed(seed)
     w = bf(torch.randn(N, K, device="cuda", generator=g) / math.sqrt(K)
            * torch.exp(torch.randn(N, 1, device="cuda", generator=g))
@@ -57,8 +58,8 @@ def _weights(fmt, N, K, seed):
     if fmt == "w4a16":
         q, s, z, deq = T4._quant(w)
         return dict(w=q, w_scale=s, w_zero=z), deq
-    q, s, deq = T8._quant(w)
-    return dict(w=q, w_scale=s), deq
+    q, s, _ = T8._quant(w)
+    return dict(w=q, w_scale=s), lambda r0, r1: q[r0:r1].to(torch.float64) * s[r0:r1, None].to(torch.float64)
 
 
 def _acts(M, K, seed, outliers=False):
@@ -80,16 +81,6 @@ def _run(ops, fusion, x, wa, b, r, inplace=False):
     return ops.gemv_batch(x, static_w=True, **wa)
 
 
-def _reference(fusion, acc, b, r):
-    if fusion == "bias":
-        return rb(acc + b.float()), 2 ** -7
-    if fusion == "residual":
-        return rb(rb(acc) + r.float()), 2 ** -7
-    if fusion == "swiglu":
-        return rb(rb(F.silu(rb(acc[:, 0::2]))) * rb(acc[:, 1::2])), 2 ** -6
-    return acc, 2 ** -7
-
-
 @pytest.mark.parametrize("fmt,name,N,K,fusion", KERNEL_CASES, ids=[f"{c[0]}-{c[1]}-{c[4]}" for c in KERNEL_CASES])
 def test_gemv_batch(cuda, fmt, name, N, K, fusion):
     ops = _ops()
@@ -100,11 +91,13 @@ def test_gemv_batch(cuda, fmt, name, N, K, fusion):
     x = _acts(Mmax, K, seed=K)
     r = bf(torch.randn(Mmax, N, device="cuda", generator=g))
     full = _run(ops, fusion, x, wa, b, r)  # M = 20: two launches
-    acc = x.float() @ deq.T
-    ref, tol = _reference(fusion, acc, b, r)
     assert bool(torch.isfinite(full.float()).all())
-    for m in range(Mmax):  # per output row, against max|ref| of that row
-        report_rel(f"gemv_batch {fmt} {name} {fusion} row {m}", full[m], ref[m], tol)
+    sms = torch.cuda.get_device_properties(cuda).multi_processor_count
+    _, depth, regime = gemv_plan(fmt, N, K, fusion, sms, batched=True)
+    e = check_gemv(f"gemv_batch {fmt} {name} {fusion}", full, x, deq, N, depth=depth,
+                   bias=b if fusion == "bias" else None, residual=r if fusion == "residual" else None,
+                   swiglu=fusion == "swiglu", record=dict(regime=regime))
+    assert not e.failures(), f"gemv_batch {fmt} {name} {fusion}: " + "; ".join(e.failures())
     # outputs past N and x rows past M are never written: out is a slice of a wider sentinel-filled tensor
     n_out = full.shape[1]
     sent = torch.full((Mmax + 1, (n_out + 7) // 8 * 8 + 8), 7.0, dtype=torch.bfloat16, device=cuda)

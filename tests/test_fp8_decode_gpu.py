@@ -1,7 +1,7 @@
 """GPU: opt-in FP8 (e4m3, one fp32 scale per row) weights in the single-stream decoder.
 
-  * vila_gemv_fp8 against fp32 math on the SAME dequantized weights (q.float() * s), at every GEMV shape of
-    NVILA-8B and NVILA-Lite-3B and with every fusion; bit-repeatable, graph replay included;
+  * vila_gemv_fp8 against the fp64 reference on the dequantized weights (tests.helpers.GemvErrors), at every GEMV
+    shape of NVILA-8B and NVILA-Lite-3B and with every fusion; bit-repeatable, graph replay included;
   * GraphDecoder in fp8 mode, teacher-forced like tests/test_decode_engines_gpu.py: the prompt runs through
     the fp32 oracle with the bf16 weights; the first id and every decoded position use an oracle whose LLM
     linear weights and lm_head are the dequantized q * s (embedding and norms unchanged);
@@ -12,10 +12,9 @@ import math
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 from oracle import vila_oracle as O
-from tests.helpers import check_close, oracle_from_state_dict, report_rel
+from tests.helpers import check_close, check_gemv, e4m3_rows, gemv_plan, oracle_from_state_dict, ref_quantize_e4m3_rows
 from tests.test_decode_engines_gpu import _fp32_truth  # noqa: F401  (autouse: the fp32 oracle is really fp32)
 from tests.test_decode_engines_gpu import _CONTEXTS, _PATHS, _check_untouched, _config, _decoded_rows, _prompt
 from tests.test_kernels_gpu import _ops, bf
@@ -82,15 +81,15 @@ def test_gemv_fp8(cuda, name, N, K, fusion):
     out = _launch(ops, fusion, x, q, s, b, r, nw, key)
     xn = O.rms_norm(x[None], nw, 1e-6)[0].float() if "norm" in fusion else x.float()
     acc = deq @ xn
-    if fusion == "bias+norm":
-        ref, tol = rb(acc + b.float()), 2 ** -7
-    elif fusion == "residual":
-        ref, tol = rb(rb(acc) + r.float()), 2 ** -7
-    elif fusion == "swiglu+norm":
-        ref, tol = rb(rb(F.silu(rb(acc[0::2]))) * rb(acc[1::2])), 2 ** -6
-    else:
-        ref, tol = acc, 2 ** -7
-    report_rel(f"gemv_fp8 {name} {fusion}", out, ref, tol)
+    rq, rs = ref_quantize_e4m3_rows(w)
+    assert torch.equal(q.view(torch.uint8), rq) and torch.equal(s, rs)
+    sms = torch.cuda.get_device_properties(cuda).multi_processor_count
+    _, depth, regime = gemv_plan("fp8", N, K, fusion, sms)
+    e = check_gemv(f"gemv_fp8 {name} {fusion}", out[None], x[None], e4m3_rows(rq, rs), N, depth=depth,
+                   norm_w=nw if "norm" in fusion else None, bias=b if fusion == "bias+norm" else None,
+                   residual=r[None] if fusion == "residual" else None, swiglu=fusion == "swiglu+norm",
+                   record=dict(regime=regime))
+    assert not e.failures(), f"gemv_fp8 {name} {fusion}: " + "; ".join(e.failures())
     if key is not None:  # the fused greedy arg-max: a best id of the fp32 reference, up to 3 bf16 ulps
         tok = int(key.item() & 0xFFFFFFFF)
         tok = 0xFFFFFFFF - tok

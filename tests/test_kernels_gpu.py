@@ -484,7 +484,9 @@ def test_rope_kv_append(cuda):
 @pytest.mark.parametrize("N,K", [(4608, 3584), (3584, 3584), (3584, 18944), (512, 2048), (1000, 1536),
                                  (152064, 3584), (37888, 3584), (64, 512)])
 def test_gemv_bias_residual_norm(cuda, N, K, variant):
+    from tests.helpers import check_gemv, gemv_plan
     ops = _ops()
+    sms = torch.cuda.get_device_properties(cuda).multi_processor_count
     g = torch.Generator(device="cuda").manual_seed(N + K)
     x = bf(torch.randn(K, device=cuda, generator=g))
     w = bf(torch.randn(N, K, device=cuda, generator=g) / math.sqrt(K))
@@ -493,16 +495,20 @@ def test_gemv_bias_residual_norm(cuda, N, K, variant):
     nw = bf(torch.randn(K, device=cuda, generator=g))
     out = ops.gemv(x, w, bias=b, residual=r, variant=variant, static_w=True)
     assert torch.equal(out, ops.gemv(x, w, bias=b, residual=r, variant=variant))  # deterministic
-    ref = rb(rb(w.float() @ x.float() + b.float()) + r.float())
-    assert rel_err(out, ref) < 1e-2
+    _, depth, regime = gemv_plan("bf16", N, K, "bias+residual", sms, variant=variant)
+    e = check_gemv(f"gemv bias+residual N={N} K={K} v{variant}", out[None], x[None], w, N, depth=depth, bias=b,
+                   residual=r[None], record=dict(regime=regime))
+    assert not e.failures(), e.failures()
     out = ops.gemv(x, w, norm_w=nw, norm_eps=1e-6, variant=variant)
-    xn = O.rms_norm(x[None], nw, 1e-6)[0]
-    ref = w.float() @ xn.float()
-    assert rel_err(out, ref) < 1e-2
+    _, depth, regime = gemv_plan("bf16", N, K, "norm", sms, variant=variant)
+    e = check_gemv(f"gemv norm N={N} K={K} v{variant}", out[None], x[None], w, N, depth=depth, norm_w=nw,
+                   record=dict(regime=regime))
+    assert not e.failures(), e.failures()
 
 
 @pytest.mark.parametrize("variant", [0, 1])
 def test_gemv_swiglu(cuda, variant):
+    from tests.helpers import check_gemv, gemv_plan
     ops = _ops()
     I, K = 18944, 3584
     g = torch.Generator(device="cuda").manual_seed(21)
@@ -511,11 +517,15 @@ def test_gemv_swiglu(cuda, variant):
     wu = bf(torch.randn(I, K, device=cuda, generator=g) / math.sqrt(K))
     w = torch.stack([wg, wu], dim=1).reshape(2 * I, K).contiguous()
     out = ops.gemv(x, w, swiglu=True, variant=variant, static_w=True)
-    ref = rb(rb(F.silu(rb(wg.float() @ x.float()))) * rb(wu.float() @ x.float()))
-    assert rel_err(out, ref) < 1e-2
+    sms = torch.cuda.get_device_properties(cuda).multi_processor_count
+    _, depth, regime = gemv_plan("bf16", 2 * I, K, "swiglu", sms, variant=variant)
+    e = check_gemv(f"gemv swiglu v{variant}", out[None], x[None], w, 2 * I, depth=depth, swiglu=True,
+                   record=dict(regime=regime))
+    assert not e.failures(), e.failures()
 
 
 def test_gemv_argmax_and_finalize(cuda):
+    from tests.helpers import check_gemv, gemv_plan
     ops = _ops()
     V, K = 152064, 3584
     g = torch.Generator(device="cuda").manual_seed(22)
@@ -534,8 +544,11 @@ def test_gemv_argmax_and_finalize(cuda):
     expect = int(torch.argmax(logits.float()))
     assert int(tok) == expect and int(hist[0]) == expect and int(step) == 1 and int(posn) == 42
     assert int(key) == 0 and torch.equal(xn, table[expect])
+    sms = torch.cuda.get_device_properties(cuda).multi_processor_count
+    _, depth, regime = gemv_plan("bf16", V, K, "argmax", sms)
+    e = check_gemv("gemv argmax lm_head", logits[None], x[None], w, V, depth=depth, record=dict(regime=regime))
+    assert not e.failures(), e.failures()
     ref = w.float() @ x.float()
-    assert rel_err(logits, ref) < 1e-2
     top2 = torch.topk(ref, 2).values
     if (top2[0] - top2[1]) > 0.05:
         assert expect == int(torch.argmax(ref))

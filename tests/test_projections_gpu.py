@@ -1,6 +1,6 @@
 """GPU: every bf16 projection the model issues, at its production shape, in its call form and in every
 GEMM dispatch regime it can reach, against an fp64 reference; and the bf16 decode GEMV at NVILA-Lite-3B's
-shapes.
+shapes (tests.helpers.GemvErrors; the other decode GEMVs run in tests/test_gemv_gpu.py).
 
 Table.  One row per distinct (N, K, epilogue, aliasing), generated from nvila_8b(), nvila_8b_dynamic_s2(),
 nvila_video_8b() and nvila_lite_3b():
@@ -35,7 +35,7 @@ import pytest
 import torch
 
 from oracle import vila_oracle as O
-from tests.helpers import REGIME, Bf16Errors, _record, dispatch_flavour, linear_reference
+from tests.helpers import REGIME, Bf16Errors, _record, check_gemv, dispatch_flavour, gemv_plan, linear_reference
 from tests.test_fp8_decode_gpu import GEMV_CASES
 from tests.test_kernels_gpu import _ops, bf
 
@@ -263,10 +263,12 @@ def test_gemv_bf16_lite(cuda, name, N, K, fusion, variant):
     assert torch.equal(out, again)
     xn = O.rms_norm(x[None], nw, 1e-6)[0] if "norm" in fusion else x
     P = (w.double() @ xn.double())[None]
-    ref_final = linear_reference(P, bias=b if fusion == "bias+norm" else None,
-                                 residual=r[None] if fusion == "residual" else None, swiglu=fusion == "swiglu+norm")
-    e = Bf16Errors().add(out[None], ref_final)
-    _record({"name": "gemv bf16", "layer": name, "N": N, "K": K, "epi": fusion, "variant": variant, **e.summary()})
+    sms = torch.cuda.get_device_properties(cuda).multi_processor_count
+    _, depth, regime = gemv_plan("bf16", N, K, fusion, sms, variant=variant)
+    e = check_gemv("gemv bf16", out[None], x[None], w, N, depth=depth, norm_w=nw if "norm" in fusion else None,
+                   bias=b if fusion == "bias+norm" else None, residual=r[None] if fusion == "residual" else None,
+                   swiglu=fusion == "swiglu+norm",
+                   record=dict(layer=name, N=N, K=K, epi=fusion, variant=variant, regime=regime))
     e.check(f"gemv {name} variant {variant}")
     if key is not None:  # the fused arg-max: the kernel's own logits decide, and it is a best id of fp64
         tok = 0xFFFFFFFF - int(key.item() & 0xFFFFFFFF)

@@ -1,6 +1,7 @@
 """GPU: opt-in W4A16 (4-bit, group-128 scale and zero point) weights in the single-stream decoder.
 
-  * vila_gemv_w4a16 against fp32 math on dequantize_w4_groups' output, at every layer GEMV shape of
+  * vila_gemv_w4a16 against the fp64 reference on the weights of the re-derived quantizer
+    (tests.helpers.ref_quantize_w4, GemvErrors), at every layer GEMV shape of
     NVILA-8B, NVILA-Lite-3B and the tiny test model with their fusions, a short last row block with the
     argmax, and outlier activations; bit-repeatable, graph replay included; every rejection;
   * GraphDecoder in w4a16 mode, teacher-forced as tests/test_fp8_decode_gpu.py does: the oracle's layer
@@ -13,22 +14,29 @@ import math
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 from oracle import vila_oracle as O
-from tests.helpers import oracle_from_state_dict, report_rel
+from tests.helpers import check_gemv, gemv_plan, oracle_from_state_dict, ref_quantize_w4, ref_w4_pack, w4_rows
 from tests.test_decode_engines_gpu import _fp32_truth  # noqa: F401  (autouse: the fp32 oracle is really fp32)
 from tests.test_decode_engines_gpu import _CONTEXTS, _PATHS, _check_untouched, _config, _decoded_rows, _prompt
-from tests.test_fp8_decode_gpu import _check_fp8_sequence, _decode, rb
+from tests.test_fp8_decode_gpu import _check_fp8_sequence, _decode
 from tests.test_kernels_gpu import _ops, bf
 
 pytestmark = pytest.mark.gpu
 
 
 def _quant(w):
-    from vila_b200.model.qwen2 import dequantize_w4_groups, quantize_w4_groups
+    """-> (packed, s, z) of quantize_w4_groups and the weights they stand for, fp32: from the quantizer's rule
+    re-derived in tests.helpers (not from the package's own unpacking), which must give the same bytes"""
+    from vila_b200.model.qwen2 import quantize_w4_groups
     packed, s, z = quantize_w4_groups(w)
-    return packed, s, z, dequantize_w4_groups(packed, s, z)
+    rq, rs, rz = ref_quantize_w4(w)
+    assert torch.equal(s.float(), rs) and torch.equal(z, rz) and torch.equal(packed, ref_w4_pack(rq))
+    rows, N = w4_rows(rq, rs, rz), w.shape[0]
+    deq = torch.empty(w.shape, dtype=torch.float32, device=w.device)  # exact: (q - z) * s has <= 12 bits
+    for r0 in range(0, N, 4096):
+        deq[r0:r0 + 4096] = rows(r0, min(N, r0 + 4096)).float()
+    return packed, s, z, deq
 
 
 # ------------------------------------------------------------------------------------------------
@@ -87,16 +95,14 @@ def test_gemv_w4a16(cuda, name, N, K, fusion):
     out = _launch(ops, fusion, x, q, s, z, b, r, nw, key)
     xn = O.rms_norm(x[None], nw, 1e-6)[0].float() if "norm" in fusion else x.float()
     acc = deq @ xn
-    if fusion == "bias+norm":
-        ref, tol = rb(acc + b.float()), 2 ** -7
-    elif fusion.startswith("residual"):
-        ref, tol = rb(rb(acc) + r.float()), 2 ** -7
-    elif fusion == "swiglu+norm":
-        ref, tol = rb(rb(F.silu(rb(acc[0::2]))) * rb(acc[1::2])), 2 ** -6
-    else:
-        ref, tol = acc, 2 ** -7
     assert bool(torch.isfinite(out.float()).all())
-    report_rel(f"gemv_w4a16 {name} {fusion}", out, ref, tol)
+    sms = torch.cuda.get_device_properties(cuda).multi_processor_count
+    _, depth, regime = gemv_plan("w4a16", N, K, fusion, sms)
+    e = check_gemv(f"gemv_w4a16 {name} {fusion}", out[None], x[None], deq, N, depth=depth,
+                   norm_w=nw if "norm" in fusion else None, bias=b if fusion == "bias+norm" else None,
+                   residual=r[None] if fusion.startswith("residual") else None, swiglu=fusion == "swiglu+norm",
+                   record=dict(regime=regime))
+    assert not e.failures(), f"gemv_w4a16 {name} {fusion}: " + "; ".join(e.failures())
     if key is not None:  # the fused greedy arg-max: a best id of the fp32 reference, up to 3 bf16 ulps
         tok = 0xFFFFFFFF - int(key.item() & 0xFFFFFFFF)
         margin = 3 * 2 ** -8 * acc.abs().max().item()

@@ -165,7 +165,9 @@ def quantize_e4m3_rows(w: torch.Tensor, rows_per_chunk: int = 16384):
     for a in range(0, N, rows_per_chunk):
         wf = w[a:a + rows_per_chunk].float()
         amax = wf.abs().amax(dim=1)
-        sc = torch.where(amax > 0, amax / E4M3_MAX, torch.ones_like(amax))
+        # tensor / tensor: IEEE division on every device (CUDA runs a Python scalar divisor as a multiplication by
+        # its rounded reciprocal, which misses amax / 448 by an ulp for some rows)
+        sc = torch.where(amax > 0, amax / torch.full_like(amax, E4M3_MAX), torch.ones_like(amax))
         q[a:a + rows_per_chunk] = (wf / sc[:, None]).to(torch.float8_e4m3fn)
         s[a:a + rows_per_chunk] = sc
     return q, s
@@ -232,7 +234,7 @@ def quantize_w4_groups(w: torch.Tensor, rows_per_chunk: int = 16384):
         wf = w[a:a + rows_per_chunk].float().view(-1, G, W4_GROUP)
         lo = wf.amin(dim=2).clamp(max=0)
         hi = wf.amax(dim=2).clamp(min=0)
-        sc = ((hi - lo) / 15).to(torch.bfloat16).float()
+        sc = ((hi - lo) / torch.full_like(hi, 15.0)).to(torch.bfloat16).float()  # IEEE division, as above
         sc = torch.where(sc == 0, torch.ones_like(sc), sc)
         zp = torch.round(-lo / sc).clamp(0, 15)
         q = (torch.round(wf / sc[..., None]) + zp[..., None]).clamp(0, 15).to(torch.uint8).view(-1, K)
