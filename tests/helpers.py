@@ -1008,3 +1008,316 @@ def w4_rows(q: torch.Tensor, s: torch.Tensor, z: torch.Tensor):
         zz = z[r0:r1].to(torch.float64).repeat_interleave(W4_GROUP, 1)
         return (q[r0:r1].to(torch.float64) - zz) * s[r0:r1].to(torch.float64).repeat_interleave(W4_GROUP, 1)
     return rows
+
+
+# ------------------------------------------------------------------------------------------------
+# norms and media data movement: exact outside bf16 rounding ties
+# ------------------------------------------------------------------------------------------------
+U32 = 2.0 ** -24  # fp32 unit roundoff (round to nearest)
+
+
+def bf16_rounding_tie_distance(x64: torch.Tensor) -> torch.Tensor:
+    """distance of fp64 x from the nearest bf16 rounding boundary (midpoint of two bf16 neighbours), in
+    fp32 ulps of x (2^-16 of its bf16 ulp)"""
+    a = x64.abs()
+    _, e = torch.frexp(a)
+    ulp = torch.ldexp(torch.ones_like(a), e - 8)  # bf16 ulp of |x| in [2^(e-1), 2^e)
+    frac = torch.remainder(a / ulp, 1.0)
+    return ((frac - 0.5).abs() * 2.0 ** 16).where(a > 0, torch.full_like(a, float("inf")))
+
+
+def bf16_rne64(x: torch.Tensor) -> torch.Tensor:
+    """fp64 -> the nearest bf16 value (ties to even) in ONE rounding, as fp64 (torch's double -> bf16 cast
+    goes through fp32, which double-rounds next to a tie); normal range"""
+    x = x.to(torch.float64)
+    ulp = bf16_ulp(x)
+    return torch.round(x / ulp) * ulp  # x / ulp and the product are exact (powers of two); round: half to even
+
+
+class TieErrors:
+    """Exact-or-tie check of a bf16 output.  Each element comes with ref_final, the fp64 value before the
+    last rounding, and eps, a bound on how far the kernel's fp32 value before that rounding can lie from
+    ref_final.  Rounding is monotone, so the kernel's output lies in [bf16(ref_final - eps), bf16(ref_final +
+    eps)]; where ref_final is further than eps from a bf16 rounding boundary that interval is the one value
+    bf16(ref_final), and the output must equal it bit for bit.  Inside the window either neighbour is accepted,
+    and nothing more, except where eps spans several bf16 values (`wide`: a cancellation), where any of them is.
+    With `then`, the rounding checked is an intermediate one (RMSNorm's bf16(x * rstd)) and the output is
+    then(intermediate): the output must be then(lo) or then(hi).
+    Recorded: n, the elements in a tie window, the flips among them (output != the correctly rounded one),
+    and `needed`, the largest |ref_final - crossed boundary| / eps over the flips: the part of eps the kernel
+    actually used (a lower bound on its error).  failures() rejects a window covering more than
+    max_window of the elements, so a too generous eps fails instead of quietly weakening the check."""
+
+    def __init__(self, max_window: float = 0.02):
+        self.max_window = max_window
+        self.n = self.window = self.wide = self.flips = self.bad = 0
+        self.first_bad = None
+        self.needed = 0.0
+
+    def add(self, got: torch.Tensor, ref_final: torch.Tensor, eps, then=None, where: str = "") -> "TieErrors":
+        got = got.to(torch.float64).reshape(-1)
+        r = ref_final.to(torch.float64).reshape(-1)
+        e = torch.as_tensor(eps, dtype=torch.float64, device=r.device).expand(ref_final.shape).reshape(-1)
+        lo, hi, want = bf16_rne64(r - e), bf16_rne64(r + e), bf16_rne64(r)
+        win = lo != hi
+        # more than two values: a cancellation (LayerNorm's + b near -x_hat w) leaves an absolute fp32 error
+        # larger than the bf16 spacing of the small result; every value in [lo, hi] is then reachable
+        wide = hi > lo + bf16_ulp(torch.minimum(lo.abs(), hi.abs())) * 1.0001
+        self.wide += int(wide.sum())
+        if then is None:
+            ok = (got >= lo) & (got <= hi)
+            flip = got != want
+            mid = (got + want) / 2
+        else:
+            out_lo, out_hi, out_want = (then(t).reshape(-1) for t in (lo, hi, want))
+            ok = (got == out_lo) | (got == out_hi) | (wide & (got >= torch.minimum(out_lo, out_hi))
+                                                     & (got <= torch.maximum(out_lo, out_hi)))
+            flip = got != out_want
+            mid = (lo + hi) / 2
+        self.n += got.numel()
+        self.window += int(win.sum())
+        self.flips += int(flip.sum())
+        nb = int((~ok).sum())
+        if nb and self.first_bad is None:
+            i = int((~ok).nonzero()[0])
+            self.first_bad = (where, i, got[i].item(), want[i].item() if then is None else None, r[i].item())
+        self.bad += nb
+        if bool((flip & ok).any()):
+            used = ((r - mid).abs() / e.clamp_min(1e-300))[flip & ok]
+            self.needed = max(self.needed, float(used.max()))
+        return self
+
+    @property
+    def window_fraction(self) -> float:
+        return self.window / max(self.n, 1)
+
+    def failures(self) -> List[str]:
+        out = []
+        if self.bad:
+            out.append(f"{self.bad} elements outside their exact-or-tie set (first: {self.first_bad})")
+        if self.window_fraction > self.max_window:
+            out.append(f"tie window covers {self.window_fraction:.2%} of the elements > {self.max_window:.2%}")
+        return out
+
+    def summary(self) -> dict:
+        return {"n": self.n, "window": self.window, "window_frac": float(f"{self.window_fraction:.3e}"),
+                "wide": self.wide, "flips": self.flips, "needed": float(f"{self.needed:.3e}")}
+
+    def check(self, name: str) -> None:
+        bad = self.failures()
+        assert not bad, f"{name}: " + "; ".join(bad)
+
+
+NORM_FAMILIES = ("random", "offset", "outlier", "small")
+
+
+def norm_inputs(family: str, rows: int, cols: int, seed: int, device="cpu", rms: bool = False):
+    """bf16 rows [rows, cols] and LayerNorm weight / bias [cols] (RMSNorm uses w only):
+      random:  N(0.3, 2^2);
+      offset:  256 + N(0, 4^2): the mean far above the spread (a residual stream with large offsets), so the
+               fp32 mean's error is what the eps of the check has to cover;
+      outlier: N(0, 1) with three channels at +-300 (alternating sign per row): outlier-dominated statistics;
+      small:   N(0, 1e-3^2): the variance (mean square) is the size of the norm's eps, so a wrong eps moves
+               every element;
+      constant (not in NORM_FAMILIES, checked exactly): every row one value (LayerNorm) or zero (RMSNorm)."""
+    g = torch.Generator(device=device).manual_seed(seed)
+    x = torch.randn(rows, cols, generator=g, device=device)
+    if family == "random":
+        x = x * 2 + 0.3
+    elif family == "offset":
+        x = 256 + 4 * x
+    elif family == "outlier":
+        sign = 1 - 2 * (torch.arange(rows, device=device) % 2).to(x.dtype)
+        for c in (3, cols // 2, cols - 5):
+            x[:, c] = 300 * sign
+    elif family == "small":
+        x = x * 1e-3
+    elif family == "constant":
+        x = torch.zeros_like(x) if rms else torch.randn(rows, 1, generator=g, device=device).expand(rows, cols) * 8
+    else:
+        raise ValueError(family)
+    w = 1 + 0.25 * torch.randn(cols, generator=g, device=device)
+    b = 0.5 * torch.randn(cols, generator=g, device=device)
+    bf = torch.bfloat16
+    return x.to(bf).contiguous(), w.to(bf), b.to(bf)
+
+
+NORM_THREADS = 256
+WARP_ROW_MIN_ROWS = 8192  # norm.cu kWarpRowMinRows
+WARP_ROW_MAX_COLS = 8 * 256  # the warp-per-row kernels hold 8 vectors of 8 per lane
+
+
+def norm_plan(rows: int, cols: int) -> dict:
+    """layernorm_bf16 / rmsnorm_bf16's choice (norm.cu): the warp-per-row kernel for rows >= 8192 and cols <=
+    2048, else one CTA of 256 threads per row.  chain: fp32 additions a value passes through in one thread's
+    partial sum (8 per 16-byte vector: 7 inside the vector's expression, 1 into the sum, times the vectors a
+    thread or lane owns); warp: the xor-shuffle tree (5); block: the tree over the 8 warps' partials (5, a
+    warp_sum with zeros).  depth = their sum, the deepest summation chain of the row sum."""
+    nvec = cols // 8
+    if rows >= WARP_ROW_MIN_ROWS and cols <= WARP_ROW_MAX_COLS:
+        regime, chain, block = "warp", 8 * _cdiv(nvec, 32), 0
+    else:
+        regime, chain, block = "cta", 8 * _cdiv(nvec, NORM_THREADS), 5
+    return dict(regime=regime, chain=chain, warp=5, block=block, depth=chain + 5 + block)
+
+
+def _gamma(n) -> float:
+    return n * U32 / (1 - n * U32)
+
+
+def _row_blocks(rows: int, cols: int, budget: int = 1 << 24):
+    step = max(1, budget // max(cols, 1))
+    for r0 in range(0, rows, step):
+        yield r0, min(rows, r0 + step)
+
+
+def layernorm_reference(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor, eps: float, depth: int):
+    """nn.LayerNorm in fp64 (one rounding, at the output), in row blocks: yields (r0, r1, ref_final, eps_elem).
+    eps_elem bounds |the kernel's fp32 value before its bf16 rounding - ref_final| (u = 2^-24, gamma_n = n u /
+    (1 - n u), d = depth of norm_plan, m the exact mean, v the exact variance, rstd = 1 / sqrt(v + eps)):
+      * the mean: the fp32 row sum errs by <= gamma_d sum|x|, the division by cols by u |m|:
+            delta = gamma_d sum|x| / cols + u |m|;
+        unless the sum is exact (every partial sum a multiple of the row's smallest bf16 ulp below 2^24 of
+        them, see mean_eps), when delta is the division's own error, computed exactly;
+      * the variance: the centred values are (x_i - m - delta)(1 + theta_i), |theta_i| <= u; the cross term of
+        delta sums to zero (sum(x - m) = 0), so the sum of their squares is within (1 + 2u)^2 of v cols +
+        delta^2 cols, and the fp32 sum of squares adds gamma_d; the division by cols and the + eps round once
+        each:  rel_var = (gamma_(d+3) v + delta^2) / (v + eps) + 2 u;
+      * rsqrtf: 2 ulps, <= 2^-22 relative; rsqrt halves the relative error of its argument:
+            rel_rstd = rel_var / 2 + 2^-22;
+      * the epilogue: x - mean, * rstd and * w round once each (u of |x - m| rstd |w|, whether or not the last
+        product is fused into the + b), the + b once (u of the result):
+            eps_elem = |w| rstd (delta + |x - m| (rel_rstd + 3 u)) (1 + 4 u) + u |ref_final| (1 + u).
+    The mean term matters when the mean is much larger than the spread (delta grows with sum|x|, rstd with
+    1 / spread)."""
+    cols = x.shape[-1]
+    x2 = x.reshape(-1, cols)
+    wd, bd = w.to(torch.float64), b.to(torch.float64)
+    for r0, r1 in _row_blocks(x2.shape[0], cols):
+        xd = x2[r0:r1].to(torch.float64)
+        m = xd.mean(dim=1, keepdim=True)
+        c = xd - m
+        v = c.pow(2).mean(dim=1, keepdim=True)
+        rstd = (v + eps).rsqrt()
+        ref = c * rstd * wd + bd
+        sa = xd.abs().sum(dim=1, keepdim=True)
+        delta = torch.where(sa < 2.0 ** 24 * _min_ulp(xd).amin(dim=1, keepdim=True),  # exact fp32 sum
+                            ((xd.sum(dim=1, keepdim=True).float() / cols).double() - m).abs(),
+                            _gamma(depth) * sa / cols + U32 * m.abs())
+        rel_var = (_gamma(depth + 3) * v + delta.pow(2)) / (v + eps) + 2 * U32
+        rel_rstd = rel_var / 2 + 2.0 ** -22
+        e = wd.abs() * rstd * (delta + c.abs() * (rel_rstd + 3 * U32)) * (1 + 4 * U32) + U32 * ref.abs() * (1 + U32)
+        yield r0, r1, ref, e
+
+
+def rmsnorm_reference(x: torch.Tensor, eps: float, depth: int):
+    """Qwen2RMSNorm's first rounding point in fp64, in row blocks: yields (r0, r1, t, eps_elem) with t = x rstd,
+    rstd = 1 / sqrt(mean(x^2) + eps).  The output is bf16(w * bf16(t)): w * bf16(t) is a product of two bf16
+    values, exact in fp32, so its rounding is exact too and the only inexact step is t.  eps_elem bounds |the
+    kernel's fp32 x * rstd' - t|: the sum of squares (every term >= 0) errs by gamma_(d+1) relative, the division
+    and + eps by u each, rsqrtf by 2^-22 and halves its argument's error, the product by u:
+        eps_elem = |t| ((gamma_(d+1) + 2 u) / 2 + 2^-22 + u) (1 + u).
+    A flip of bf16(t) inside that window moves the output by |w| ulp(bf16(t)) before its own rounding."""
+    cols = x.shape[-1]
+    x2 = x.reshape(-1, cols)
+    for r0, r1 in _row_blocks(x2.shape[0], cols):
+        xd = x2[r0:r1].to(torch.float64)
+        t = xd * (xd.pow(2).mean(dim=1, keepdim=True) + eps).rsqrt()
+        rel = (_gamma(depth + 1) + 2 * U32) / 2 + 2.0 ** -22 + U32
+        yield r0, r1, t, t.abs() * rel * (1 + U32)
+
+
+def rmsnorm_then(w: torch.Tensor):
+    """the output as a function of the intermediate bf16(x rstd) [rows, cols] (flattened): bf16(w * m)"""
+    wd = w.to(torch.float64)
+    return lambda m: bf16_rne64(m.reshape(-1, wd.shape[0]) * wd)
+
+
+def mean_eps(n, sum_abs: torch.Tensor, mean: torch.Tensor, inv: bool, min_ulp: torch.Tensor) -> torch.Tensor:
+    """bound on |fp32 mean of n bf16 values - exact mean| (n a number or a tensor of window sizes):
+      * the sequential sum: every value, so every partial sum, is a multiple of the smallest bf16 ulp among
+        them (min_ulp), and a multiple of it below 2^24 min_ulp in magnitude is an fp32 number: where sum|v| is
+        below that, the sum is exact; elsewhere it errs by <= gamma_(n-1) sum|v|;
+      * then either a division by n (u |mean|) or (inv) a product with fl(1 / n) (u for the reciprocal, u for
+        the product).  After an exact sum that last step is one fp32 operation on known values, so its
+        error is computed exactly instead of bounded.
+    This matters: the mean of two bf16 values of one binade is a bf16 rounding tie half the time, and fp32
+    computes it exactly, so round-to-nearest-even decides it, with no tie window."""
+    n = torch.as_tensor(n, dtype=torch.float64, device=mean.device)
+    exact_sum = sum_abs < 2.0 ** 24 * min_ulp
+    e_sum = torch.where(exact_sum, torch.zeros_like(sum_abs), (n - 1) * U32 / (1 - (n - 1) * U32) * sum_abs / n)
+    # with an exact sum s the last step is one known fp32 operation: its result is computed exactly here
+    s = torch.round(mean * n / min_ulp.clamp(max=1e300)) * min_ulp  # the sum, snapped to its grid
+    if inv:
+        r = (1.0 / n).to(torch.float32).to(torch.float64)
+        one = (s * r).to(torch.float32).to(torch.float64)  # s * fl(1/n): 48 bits, exact in fp64
+    else:
+        one = (s / n).to(torch.float32).to(torch.float64)  # fp32 division: correctly rounded
+    e_exact = (one - mean).abs()
+    e_div = torch.where(exact_sum & torch.isfinite(e_exact), e_exact,
+                        (2 if inv else 1) * U32 * mean.abs() * (1 + U32))
+    return e_sum + e_div
+
+
+def _min_ulp(v: torch.Tensor) -> torch.Tensor:
+    """bf16 ulp of each value, +inf at zeros (which are multiples of anything)"""
+    return torch.where(v != 0, bf16_ulp(v), torch.full_like(v, float("inf")))
+
+
+def s2_merge_reference(tiles: torch.Tensor, splits_h, splits_w, out_bh: int, out_bw: int, share_tile=False):
+    """the dynamic-S2 merge of ONE image in fp64, as the reference composes it (oracle.merge_chessboard per scale,
+    F.interpolate(mode="area") == F.adaptive_avg_pool2d, the channel concatenation, oracle.split_chessboard),
+    plus the fp32 bound of the kernel's windowed mean (mean_eps with the reciprocal).  tiles [n, side^2, C]
+    -> (ref_final, eps) [out_bh * out_bw, side^2, n_scales * C]."""
+    import torch.nn.functional as F
+    n, N, C = tiles.shape
+    side = int(round(N ** 0.5))
+    t = tiles.to(torch.float64)
+    OH, OW = out_bh * side, out_bw * side
+    refs, epss = [], []
+    cnt = 0
+    for sh, sw in zip(splits_h, splits_w):
+        k = sh * sw
+        src = t[0:1] if share_tile else t[cnt:cnt + k]
+        if not share_tile:
+            cnt += k
+        fmap = O.merge_chessboard(src, sh, sw) if not share_tile else \
+            src.reshape(1, side, side, C).permute(0, 3, 1, 2)
+        ref = F.adaptive_avg_pool2d(fmap, (OH, OW))
+        sa = F.adaptive_avg_pool2d(fmap.abs(), (OH, OW))
+        mu = -F.adaptive_max_pool2d(-_min_ulp(fmap), (OH, OW))
+        # window sizes: [floor(o I / O), ceil((o + 1) I / O))
+        IH, IW = fmap.shape[-2:]
+        oy, ox = torch.arange(OH), torch.arange(OW)
+        ny = (((oy + 1) * IH + OH - 1) // OH - (oy * IH) // OH).to(torch.float64)
+        nx = (((ox + 1) * IW + OW - 1) // OW - (ox * IW) // OW).to(torch.float64)
+        nwin = (ny[:, None] * nx[None, :]).to(t.device)
+        e = mean_eps(nwin, sa * nwin, ref, inv=True, min_ulp=mu)
+        refs.append(ref)
+        epss.append(e)
+
+    def split(m):
+        return O.split_chessboard(torch.cat(m, dim=1), out_bh, out_bw).flatten(2).transpose(1, 2)
+    return split(refs), split(epss)
+
+
+def tsp_pool_reference(x: torch.Tensor, pt: int, ph: int, pw: int):
+    """TSP pooling in fp64 with the reference's three bf16 rounding points (t-mean, then h-mean, then w-mean,
+    each rounded: three chained .mean() on bf16 tensors).  x [T, h, w, C] -> (ref_final, eps) of the last
+    rounding, [T/pt, h/ph, w/pw, C].  An earlier rounding that lies within its own eps of a tie may go either
+    way in fp32; each such possible flip widens the next stage's eps by its ulp / pool (so the window of the
+    final rounding includes every value a flipped intermediate can lead to)."""
+    T, h, w, C = x.shape
+    v = x.to(torch.float64)
+    extra = torch.zeros_like(v)
+    for dim, p in ((0, pt), (1, ph), (2, pw)):
+        shp = v.shape[:dim] + (v.shape[dim] // p, p) + v.shape[dim + 1:]
+        grp = v.reshape(shp)
+        mean = grp.mean(dim + 1)
+        e = mean_eps(p, grp.abs().sum(dim + 1), mean, inv=False, min_ulp=_min_ulp(grp).amin(dim + 1)) \
+            + extra.reshape(shp).sum(dim + 1) / p
+        if dim == 2:
+            return mean, e
+        v = bf16_rne64(mean)
+        win = bf16_rne64(mean - e) != bf16_rne64(mean + e)
+        extra = torch.where(win, bf16_ulp(v), torch.zeros_like(v))

@@ -27,7 +27,8 @@ import pytest
 import torch
 
 from oracle import vila_oracle as O
-from tests.helpers import ATTN_FAMILIES, AttnErrors, _record, attention_errors, attention_inputs
+from tests.helpers import (ATTN_FAMILIES, AttnErrors, _record, attention_errors, attention_inputs,
+                           bf16_rounding_tie_distance)
 from tests.test_kernels_gpu import _ops
 
 pytestmark = pytest.mark.gpu
@@ -282,16 +283,6 @@ def _inv_freq(D, dev):
     return O.rope_inv_freq(D, 1e6).to(dev)  # = Qwen2ForCausalLM.inv_freq (fp32)
 
 
-def _bf16_rounding_tie_distance(x64):
-    """distance of fp64 x from the nearest bf16 rounding boundary (midpoint of two bf16 neighbours), in
-    fp32 ulps of x"""
-    a = x64.abs()
-    _, e = torch.frexp(a)
-    ulp = torch.ldexp(torch.ones_like(a), e - 8)  # bf16 ulp of |x| in [2^(e-1), 2^e)
-    frac = torch.remainder(a / ulp, 1.0)
-    return ((frac - 0.5).abs() * 2.0 ** 16).where(a > 0, torch.full_like(a, float("inf")))
-
-
 def test_rope_table_exact(cuda):
     """rope_table == bf16(cos / sin in fp64 of the fp32 angle fp32(pos) * inv_freq), except entries within
     4 fp32 ulps of a bf16 rounding boundary (sincosf is accurate to ~1 fp32 ulp), which may be one bf16 ulp
@@ -305,7 +296,7 @@ def test_rope_table_exact(cuda):
         x64 = torch.cat([torch.cos(ang.double()), torch.sin(ang.double())], dim=1)
         want = x64.to(torch.bfloat16)
         diff = tab != want
-        near = _bf16_rounding_tie_distance(x64) < 4.0
+        near = bf16_rounding_tie_distance(x64) < 4.0
         off_ulps = (tab.double() - want.double()).abs() / torch.ldexp(torch.ones_like(x64), torch.frexp(
             torch.maximum(tab.double().abs(), want.double().abs()))[1] - 8)
         _record({"name": "rope_table exact", "D": D, "positions": SP_MAX_POS, "entries": tab.numel(),

@@ -202,42 +202,6 @@ def test_linear_swiglu(cuda):
 
 
 # ------------------------------------------------------------------------------------------------
-# norms
-# ------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("rows,cols", [(1024, 1152), (256, 4608), (7, 13824), (121, 3456),
-                                       (16384, 1152), (8195, 144), (9000, 2048), (8192, 2056)])  # >= 8192 rows: warp-per-row kernel (cols <= 2048)
-def test_layernorm(cuda, rows, cols):
-    ops = _ops()
-    g = torch.Generator(device="cuda").manual_seed(rows + cols)
-    x = bf(torch.randn(rows, cols, device=cuda, generator=g) * 3 + 0.5)
-    w = bf(torch.randn(cols, device=cuda, generator=g))
-    b = bf(torch.randn(cols, device=cuda, generator=g))
-    out = ops.layernorm(x, w, b, 1e-6)
-    ref = F.layer_norm(x.float(), (cols,), w.float(), b.float(), 1e-6)
-    assert rel_err(out, ref) < 5e-3
-
-
-@pytest.mark.parametrize("rows,cols", [(280, 3584), (1, 3584), (33, 2048),
-                                       (16470, 3584), (8193, 2048), (8200, 4096), (8192, 512)])  # >= 8192 rows: warp-per-row kernel
-def test_rmsnorm(cuda, rows, cols):
-    ops = _ops()
-    g = torch.Generator(device="cuda").manual_seed(rows + cols)
-    x = bf(torch.randn(rows, cols, device=cuda, generator=g) * 2)
-    w = bf(torch.randn(cols, device=cuda, generator=g))
-    out = ops.rmsnorm(x.clone(), w, 1e-6)
-    ref = O.rms_norm(x, w, 1e-6)  # bf16 in, reference rounding points
-    assert rel_err(out, ref) < 1e-6 + 2 ** -7  # at most one bf16 ulp apart
-    assert (out.float() - ref.float()).abs().mean().item() < 1e-4
-    # fused residual add
-    r = bf(torch.randn(rows, cols, device=cuda, generator=g))
-    x2 = x.clone()
-    out2 = ops.rmsnorm(x2, w, 1e-6, residual_add=r)
-    xs = x + r
-    assert torch.equal(x2, xs)
-    assert rel_err(out2, O.rms_norm(xs, w, 1e-6)) < 2 ** -7
-
-
-# ------------------------------------------------------------------------------------------------
 # attention
 # ------------------------------------------------------------------------------------------------
 def ref_attention(q, k, v, causal, scale):
@@ -370,76 +334,6 @@ def test_fmha2_lazy_rescale_growing_maxima(cuda):
             out = ops.fmha(q, k, v, B=1, Sq=S, Sk=S, causal=causal, scale=D ** -0.5, variant=variant)
             assert torch.isfinite(out.float()).all()
             report_rel(f"fmha{variant} growing maxima d={D}", out, ref, 1.5e-2)
-
-
-# ------------------------------------------------------------------------------------------------
-# data movement (bit-exact unless averaged)
-# ------------------------------------------------------------------------------------------------
-def test_patch_im2col(cuda):
-    ops = _ops()
-    g = torch.Generator(device="cuda").manual_seed(12)
-    px = bf(torch.randn(3, 3, 56, 84, device=cuda, generator=g))
-    out = ops.patch_im2col(px, 14, 592)
-    ref = F.unfold(px.float(), kernel_size=14, stride=14).transpose(1, 2).reshape(-1, 588)
-    assert torch.equal(out[:, :588].float(), ref)
-    assert out[:, 588:].abs().max() == 0
-
-
-@pytest.mark.parametrize("h,w,r", [(32, 32, 2), (27, 27, 2), (32, 32, 3), (27, 27, 3), (5, 7, 2)])
-def test_space_to_depth(cuda, h, w, r):
-    ops = _ops()
-    g = torch.Generator(device="cuda").manual_seed(h * w + r)
-    x = bf(torch.randn(2, h * w, 64, device=cuda, generator=g))
-    out = ops.space_to_depth(x, h, w, r)
-    ref = O.flat_square(x.view(2, h, w, 64), r)
-    assert torch.equal(out, ref.reshape(2, -1, ref.shape[-1]))
-
-
-@pytest.mark.parametrize("idx", [-1, 0, 1])
-def test_s2_merge_and_chessboard(cuda, idx):
-    ops = _ops()
-    side, Cc = 4, 16
-    scales = [4, 8, 12]
-    bs = (2, 3)
-    g = torch.Generator(device="cuda").manual_seed(13)
-    tiles = bf(torch.randn(1 + 4 + 6, side * side, Cc, device=cuda, generator=g))
-    feats, nbs = O.merge_features_for_dynamic_s2(tiles, [bs], scales, idx)
-    ref = O.split_chessboard(feats[0], nbs[0][0], nbs[0][1]).flatten(2).transpose(1, 2)
-    out = ops.s2_merge(tiles, [1, 2, bs[0]], [1, 2, bs[1]], nbs[0][0], nbs[0][1])
-    assert out.shape == ref.shape
-    assert (out.float() - ref.float()).abs().max().item() <= 2 ** -7 * ref.float().abs().max().item()
-    # single-tile image (block_size None): features repeated over scales
-    f1, nb1 = O.merge_features_for_dynamic_s2(tiles[:1], [None], scales, idx)
-    ref1 = f1[0].flatten(2).transpose(1, 2)
-    out1 = ops.s2_merge(tiles[:1], [1, 1, 1], [1, 1, 1], 1, 1, share_tile=True)
-    assert torch.equal(out1, ref1)
-    # chessboard merge of projected tiles
-    proj = bf(torch.randn(6, 4, 32, device=cuda, generator=g))
-    refm = O.merge_chessboard(proj, 2, 3)[0].flatten(1).transpose(0, 1)
-    assert torch.equal(ops.chessboard_merge(proj, 2, 3), refm)
-
-
-def test_tsp_pool(cuda):
-    ops = _ops()
-    g = torch.Generator(device="cuda").manual_seed(14)
-    x = bf(torch.randn(16, 4, 4, 64, device=cuda, generator=g))
-    for ps in [(8, 1, 1), (4, 2, 2), (1, 1, 1)]:
-        ref = x
-        for dim, pp in enumerate(ps):
-            ref = O.tsp_pool(ref, pp, dim)
-        out = ops.tsp_pool(x, *ps)
-        assert (out.float() - ref.float()).abs().max().item() <= 2 ** -7 * ref.float().abs().max().item()
-
-
-def test_embed_splice(cuda):
-    ops = _ops()
-    g = torch.Generator(device="cuda").manual_seed(15)
-    table = bf(torch.randn(100, 256, device=cuda, generator=g))
-    media = bf(torch.randn(10, 256, device=cuda, generator=g))
-    src = torch.tensor([5, 7, -1, -2, -3, 99, 0, -10], dtype=torch.int32, device=cuda)
-    out = ops.embed_splice(table, media, src)
-    ref = torch.stack([table[s] if s >= 0 else media[-(s + 1)] for s in src.tolist()])
-    assert torch.equal(out, ref)
 
 
 def test_rope_kv_append(cuda):
