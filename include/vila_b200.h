@@ -420,6 +420,38 @@ typedef struct vila_sample_finalize_params {
 int vila_sample_finalize(const vila_sample_finalize_params* p, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * vila_token_logprobs — the log-probability of each row's chosen token and its n most likely alternatives, for
+ * M rows of bf16 logits [M, V] (row stride ld), under the raw model distribution (temperature 1, no top-k / top-p,
+ * whatever the row was sampled with).  Replaces HF generate(output_scores=True) + torch.log_softmax over the
+ * scores, and gives OpenAI's `logprobs` / `top_logprobs` of a chat completion.  The rule (vila_b200/logprobs.py
+ * states it in numpy), for row x, its token t = tokens[row] and n:
+ *   m = max float(x_i), Z = sum_i exp(float(x_i) - m), lse = m + log Z
+ *   logprob(t) = float(x_t) - lse
+ *   top = the first n indices of a stable sort by float(x_i) descending (ties to the lower index), with their
+ *         values float(x_j) - lse
+ * The kernel computes (float(x_j) - m) - log Z in fp32 (expf / logf), within 1e-5 + 1e-6 |lp| of the rule in fp64;
+ * the top ids are exact, and the token's value equals its entry in top bit for bit.  Results go straight into
+ * history buffers at column c = min(step[row], cols - 1): lp_hist[row * cols + c] (fp32), top_ids / top_lp
+ * [(row * cols + c) * n + j] (int32 / fp32, j = 0 best).  A row with position < 0 is idle: nothing is written.
+ * tokens and step are int64, position int32.  A row's bits depend on its logits only: not on M, on the row index
+ * or on the other rows (fixed-order fp32 sums, no float atomics).  1 <= V <= 327,680, M <= 65535, 0 <= n <= 20 and
+ * n <= V (top_ids / top_lp may be NULL when n == 0), cols >= 1; the argument errors are reported before any device
+ * call.  One cluster of 8 CTAs per row, PDL.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct vila_logprobs_params {
+  const void* logits;
+  int64_t ld;
+  const int64_t* tokens;
+  const int64_t* step;
+  const int32_t* position;
+  float* lp_hist;
+  int32_t* top_ids;
+  float* top_lp;
+  int32_t M, V, cols, n;
+} vila_logprobs_params;
+int vila_token_logprobs(const vila_logprobs_params* p, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * vila_prefix_block_hash — a 128-bit digest of every full 128-row block of a bf16 matrix x [rows, cols] (row
  * stride ld elements), for prefix caching in the continuous-batching engine: out [rows / 128][2] (uint64).  The
  * reference has no counterpart: it prefills every request in full (serving/server.py:65-73, llava_arch.py:823-833).

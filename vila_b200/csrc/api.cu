@@ -447,6 +447,24 @@ int vila_sample_finalize(const vila_sample_finalize_params* p, void* stream) {
   return vb::sample_finalize(d, st(stream));
 }
 
+// HF generate(output_scores=True) + torch.log_softmax / OpenAI logprobs for the batched engine
+int vila_token_logprobs(const vila_logprobs_params* p, void* stream) {
+  VB_CHECK(p != nullptr, "vila_token_logprobs: params are required");
+  vb::LogprobParams d;
+  d.logits = cb(p->logits);
+  d.ld = p->ld;
+  d.tokens = p->tokens;
+  d.step = p->step;
+  d.position = p->position;
+  d.lp_hist = p->lp_hist;
+  d.top_ids = p->top_ids;
+  d.top_lp = p->top_lp;
+  d.M = p->M; d.V = p->V; d.cols = p->cols; d.n = p->n;
+  if (int rc = vb::token_logprobs_check(d)) return rc;
+  VB_REQUIRE_DEVICE();
+  return vb::token_logprobs(d, st(stream));
+}
+
 // the reference prefills every request in full (serving/server.py:65-73, llava_arch.py:823-833): no seam
 int vila_prefix_block_hash(const void* x, int64_t ld, int64_t rows, int64_t cols, uint64_t key0, uint64_t key1,
                            uint64_t* out, void* stream) {

@@ -268,6 +268,21 @@ struct SampleFinalizeParams {
 };
 int sample_finalize_check(const SampleFinalizeParams& p);  // the argument errors, before any device call
 int sample_finalize(const SampleFinalizeParams& p, cudaStream_t stream);
+// per-row log-probability of the chosen token and the n best tokens (vila_b200/logprobs.py's rule), written at
+// column min(step[row], cols - 1) of the engine's history buffers
+struct LogprobParams {
+  const __nv_bfloat16* logits;  // [M, ld]
+  int64_t ld;                   // row stride (elements), >= V
+  const int64_t* tokens;        // [M] the chosen token of each row
+  const int64_t* step;          // [M] history column
+  const int32_t* position;      // [M] < 0: idle row, nothing written
+  float* lp_hist;               // [M, cols]
+  int32_t* top_ids;             // [M, cols, n] (null when n == 0)
+  float* top_lp;                // [M, cols, n] (null when n == 0)
+  int M, V, cols, n;
+};
+int token_logprobs_check(const LogprobParams& p);  // the argument errors, before any device call
+int token_logprobs(const LogprobParams& p, cudaStream_t stream);
 
 // ---- block digests for prefix caching in the batched engine (prefix_hash.cu) ----------------------------
 // out[b] = (d_0, d_1) of every full 128-row block b of x [rows, cols] bf16 (row stride ld elements); the rule is

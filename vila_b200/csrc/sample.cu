@@ -27,6 +27,9 @@
 //
 // Replaces HF TemperatureLogitsWarper / TopKLogitsWarper / TopPLogitsWarper + torch.multinomial in
 // GenerationMixin._sample, reached from llava_arch.py:823-833.
+//
+// vila_token_logprobs (token_logprobs_kernel, below the samplers so that it shares their cluster helpers) gives the
+// batched engine each chosen token's log-probability and its top alternatives under the raw model distribution.
 #include <math.h>
 
 #include "common.cuh"
@@ -439,8 +442,216 @@ __global__ void __launch_bounds__(kSampThreads, 2) sample_finalize_kernel(Finali
   cluster_sync_all();  // no CTA leaves while another reads its shared memory
 }
 
+// ---- vila_token_logprobs ----------------------------------------------------------------------------------------
+// The rule (vila_b200/logprobs.py states it in numpy): m = max float(x), Z = sum exp(float(x_i) - m); the chosen
+// token's value and those of the first n indices of a stable descending sort (ties to the lower index) are
+// (float(x_j) - m) - log Z.  One cluster of kSampCluster CTAs per row, each holding its slice of float(x) in shared
+// memory: a max pass (cta_argmax / cluster_argmax), a fixed-order fp32 exp-sum per CTA added in rank order, n rounds of
+// a CTA arg-max over the slice that excludes the winners already taken, then a rank-ordered merge of the cluster's
+// kC * n candidates on rank 0.  The slice of a row follows from V alone and every sum runs in a fixed order, so a
+// row's bits depend on that row only.
+
+constexpr int kLpMaxTop = 20;
+
+struct LogprobArgs {
+  const __nv_bfloat16* logits;
+  int64_t ld;
+  const int64_t* tokens;
+  const int64_t* step;
+  const int32_t* position;
+  float* lp_hist;
+  int32_t* top_ids;
+  float* top_lp;
+  int V, slice, cols, n;
+};
+
+struct LogprobScratch {
+  SampleScratch s;  // first: cta_argmax / cluster_argmax work on it
+  float warp_z[kSampWarps];
+  double cta_z;               // this CTA's exp-sum (fp32 value), read by rank 0 through DSMEM
+  float round_v[2][kSampWarps];  // per-warp winners of a top-n round, double-buffered by round parity
+  int round_i[2][kSampWarps];
+  double cand_v[kLpMaxTop];   // this CTA's top-n, best first (index INT_MAX: the slice ran out)
+  int cand_i[kLpMaxTop];
+  float all_v[kSampCluster * kLpMaxTop];  // rank 0: every CTA's candidates
+  int all_i[kSampCluster * kLpMaxTop];
+  float log_z;
+};
+
+// the best (value, index) of this thread's elements of the slice (NaN marks a value already taken)
+__device__ __forceinline__ void thread_best(const float* s_sh, int n_local, int base, float* bv, int* bi) {
+  float v = -INFINITY;
+  int i = INT_MAX;
+  for (int j = threadIdx.x * 4; j < n_local; j += kSampThreads * 4) {
+    const float4 s4 = *reinterpret_cast<const float4*>(s_sh + j);
+    const float s[4] = {s4.x, s4.y, s4.z, s4.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+      if (j + e < n_local && (s[e] > v || (s[e] == v && base + j + e < i))) v = s[e], i = base + j + e;
+  }
+  *bv = v;
+  *bi = i;
+}
+
+__global__ void __launch_bounds__(kSampThreads, 2) token_logprobs_kernel(LogprobArgs a) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  LogprobScratch& sc = *reinterpret_cast<LogprobScratch*>(smem);
+  float* s_sh = reinterpret_cast<float*>(smem + ((sizeof(LogprobScratch) + 15) & ~size_t(15)));
+  griddep_wait();
+  griddep_launch_dependents();
+  const int row = blockIdx.y;
+  if (a.position[row] < 0) return;  // idle row: the whole cluster leaves, nothing is written
+  const uint32_t rank = cluster_ctarank();
+  const int base = static_cast<int>(rank) * a.slice;
+  const int n_local = max(0, min(a.slice, a.V - base));
+  const __nv_bfloat16* lrow = a.logits + static_cast<int64_t>(row) * a.ld + base;
+  const bool vec = (reinterpret_cast<uintptr_t>(lrow) & 7) == 0;
+
+  // pass 1: float(x) into shared memory and the slice's first arg-max
+  float best = -INFINITY;
+  int best_i = INT_MAX;
+  for (int j = threadIdx.x * 4; j < n_local; j += kSampThreads * 4) {
+    float v[4];
+    if (vec && j + 4 <= n_local) {
+      const uint2 w = *reinterpret_cast<const uint2*>(lrow + j);
+      v[0] = bf_lo(w.x); v[1] = bf_hi(w.x); v[2] = bf_lo(w.y); v[3] = bf_hi(w.y);
+    } else {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) v[e] = j + e < n_local ? __bfloat162float(lrow[j + e]) : 0.f;
+    }
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+      if (j + e < n_local && (v[e] > best || (best_i == INT_MAX && v[e] == v[e]))) best = v[e], best_i = base + j + e;
+    *reinterpret_cast<float4*>(s_sh + j) = make_float4(v[0], v[1], v[2], v[3]);
+  }
+  cta_argmax(sc.s, best, best_i, 0);
+  float m;
+  {
+    double v;
+    int i;
+    cluster_argmax<kSampCluster>(sc.s, 0, &v, &i);
+    m = static_cast<float>(v);
+  }
+
+  // pass 2: this CTA's exp-sum, each thread over its elements in order, then lane 0's butterfly, then warps in order
+  float z = 0.f;
+  for (int j = threadIdx.x * 4; j < n_local; j += kSampThreads * 4) {
+    const float4 s4 = *reinterpret_cast<const float4*>(s_sh + j);
+    const float s[4] = {s4.x, s4.y, s4.z, s4.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+      if (j + e < n_local) z += expf(s[e] - m);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) z += __shfl_xor_sync(0xffffffffu, z, o);
+  const int w = threadIdx.x >> 5;
+  if ((threadIdx.x & 31) == 0) sc.warp_z[w] = z;
+
+  // top-n: each round the best value not yet taken; only the elements of the thread that held it are rescanned
+  float tv;
+  int ti;
+  if (a.n > 0) thread_best(s_sh, n_local, base, &tv, &ti);
+#pragma unroll 1
+  for (int r = 0; r < a.n; ++r) {
+    float v = tv;
+    int i = ti;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, v, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, i, o);
+      if (ov > v || (ov == v && oi < i)) v = ov, i = oi;
+    }
+    if ((threadIdx.x & 31) == 0) sc.round_v[r & 1][w] = v, sc.round_i[r & 1][w] = i;
+    __syncthreads();  // round r + 1 writes the other buffer; round r + 2 this one, after round r + 1's barrier
+    v = sc.round_v[r & 1][0];
+    i = sc.round_i[r & 1][0];
+    for (int k = 1; k < kSampWarps; ++k) {
+      const float ov = sc.round_v[r & 1][k];
+      const int oi = sc.round_i[r & 1][k];
+      if (ov > v || (ov == v && oi < i)) v = ov, i = oi;
+    }
+    if (threadIdx.x == 0) sc.cand_v[r] = v, sc.cand_i[r] = i;
+    const int owner = ((i - base) >> 2) & (kSampThreads - 1);  // the thread whose elements held the winner
+    if (i != INT_MAX && (owner >> 5) == w) {
+      // the owner's warp takes the value out and finds the owner's next best: lane l reads the owner's float4s
+      // l, l + 32, ... (a serial rescan by the owner alone took ~3 us a round on an H100)
+      if (static_cast<int>(threadIdx.x) == owner) s_sh[i - base] = __int_as_float(0x7fffffff);
+      __syncwarp();
+      float bv = -INFINITY;
+      int bi = INT_MAX;
+      for (int j = owner * 4 + (threadIdx.x & 31) * (kSampThreads * 4); j < n_local; j += 32 * kSampThreads * 4) {
+        const float4 s4 = *reinterpret_cast<const float4*>(s_sh + j);
+        const float sv[4] = {s4.x, s4.y, s4.z, s4.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          if (j + e < n_local && (sv[e] > bv || (sv[e] == bv && base + j + e < bi))) bv = sv[e], bi = base + j + e;
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (ov > bv || (ov == bv && oi < bi)) bv = ov, bi = oi;
+      }
+      if (static_cast<int>(threadIdx.x) == owner) tv = bv, ti = bi;
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float cz = 0.f;
+    for (int k = 0; k < kSampWarps; ++k) cz += sc.warp_z[k];
+    sc.cta_z = cz;
+  }
+  cluster_sync_all();  // publishes cta_z and the candidates
+
+  if (rank == 0) {
+    const int nc = kSampCluster * a.n;
+    if (static_cast<int>(threadIdx.x) < nc) {
+      const uint32_t src = threadIdx.x / a.n;
+      const int k = threadIdx.x % a.n;
+      sc.all_v[threadIdx.x] = static_cast<float>(ld_dsmem_f64(&sc.cand_v[k], src));
+      sc.all_i[threadIdx.x] = ld_dsmem_s32(&sc.cand_i[k], src);
+    }
+    if (threadIdx.x == kSampThreads - 1) {
+      float zz = 0.f;
+      for (uint32_t q = 0; q < kSampCluster; ++q) zz += static_cast<float>(ld_dsmem_f64(&sc.cta_z, q));
+      sc.log_z = logf(zz);
+    }
+    __syncthreads();
+    const float log_z = sc.log_z;
+    const int64_t col = max(int64_t(0), min(a.step[row], static_cast<int64_t>(a.cols - 1)));
+    const int64_t at = static_cast<int64_t>(row) * a.cols + col;
+    if (threadIdx.x == 0) {
+      const int64_t t = a.tokens[row];
+      a.lp_hist[at] = t >= 0 && t < a.V
+                          ? (__bfloat162float(a.logits[static_cast<int64_t>(row) * a.ld + t]) - m) - log_z
+                          : __int_as_float(0x7fffffff);  // not a token of this vocabulary
+    }
+    if (static_cast<int>(threadIdx.x) < nc) {
+      const float v = sc.all_v[threadIdx.x];
+      const int i = sc.all_i[threadIdx.x];
+      if (i != INT_MAX) {
+        int place = 0;  // candidates ahead of this one in (value descending, index ascending) order
+        for (int k = 0; k < nc; ++k) {
+          const float ov = sc.all_v[k];
+          const int oi = sc.all_i[k];
+          place += oi != INT_MAX && (ov > v || (ov == v && oi < i));
+        }
+        if (place < a.n) {
+          a.top_ids[at * a.n + place] = i;
+          a.top_lp[at * a.n + place] = (v - m) - log_z;
+        }
+      }
+    }
+  }
+  cluster_sync_all();  // no CTA leaves while rank 0 reads its shared memory
+}
+
 size_t sample_smem_bytes(int slice) {
   return ((sizeof(SampleScratch) + 15) & ~size_t(15)) + static_cast<size_t>(slice) * sizeof(float);
+}
+
+size_t logprob_smem_bytes(int slice) {
+  return ((sizeof(LogprobScratch) + 15) & ~size_t(15)) + static_cast<size_t>(slice) * sizeof(float);
 }
 
 // values per CTA when a cluster of `cluster` CTAs splits a row of V: a multiple of 4
@@ -505,6 +716,39 @@ int sample_finalize(const SampleFinalizeParams& p, cudaStream_t stream) {
                                  (int)sample_smem_bytes(slice_for(kSampCluster * kSampMaxSlice, kFinCluster))));
   VB_CUDA(launch_pdl_cluster(kern, dim3(kFinCluster), dim3(kSampThreads), sample_smem_bytes(slice), stream,
                              dim3(kFinCluster, 1, 1), a));
+  return 0;
+}
+
+int token_logprobs_check(const LogprobParams& p) {
+  VB_CHECK(p.logits && p.tokens && p.step && p.position && p.lp_hist,
+           "token_logprobs: logits, tokens, step, position and lp_hist are required");
+  VB_CHECK(p.M >= 1 && p.M <= 65535, "token_logprobs: bad row count M=%d (1..65535)", p.M);
+  VB_CHECK(p.V >= 1 && p.V <= kSampCluster * kSampMaxSlice, "token_logprobs: bad vocabulary size V=%d (1..%d)", p.V,
+           kSampCluster * kSampMaxSlice);
+  VB_CHECK(p.ld >= p.V, "token_logprobs: row stride %lld is smaller than V=%d", (long long)p.ld, p.V);
+  VB_CHECK(p.cols >= 1, "token_logprobs: cols=%d must be >= 1", p.cols);
+  VB_CHECK(p.n >= 0 && p.n <= kLpMaxTop && p.n <= p.V, "token_logprobs: n=%d must be in 0..%d and <= V=%d", p.n,
+           kLpMaxTop, p.V);
+  VB_CHECK(p.n == 0 || (p.top_ids && p.top_lp), "token_logprobs: n=%d needs top_ids and top_lp", p.n);
+  VB_CHECK((reinterpret_cast<uintptr_t>(p.logits) & 1) == 0 && (reinterpret_cast<uintptr_t>(p.tokens) & 7) == 0 &&
+               (reinterpret_cast<uintptr_t>(p.step) & 7) == 0 && (reinterpret_cast<uintptr_t>(p.position) & 3) == 0 &&
+               (reinterpret_cast<uintptr_t>(p.lp_hist) & 3) == 0 && (reinterpret_cast<uintptr_t>(p.top_ids) & 3) == 0 &&
+               (reinterpret_cast<uintptr_t>(p.top_lp) & 3) == 0,
+           "token_logprobs: misaligned pointer");
+  return 0;
+}
+
+int token_logprobs(const LogprobParams& p, cudaStream_t stream) {
+  if (int rc = token_logprobs_check(p)) return rc;
+  const int slice = slice_for(p.V, kSampCluster);
+  LogprobArgs a{p.logits, p.ld, p.tokens, p.step, p.position, p.lp_hist, p.top_ids, p.top_lp, p.V, slice, p.cols,
+                p.n};
+  static PerDeviceOnce attr_once;
+  if (attr_once.first())
+    VB_CUDA(cudaFuncSetAttribute(token_logprobs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)logprob_smem_bytes(kSampMaxSlice)));
+  VB_CUDA(launch_pdl_cluster(token_logprobs_kernel, dim3(kSampCluster, p.M), dim3(kSampThreads),
+                             logprob_smem_bytes(slice), stream, dim3(kSampCluster, 1, 1), a));
   return 0;
 }
 

@@ -12,7 +12,7 @@ import torch
 
 from . import _lib
 from ._lib import (DecodeAttnFp8Params, DecodeAttnParams, DecodeAttnSplitParams, FmhaParams, GemvBatchParams,
-                   GemvParams, SampleFinalizeParams, SampleParams, check)
+                   GemvParams, LogprobsParams, SampleFinalizeParams, SampleParams, check)
 
 ACT_NONE, ACT_GELU_TANH, ACT_GELU_ERF, ACT_SILU = 0, 1, 2, 3
 
@@ -701,6 +701,48 @@ def sample_finalize(logits: torch.Tensor, inv_temperature: torch.Tensor, top_k: 
     p.embed_table, p.x_next = _p(embed_table), _p(x_next)
     p.V, p.hidden = logits.numel(), hidden
     check(_lib.load().vila_sample_finalize(C.byref(p), _stream()), "vila_sample_finalize")
+
+
+def token_logprobs(logits: torch.Tensor, tokens: torch.Tensor, step: torch.Tensor, positions: torch.Tensor, *,
+                   lp_hist: torch.Tensor, top_ids: Optional[torch.Tensor] = None,
+                   top_lp: Optional[torch.Tensor] = None) -> None:
+    """The log-probability of each row's chosen token and its n most likely alternatives, by the rule of
+    vila_b200/logprobs.py (vila_token_logprobs, one launch).  logits [M, V] bf16 (unit column stride, any row stride);
+    per row: tokens int64 (the chosen token), step int64 (the history column, clamped to cols - 1), positions int32
+    (< 0: idle row, nothing written).  Outputs at column min(step, cols - 1) of each row: lp_hist fp32 [M, cols],
+    top_ids int32 [M, cols, n] and top_lp fp32 [M, cols, n], best first (both None: n = 0)."""
+    _need(logits.dim() == 2 and logits.stride(1) == 1 and logits.stride(0) >= logits.shape[1],
+          f"token_logprobs: logits must be [M, V] with unit column stride, got {tuple(logits.shape)} strides "
+          f"{tuple(logits.stride())}")
+    M, V = logits.shape
+    _need(1 <= M <= 65535 and 1 <= V <= SAMPLE_MAX_VOCAB,
+          f"token_logprobs: M={M} must be in 1..65535 and V={V} in 1..{SAMPLE_MAX_VOCAB}")
+    _need((top_ids is None) == (top_lp is None), "token_logprobs: top_ids and top_lp go together")
+    _need(lp_hist.dim() == 2 and lp_hist.shape[0] == M and lp_hist.shape[1] >= 1 and lp_hist.is_contiguous(),
+          f"token_logprobs: lp_hist must be a contiguous [{M}, cols] buffer, got {tuple(lp_hist.shape)}")
+    cols = lp_hist.shape[1]
+    n = 0 if top_ids is None else top_ids.shape[-1]
+    arrays = [(logits, "logits", torch.bfloat16), (tokens, "tokens", torch.int64), (step, "step", torch.int64),
+              (positions, "positions", torch.int32), (lp_hist, "lp_hist", torch.float32)]
+    if top_ids is not None:
+        for t, name in ((top_ids, "top_ids"), (top_lp, "top_lp")):
+            _need(t.dim() == 3 and t.shape == (M, cols, n) and t.is_contiguous(),
+                  f"token_logprobs: {name} must be a contiguous [{M}, {cols}, n] buffer, got {tuple(t.shape)}")
+        _need(0 <= n <= 20 and n <= V, f"token_logprobs: n={n} must be in 0..20 and <= V={V}")
+        arrays += [(top_ids, "top_ids", torch.int32), (top_lp, "top_lp", torch.float32)]
+    for t, name, dt in arrays:
+        _need(t.dtype == dt, f"token_logprobs: {name} must be {dt}, got {t.dtype}")
+        if name in ("tokens", "step", "positions"):
+            _need(t.dim() == 1 and t.numel() == M and t.is_contiguous(),
+                  f"token_logprobs: {name} must be a contiguous [{M}] vector, got {tuple(t.shape)}")
+    for t, name, _ in arrays:
+        _chk(t, name, t.dtype)
+    p = LogprobsParams()
+    p.logits, p.ld, p.tokens, p.step, p.position = _p(logits), logits.stride(0), _p(tokens), _p(step), _p(positions)
+    p.lp_hist = _p(lp_hist)
+    p.top_ids, p.top_lp = (_p(top_ids), _p(top_lp)) if n else (None, None)
+    p.M, p.V, p.cols, p.n = M, V, cols, n
+    check(_lib.load().vila_token_logprobs(C.byref(p), _stream()), "vila_token_logprobs")
 
 
 def prefix_block_hash(x: torch.Tensor, key0: int, key1: int) -> torch.Tensor:

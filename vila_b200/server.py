@@ -11,6 +11,10 @@ on the single-stream graph decoder (generate_content(stream=True) with a samplin
 every request is decoded greedily.  With --prefix-cache every non-streaming request goes to the batched engine, which
 the model keeps between batches together with the K/V pages of the prompt blocks it has seen: a request that starts
 like an earlier one (another question about the same video or image) prefills only what follows the shared blocks.
+A non-streaming request with `logprobs` (and optionally `top_logprobs`, 0..20) is always decoded by the batched engine,
+which computes each token's log-probability and its top alternatives on the device (vila_b200/logprobs.py); its
+choice carries OpenAI's `logprobs.content` list.  Streaming requests cannot have logprobs yet: the single-stream
+decoder does not compute them.
 
     python -m vila_b200.server --model-path <dir> --port 8000
 """
@@ -69,6 +73,8 @@ class ChatCompletionRequest(BaseModel):
     num_beams: Optional[int] = 1
     client: Optional[dict] = None
     seed: Optional[int] = None
+    logprobs: Optional[bool] = False
+    top_logprobs: Optional[int] = None
 
 
 def load_image(url: str):
@@ -173,33 +179,72 @@ class Engine:
                              f"but the request model is {req.model}")
         # checked before the request joins a batch: a bad value fails this request only
         params = self._sampling(req) if self.sample else None
+        top = self._top_logprobs(req)
+        if top is not None and not hasattr(self.model, "generate_batch"):
+            raise ValueError("logprobs need a model with generate_batch (the batched engine computes them)")
         loop = asyncio.get_running_loop()
         fut = loop.create_future()
-        self.pending.append((req, fut, params))
+        self.pending.append((req, fut, params, top))
         async with self.lock:
             if not fut.done():  # this task drains the queue for everyone that piled up behind the lock
                 batch, self.pending = self.pending[:self.slots], self.pending[self.slots:]
                 try:
-                    texts = await loop.run_in_executor(None, self._run_batch, [r for r, _, _ in batch],
-                                                       [p for _, _, p in batch] if self.sample else None)
+                    results = await loop.run_in_executor(None, self._run_batch, [b[0] for b in batch],
+                                                         [b[2] for b in batch] if self.sample else None,
+                                                         [b[3] for b in batch])
                 except Exception as e:  # every request of the failed batch gets the error, none is left waiting
-                    for _, f, _ in batch:
-                        if not f.done():
-                            f.set_exception(e)
+                    for b in batch:
+                        if not b[1].done():
+                            b[1].set_exception(e)
                 else:
-                    for (_, f, _), t in zip(batch, texts):
-                        if not f.done():
-                            f.set_result(t)
-        text = await fut
+                    for b, res in zip(batch, results):
+                        if not b[1].done():
+                            b[1].set_result(res)
+        text, content = await fut
+        choice = {"message": {"role": "assistant", "content": text}}
+        if content is not None:
+            choice["logprobs"] = {"content": content}
         return {"id": uuid.uuid4().hex, "object": "chat.completion", "created": int(time.time()),
-                "model": req.model, "index": 0,
-                "choices": [{"message": {"role": "assistant", "content": text}}]}
+                "model": req.model, "index": 0, "choices": [choice]}
 
-    def _run_batch(self, reqs: List[ChatCompletionRequest], sampling: Optional[list] = None) -> List[str]:
-        """sampling: one SamplingParams per request (Engine(sample=True)), or None for greedy decoding"""
+    @staticmethod
+    def _top_logprobs(req: ChatCompletionRequest) -> Optional[int]:
+        """a request's number of top alternatives per token (None: no logprobs); a bad combination raises"""
+        if req.top_logprobs is not None and not req.logprobs:
+            raise ValueError("top_logprobs needs logprobs=true")
+        if not req.logprobs:
+            return None
+        n = 0 if req.top_logprobs is None else req.top_logprobs
+        if not isinstance(n, int) or isinstance(n, bool) or not 0 <= n <= 20:
+            raise ValueError(f"top_logprobs must be an integer in 0..20, got {n!r}")
+        return n
+
+    def _logprobs_content(self, ids: List[int], entries, n: int) -> List[Dict[str, Any]]:
+        """OpenAI's logprobs.content: one entry per id the text was decoded from (the stop token excluded)"""
+        tok = self.model.tokenizer
+        stop = set(getattr(tok, "stop_token_ids", None) or ())
+        if ids and ids[-1] in stop:
+            ids = ids[:-1]
+
+        def item(i: int, lp: float) -> Dict[str, Any]:
+            text = tok.decode([i])
+            return {"token": text, "logprob": lp, "bytes": list(text.encode("utf-8"))}
+
+        return [dict(item(e.token, e.logprob), top_logprobs=[item(i, lp) for i, lp in e.top[:n]])
+                for e in entries[:len(ids)]]
+
+    def _run_batch(self, reqs: List[ChatCompletionRequest], sampling: Optional[list] = None,
+                   top: Optional[list] = None) -> List[tuple]:
+        """sampling: one SamplingParams per request (Engine(sample=True)), or None for greedy decoding; top: each
+        request's top_logprobs count, None where it did not ask for logprobs.  -> (text, logprobs content or None) per
+        request"""
         m = self.model
-        if sampling is None and not self.prefix_cache and (len(reqs) == 1 or not hasattr(m, "generate_batch")):
-            return [m.generate_content(build_prompt(r.messages), generation_config=self._gen_config(r)) for r in reqs]
+        top = top if top is not None else [None] * len(reqs)
+        want_lp = any(n is not None for n in top)
+        if (sampling is None and not self.prefix_cache and not want_lp
+                and (len(reqs) == 1 or not hasattr(m, "generate_batch"))):
+            return [(m.generate_content(build_prompt(r.messages), generation_config=self._gen_config(r)), None)
+                    for r in reqs]
         prepared = [m._prepare_content(build_prompt(r.messages)) for r in reqs]
         # the default is not passed: a model whose generate_batch predates the kv_cache argument keeps working
         kw = {} if self.kv_cache == "bf16" else {"kv_cache": self.kv_cache}
@@ -207,11 +252,16 @@ class Engine:
             kw["sampling"] = sampling
         if self.prefix_cache:
             kw.update(prefix_cache=True, max_tokens_per_slot=self.max_tokens_per_slot)
-        ids = m.generate_batch([{"input_ids": i, "media": md, "media_config": mc} for i, md, mc in prepared],
+        if want_lp:  # as kv_cache: only passed when asked for
+            kw["logprobs"] = max(n for n in top if n is not None)
+        res = m.generate_batch([{"input_ids": i, "media": md, "media_config": mc} for i, md, mc in prepared],
                                max_new_tokens=max(r.max_tokens or 512 for r in reqs), slots=self.slots, **kw)
+        ids, lps = res if want_lp else (res, None)
         outs = []
-        for r, g in zip(reqs, ids):
-            outs.append(m.tokenizer.decode(g[:r.max_tokens or 512], skip_special_tokens=True).strip())
+        for k, (r, g) in enumerate(zip(reqs, ids)):
+            g = g[:r.max_tokens or 512]
+            text = m.tokenizer.decode(g, skip_special_tokens=True).strip()
+            outs.append((text, None if top[k] is None else self._logprobs_content(g, lps[k], top[k])))
         return outs
 
     @staticmethod
@@ -225,6 +275,9 @@ class Engine:
         """a streamed request's generation config: a copy of the model's default with the request's max_tokens,
         and do_sample set explicitly: with --sample the request's temperature, top_p (top_k 0) and seed, else
         greedy whatever the checkpoint's config says.  Bad values raise."""
+        if req.logprobs or req.top_logprobs is not None:
+            raise ValueError("logprobs are not supported with stream=true: the single-stream decoder that serves "
+                             "streaming requests does not compute them yet; send the request without stream")
         gc = copy.copy(self.model.default_generation_config)
         gc.max_new_tokens = req.max_tokens
         gc.do_sample = False

@@ -34,7 +34,10 @@ tokens per byte by B.  Here:
     blocks at the same positions takes those pages into its page-table row and prefills only its suffix.  Full prompt
     pages are never written after the prefill (decode appends at positions >= S), so sharing needs no copy.  A hit
     request's ids equal those of a chunked prefill of its suffix over the donor's prefix pages; they may differ from
-    its uncached ids, since the donor's prefill may have run its GEMMs at another M.
+    its uncached ids, since the donor's prefill may have run its GEMMs at another M;
+  * with logprobs=n (vila_b200/logprobs.py) vila_token_logprobs reads each step's logits row once the token is chosen
+    and writes the token's log-probability and its n best alternatives into per-slot history buffers beside `hist`;
+    the tokens are the same as without it.
 """
 from __future__ import annotations
 
@@ -45,6 +48,7 @@ import numpy as np
 import torch
 
 from . import ops
+from .logprobs import TokenLogprob, check_top
 from .prefix_cache import PrefixPages, random_keys
 from .sampling import SamplingParams, signed64
 
@@ -172,11 +176,16 @@ class BatchedDecoder:
     admit() prefills only the part of the prompt past the cached blocks, released blocks stay findable until their
     pages are needed, `prefix_stats` counts the work saved and clear_prefix_cache() drops the unused blocks.  The
     fp8 KV cache is not supported with it (its admission prefills into a bf16 staging cache, which would need the
-    prefix in bf16)."""
+    prefix in bf16).
+
+    logprobs None (default) records no log-probabilities.  An int n in 0..20 keeps, beside `hist`, each token's
+    log-probability under the raw model distribution (`lp_hist`) and its n most likely alternatives (`top_ids`,
+    `top_lp`), written by vila_token_logprobs in every step graph and at admission; generated_logprobs(slot) reads
+    them."""
 
     def __init__(self, llm, slots: int = 8, max_tokens_per_slot: int = 2048, max_new: int = 1024,
                  total_pages: Optional[int] = None, kv_cache: str = "bf16", sampling: bool = False,
-                 prefix_cache: bool = False):
+                 prefix_cache: bool = False, logprobs: Optional[int] = None):
         if kv_cache not in KV_CACHE_FORMATS:
             raise ValueError(f"kv_cache must be one of {KV_CACHE_FORMATS}, got {kv_cache!r}")
         if prefix_cache and kv_cache == "fp8":
@@ -184,6 +193,7 @@ class BatchedDecoder:
                              "a bf16 staging cache, which would need the cached prefix in bf16")
         self.kv_cache = kv_cache
         self.prefix_cache = bool(prefix_cache)
+        self.logprobs = None if logprobs is None else check_top(logprobs)
         cfg = llm.config
         self.llm, self.slots = llm, slots
         self.decode_weights = getattr(llm, "decode_weights", "bf16")
@@ -221,8 +231,13 @@ class BatchedDecoder:
             self.top_k = torch.zeros(slots, dtype=torch.int32, device=dev)
             self.top_p = torch.ones(slots, dtype=torch.float32, device=dev)
             self.seed = torch.zeros(slots, dtype=torch.int64, device=dev)
+        if self.sampling or self.logprobs is not None:
             self._zero_pos = torch.zeros(1, dtype=torch.int32, device=dev)    # admission: row active, t = 0
             self._zero_step = torch.zeros(1, dtype=torch.int64, device=dev)
+        if self.logprobs is not None:  # vila_token_logprobs writes column step_idx of each active slot
+            self.lp_hist = torch.zeros(slots, max_new + 8, dtype=torch.float32, device=dev)
+            self.top_ids = torch.zeros(slots, max_new + 8, self.logprobs, dtype=torch.int32, device=dev)
+            self.top_lp = torch.zeros(slots, max_new + 8, self.logprobs, dtype=torch.float32, device=dev)
         # attention configurations this slot size can need (attention_config): None, then ladder entries
         self.configs: List[Optional[int]] = [None] + [
             n for i, n in enumerate(SPLIT_LADDER)
@@ -253,9 +268,10 @@ class BatchedDecoder:
     def launches_per_step(self) -> int:
         """library kernels of one step in the configuration of the last run(): 7 per layer (9 with the bf16
         split-KV kernel: RoPE/append and attention added; always 7 with the fp8 KV cache) + final RMSNorm and
-        lm_head (+ vila_sample_batch with sampling)"""
+        lm_head (+ vila_sample_batch with sampling, + vila_token_logprobs with logprobs)"""
         per_layer = 7 if self.config is None or self.kv_cache == "fp8" else 9
-        return per_layer * self.llm.config.num_hidden_layers + 2 + (1 if self.sampling else 0)
+        return (per_layer * self.llm.config.num_hidden_layers + 2 + (1 if self.sampling else 0)
+                + (0 if self.logprobs is None else 1))
 
     # ---- prefix cache ---------------------------------------------------------------------------
     def prefix_digests(self, inputs_embeds: torch.Tensor) -> np.ndarray:
@@ -363,6 +379,8 @@ class BatchedDecoder:
             self.hist[slot, 0] = tok
             self.step_idx[slot, 0] = 1
             self.x[slot] = llm.model.embed_tokens.weight[tok]
+        if self.logprobs is not None:  # entry 0 from the admission logits: M = 1, column 0
+            self._logprobs(logits[:1], slice(slot, slot + 1), self._zero_step, self._zero_pos)
         self.positions[slot] = S  # position of the token just chosen == tokens cached so far
         self._pos_host[slot] = S
 
@@ -381,6 +399,10 @@ class BatchedDecoder:
             self.slot_pages[slot].extend(new)
             self.page_tables[slot, first:first + need] = torch.tensor(new, dtype=torch.int32,
                                                                       device=self.page_tables.device)
+
+    def _logprobs(self, logits: torch.Tensor, rows: slice, step: torch.Tensor, positions: torch.Tensor) -> None:
+        top = dict(top_ids=self.top_ids[rows], top_lp=self.top_lp[rows]) if self.logprobs else {}
+        ops.token_logprobs(logits, self.tokens[rows], step, positions, lp_hist=self.lp_hist[rows], **top)
 
     def _weights(self, li: Optional[int]):
         """quantized modes: (qkv, o, gate/up, down) of layer li, or lm_head for li None, each a dict of
@@ -448,6 +470,8 @@ class BatchedDecoder:
         else:
             tok = torch.argmax(logits.float(), dim=-1)
             self.tokens.copy_(torch.where(active, tok, self.tokens))
+        if self.logprobs is not None:  # idle slots (position < 0) are not written
+            self._logprobs(logits, slice(None), self.step_idx.view(-1), self.positions)
         col = self.step_idx.clamp(max=self.hist.shape[1] - 1)
         self.hist.scatter_(1, col, self.tokens[:, None])
         self.step_idx.add_(active[:, None].to(torch.int64))
@@ -493,6 +517,15 @@ class BatchedDecoder:
         n = int(self.step_idx[slot, 0])
         return self.hist[slot, :n].tolist()
 
+    def generated_logprobs(self, slot: int) -> List[TokenLogprob]:
+        """one TokenLogprob per id of generated(slot) (decoders built with logprobs only)"""
+        if self.logprobs is None:
+            raise ValueError("generated_logprobs() needs a decoder built with logprobs=n")
+        n = int(self.step_idx[slot, 0])
+        ids, lps = self.hist[slot, :n].tolist(), self.lp_hist[slot, :n].tolist()
+        top_ids, top_lp = self.top_ids[slot, :n].tolist(), self.top_lp[slot, :n].tolist()
+        return [TokenLogprob(t, lp, list(zip(ti, tl))) for t, lp, ti, tl in zip(ids, lps, top_ids, top_lp)]
+
 
 def sampling_for_requests(sampling: Union[None, SamplingParams, Sequence[SamplingParams]],
                           n: int) -> Optional[List[SamplingParams]]:
@@ -518,7 +551,8 @@ def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eo
                    decoder: Optional[BatchedDecoder] = None, total_pages: Optional[int] = None,
                    kv_cache: str = "bf16",
                    sampling: Union[None, SamplingParams, Sequence[SamplingParams]] = None,
-                   prefix_cache: bool = False) -> List[List[int]]:
+                   prefix_cache: bool = False, logprobs: Optional[int] = None
+                   ) -> Union[List[List[int]], Tuple[List[List[int]], List[List[TokenLogprob]]]]:
     """Decode `prompts` (list of inputs_embeds [S_i, hidden]) with continuous batching: at most
     `slots` requests in flight; a finished request (EOS or max_new_tokens) frees its slot for the next
     one in the queue.  Returns the new ids per request (EOS included), in request order.
@@ -533,8 +567,16 @@ def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eo
     prefix_cache True: requests share the pages of the full prompt blocks they start with (BatchedDecoder); a request
     is admitted when the pool can hold the pages it must newly take, ceil((S + max_new_tokens + check_every) / 128)
     minus its cached blocks, out of the free and evictable pages other than its own cached blocks.  A passed-in
-    `decoder` with the other setting, or whose max_new is below max_new_tokens, is a ValueError."""
+    `decoder` with the other setting, or whose max_new is below max_new_tokens, is a ValueError.
+    logprobs None: returns the ids.  An int n in 0..20: returns (ids, logprobs), logprobs[r] holding one TokenLogprob
+    (the id, its log-probability under the raw model distribution and its n best alternatives) per id of ids[r]
+    (vila_b200/logprobs.py).  A passed-in `decoder` built without logprobs or with fewer than n is a ValueError."""
     params = sampling_for_requests(sampling, len(prompts))
+    if logprobs is not None:
+        logprobs = check_top(logprobs)
+        have = getattr(decoder, "logprobs", None) if decoder is not None else logprobs
+        if have is None or have < logprobs:
+            raise ValueError(f"logprobs={logprobs} was requested but the decoder was built with logprobs={have}")
     if decoder is not None and getattr(decoder, "prefix_cache", False) != bool(prefix_cache):
         raise ValueError(f"decoder was built with prefix_cache={getattr(decoder, 'prefix_cache', False)}, "
                          f"prefix_cache={bool(prefix_cache)} was asked for")
@@ -556,7 +598,8 @@ def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eo
                                                         check_every, slots, max_tokens_per_slot)
         decoder = BatchedDecoder(llm, slots, max_tokens_per_slot, max_new=max_new_tokens,
                                  total_pages=total_pages if total_pages is not None else pool_pages,
-                                 kv_cache=kv_cache, sampling=params is not None, prefix_cache=prefix_cache)
+                                 kv_cache=kv_cache, sampling=params is not None, prefix_cache=prefix_cache,
+                                 logprobs=logprobs)
     dec = decoder
     dec.capture()
     cap = dec.pages_per_slot * PAGE
@@ -566,6 +609,7 @@ def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eo
     queue: Deque[int] = deque(range(len(prompts)))
     owner: Dict[int, int] = {}           # slot -> request
     out: List[Optional[List[int]]] = [None] * len(prompts)
+    out_lp: List[List[TokenLogprob]] = [[] for _ in prompts]
     eos = set(int(e) for e in eos_token_ids)
 
     def harvest(slot: int, ids: List[int]) -> Optional[List[int]]:
@@ -602,7 +646,11 @@ def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eo
             for s in list(owner):
                 done = harvest(s, dec.generated(s))
                 if done is not None:
-                    out[owner.pop(s)] = done
+                    r = owner.pop(s)
+                    out[r] = done
+                    if logprobs is not None:  # truncated as the ids are; a larger decoder's top lists cut to n
+                        out_lp[r] = [TokenLogprob(e.token, e.logprob, e.top[:logprobs])
+                                     for e in dec.generated_logprobs(s)[:len(done)]]
                     dec.release(s)
     except BaseException:
         # a failed request fails the call, but a decoder that outlives it (a kept prefix-caching engine) must not keep
@@ -611,4 +659,5 @@ def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eo
             if s in owner or getattr(dec, "slot_pages", [[]] * dec.slots)[s]:
                 dec.release(s)
         raise
-    return [o or [] for o in out]
+    ids = [o or [] for o in out]
+    return ids if logprobs is None else (ids, out_lp)
