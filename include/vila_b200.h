@@ -452,6 +452,32 @@ typedef struct vila_logprobs_params {
 int vila_token_logprobs(const vila_logprobs_params* p, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * vila_apply_penalties — OpenAI's presence and frequency penalties on M rows of bf16 logits [M, V] (row stride ld),
+ * written to out [M, V] (contiguous).  The rule (vila_b200/penalties.py states it in numpy), for row x with presence
+ * p = presence[row], frequency f = frequency[row] and c_j the number of times id j occurs in history columns
+ * 0 .. min(step[row], cols) - 1 (history [M, cols] int64; ids outside [0, V) are ignored):
+ *   c_j > 0:  out_j = bf16_rn(float(x_j) - (fp32(c_j * f) + p))   (fp32, round to nearest at each operation)
+ *   c_j == 0: out_j = x_j, bit for bit
+ * A row with position < 0 is idle: its output row is not written.  The counts are integer shared-memory atomics and
+ * every output element is written once by one thread, so the output bits do not depend on thread order, M, the row
+ * index or the other rows.  1 <= V <= 327,680, 1 <= M <= 65535, cols >= 1; step int64, position int32, presence
+ * and frequency fp32 [M]; the argument errors are reported before any device call.  One CTA per (4096-entry chunk,
+ * row), PDL.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct vila_penalty_params {
+  const void* logits;
+  int64_t ld;
+  const int64_t* history;
+  const int64_t* step;
+  const int32_t* position;
+  const float* presence;
+  const float* frequency;
+  void* out;
+  int32_t M, V, cols;
+} vila_penalty_params;
+int vila_apply_penalties(const vila_penalty_params* p, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * vila_prefix_block_hash — a 128-bit digest of every full 128-row block of a bf16 matrix x [rows, cols] (row
  * stride ld elements), for prefix caching in the continuous-batching engine: out [rows / 128][2] (uint64).  The
  * reference has no counterpart: it prefills every request in full (serving/server.py:65-73, llava_arch.py:823-833).

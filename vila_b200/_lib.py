@@ -100,6 +100,14 @@ class LogprobsParams(C.Structure):
     ]
 
 
+class PenaltyParams(C.Structure):
+    _fields_ = [
+        ("logits", c_void_p), ("ld", c_i64), ("history", c_void_p), ("step", c_void_p), ("position", c_void_p),
+        ("presence", c_void_p), ("frequency", c_void_p), ("out", c_void_p), ("M", C.c_int32), ("V", C.c_int32),
+        ("cols", C.c_int32),
+    ]
+
+
 # name -> argtypes; every function returns int (0 == ok) unless listed in _RESTYPES
 SIGNATURES = {
     "vila_abi_version": [],
@@ -148,6 +156,7 @@ SIGNATURES = {
     "vila_sample_batch": [C.POINTER(SampleParams), c_void_p],
     "vila_sample_finalize": [C.POINTER(SampleFinalizeParams), c_void_p],
     "vila_token_logprobs": [C.POINTER(LogprobsParams), c_void_p],
+    "vila_apply_penalties": [C.POINTER(PenaltyParams), c_void_p],
     "vila_prefix_block_hash": [c_void_p, c_i64, c_i64, c_i64, C.c_uint64, C.c_uint64, c_void_p, c_void_p],
 }
 _RESTYPES = {"vila_last_error": C.c_char_p}

@@ -30,6 +30,7 @@ SOURCES = [
     "kv_fp8.cu",
     "sample.cu",
     "prefix_hash.cu",
+    "penalties.cu",
 ]
 HEADERS = ["common.cuh", "wgmma.cuh", "kernels.h", "../../include/vila_b200.h"]
 

@@ -465,6 +465,24 @@ int vila_token_logprobs(const vila_logprobs_params* p, void* stream) {
   return vb::token_logprobs(d, st(stream));
 }
 
+// OpenAI presence_penalty / frequency_penalty for the batched engine (the reference serves neither)
+int vila_apply_penalties(const vila_penalty_params* p, void* stream) {
+  VB_CHECK(p != nullptr, "vila_apply_penalties: params are required");
+  vb::PenaltyParams d;
+  d.logits = cb(p->logits);
+  d.ld = p->ld;
+  d.history = p->history;
+  d.step = p->step;
+  d.position = p->position;
+  d.presence = p->presence;
+  d.frequency = p->frequency;
+  d.out = mb(p->out);
+  d.M = p->M; d.V = p->V; d.cols = p->cols;
+  if (int rc = vb::apply_penalties_check(d)) return rc;
+  VB_REQUIRE_DEVICE();
+  return vb::apply_penalties(d, st(stream));
+}
+
 // the reference prefills every request in full (serving/server.py:65-73, llava_arch.py:823-833): no seam
 int vila_prefix_block_hash(const void* x, int64_t ld, int64_t rows, int64_t cols, uint64_t key0, uint64_t key1,
                            uint64_t* out, void* stream) {

@@ -284,6 +284,22 @@ struct LogprobParams {
 int token_logprobs_check(const LogprobParams& p);  // the argument errors, before any device call
 int token_logprobs(const LogprobParams& p, cudaStream_t stream);
 
+// ---- presence / frequency penalties in the batched engine (penalties.cu) --------------------------------
+// out = the rows of logits with vila_b200/penalties.py's rule applied, over history columns 0..min(step, cols) - 1
+struct PenaltyParams {
+  const __nv_bfloat16* logits;  // [M, ld]
+  int64_t ld;                   // row stride (elements), >= V
+  const int64_t* history;       // [M, cols] generated ids
+  const int64_t* step;          // [M] ids generated so far (t)
+  const int32_t* position;      // [M] < 0: idle row, its output row is not written
+  const float* presence;        // [M]
+  const float* frequency;       // [M]
+  __nv_bfloat16* out;           // [M, V]
+  int M, V, cols;
+};
+int apply_penalties_check(const PenaltyParams& p);  // the argument errors, before any device call
+int apply_penalties(const PenaltyParams& p, cudaStream_t stream);
+
 // ---- block digests for prefix caching in the batched engine (prefix_hash.cu) ----------------------------
 // out[b] = (d_0, d_1) of every full 128-row block b of x [rows, cols] bf16 (row stride ld elements); the rule is
 // vila_b200/prefix_cache.py's.  The check reports the argument errors before any device call.

@@ -587,7 +587,7 @@ class LlavaLlamaModel(nn.Module):
     def generate_batch(self, requests: List[Dict[str, Any]], max_new_tokens: int = 128, slots: int = 8,
                        max_tokens_per_slot: Optional[int] = None, eos_token_id=None,
                        kv_cache: str = "bf16", sampling=None, prefix_cache: bool = False,
-                       logprobs: Optional[int] = None):
+                       logprobs: Optional[int] = None, penalties=None):
         """Serve several independent requests with continuous batching over one shared paged KV pool
         (vila_b200/serving.py; the reference's servers run them one at a time, serving/server.py:65-73).
         requests: dicts with the `generate` arguments (`input_ids` [1, T], `media`, `media_config`).
@@ -599,10 +599,12 @@ class LlavaLlamaModel(nn.Module):
         prefix_cache: True shares the K/V pages of the full 128-token prompt blocks that requests start with (the
         same video or image, one system prompt), and needs max_tokens_per_slot.  The model keeps the engine it
         builds (max_new = max_tokens_per_slot), and with it the cached blocks, for later calls with the same slots,
-        max_tokens_per_slot, decode-weight mode, kv_cache, sampling (greedy or not) and logprobs; any other call
-        rebuilds it.
+        max_tokens_per_slot, decode-weight mode, kv_cache, sampling (greedy or not), logprobs and penalties (asked
+        for or not); any other call rebuilds it.
         logprobs: None (default) returns the new ids of every request in order; an int n in 0..20 returns (ids,
-        logprobs) with one vila_b200.logprobs.TokenLogprob per id (serving.generate_batch)."""
+        logprobs) with one vila_b200.logprobs.TokenLogprob per id (serving.generate_batch).
+        penalties: None (default) applies none; a vila_b200.penalties.PenaltyParams, or a list with one PenaltyParams or
+        None per request, applies OpenAI's presence / frequency penalties on the device (serving.generate_batch)."""
         from ..serving import BatchedDecoder, generate_batch
         if prefix_cache and max_tokens_per_slot is None:
             raise ValueError("generate_batch(prefix_cache=True) needs max_tokens_per_slot: the engine and its cached "
@@ -618,6 +620,7 @@ class LlavaLlamaModel(nn.Module):
         if prefix_cache:
             key = (slots, max_tokens_per_slot, getattr(self.llm, "decode_weights", "bf16"), kv_cache,
                    sampling is not None, logprobs)
+            key += (penalties is not None,)
             kept = getattr(self, "_prefix_engine", None)
             if kept is None or kept[0] != key:
                 if kept is not None:  # free the old pool and its graphs before the new ones are allocated
@@ -625,12 +628,12 @@ class LlavaLlamaModel(nn.Module):
                     gc.collect()
                 kept = (key, BatchedDecoder(self.llm, slots, max_tokens_per_slot, max_new=max_tokens_per_slot,
                                             kv_cache=kv_cache, sampling=sampling is not None, prefix_cache=True,
-                                            logprobs=logprobs))
+                                            logprobs=logprobs, penalties=penalties is not None))
                 self._prefix_engine = kept
             decoder = kept[1]
         return generate_batch(self.llm, prompts, max_new_tokens, eos, slots=slots,
                               max_tokens_per_slot=max_tokens_per_slot, decoder=decoder, kv_cache=kv_cache,
-                              sampling=sampling, prefix_cache=prefix_cache, logprobs=logprobs)
+                              sampling=sampling, prefix_cache=prefix_cache, logprobs=logprobs, penalties=penalties)
 
     @property
     def default_generation_config(self):

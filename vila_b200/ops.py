@@ -12,7 +12,7 @@ import torch
 
 from . import _lib
 from ._lib import (DecodeAttnFp8Params, DecodeAttnParams, DecodeAttnSplitParams, FmhaParams, GemvBatchParams,
-                   GemvParams, LogprobsParams, SampleFinalizeParams, SampleParams, check)
+                   GemvParams, LogprobsParams, PenaltyParams, SampleFinalizeParams, SampleParams, check)
 
 ACT_NONE, ACT_GELU_TANH, ACT_GELU_ERF, ACT_SILU = 0, 1, 2, 3
 
@@ -743,6 +743,40 @@ def token_logprobs(logits: torch.Tensor, tokens: torch.Tensor, step: torch.Tenso
     p.top_ids, p.top_lp = (_p(top_ids), _p(top_lp)) if n else (None, None)
     p.M, p.V, p.cols, p.n = M, V, cols, n
     check(_lib.load().vila_token_logprobs(C.byref(p), _stream()), "vila_token_logprobs")
+
+
+def apply_penalties(logits: torch.Tensor, history: torch.Tensor, step: torch.Tensor, positions: torch.Tensor,
+                    presence: torch.Tensor, frequency: torch.Tensor, *, out: torch.Tensor) -> torch.Tensor:
+    """OpenAI presence / frequency penalties by the rule of vila_b200/penalties.py (vila_apply_penalties, one launch).
+    logits [M, V] bf16 (unit column stride, any row stride); history int64 [M, cols] (contiguous) of generated ids;
+    per row: step int64 (t: history columns 0..min(t, cols) - 1 count), positions int32 (< 0: idle row, its output
+    row is not written), presence and frequency fp32.  out: a contiguous bf16 [M, V] buffer.  -> out"""
+    _need(logits.dim() == 2 and logits.stride(1) == 1 and logits.stride(0) >= logits.shape[1],
+          f"apply_penalties: logits must be [M, V] with unit column stride, got {tuple(logits.shape)} strides "
+          f"{tuple(logits.stride())}")
+    M, V = logits.shape
+    _need(1 <= M <= 65535 and 1 <= V <= SAMPLE_MAX_VOCAB,
+          f"apply_penalties: M={M} must be in 1..65535 and V={V} in 1..{SAMPLE_MAX_VOCAB}")
+    _need(history.dim() == 2 and history.shape[0] == M and history.shape[1] >= 1 and history.is_contiguous(),
+          f"apply_penalties: history must be a contiguous [{M}, cols] buffer, got {tuple(history.shape)}")
+    _need(out.shape == (M, V) and out.is_contiguous(),
+          f"apply_penalties: out must be a contiguous [{M}, {V}] buffer, got {tuple(out.shape)}")
+    arrays = [(logits, "logits", torch.bfloat16), (history, "history", torch.int64), (step, "step", torch.int64),
+              (positions, "positions", torch.int32), (presence, "presence", torch.float32),
+              (frequency, "frequency", torch.float32), (out, "out", torch.bfloat16)]
+    for t, name, dt in arrays:
+        _need(t.dtype == dt, f"apply_penalties: {name} must be {dt}, got {t.dtype}")
+        if name in ("step", "positions", "presence", "frequency"):
+            _need(t.dim() == 1 and t.numel() == M and t.is_contiguous(),
+                  f"apply_penalties: {name} must be a contiguous [{M}] vector, got {tuple(t.shape)}")
+    for t, name, _ in arrays:
+        _chk(t, name, t.dtype)
+    p = PenaltyParams()
+    p.logits, p.ld, p.history, p.step, p.position = _p(logits), logits.stride(0), _p(history), _p(step), _p(positions)
+    p.presence, p.frequency, p.out = _p(presence), _p(frequency), _p(out)
+    p.M, p.V, p.cols = M, V, history.shape[1]
+    check(_lib.load().vila_apply_penalties(C.byref(p), _stream()), "vila_apply_penalties")
+    return out
 
 
 def prefix_block_hash(x: torch.Tensor, key0: int, key1: int) -> torch.Tensor:

@@ -14,7 +14,10 @@ like an earlier one (another question about the same video or image) prefills on
 A non-streaming request with `logprobs` (and optionally `top_logprobs`, 0..20) is always decoded by the batched engine,
 which computes each token's log-probability and its top alternatives on the device (vila_b200/logprobs.py); its
 choice carries OpenAI's `logprobs.content` list.  Streaming requests cannot have logprobs yet: the single-stream
-decoder does not compute them.
+decoder does not compute them.  A non-streaming request with a non-zero `presence_penalty` or `frequency_penalty` (each
+in [-2, 2]) is likewise always decoded by the batched engine, which applies OpenAI's penalties over the request's
+generated ids on the device (vila_b200/penalties.py), greedily unless --sample is set.  Streaming requests cannot have
+penalties yet: the single-stream decoder does not apply them.
 
     python -m vila_b200.server --model-path <dir> --port 8000
 """
@@ -75,6 +78,8 @@ class ChatCompletionRequest(BaseModel):
     seed: Optional[int] = None
     logprobs: Optional[bool] = False
     top_logprobs: Optional[int] = None
+    presence_penalty: Optional[float] = 0.0
+    frequency_penalty: Optional[float] = 0.0
 
 
 def load_image(url: str):
@@ -182,16 +187,20 @@ class Engine:
         top = self._top_logprobs(req)
         if top is not None and not hasattr(self.model, "generate_batch"):
             raise ValueError("logprobs need a model with generate_batch (the batched engine computes them)")
+        pen = self._penalties(req)
+        if pen is not None and not hasattr(self.model, "generate_batch"):
+            raise ValueError("presence / frequency penalties need a model with generate_batch (the batched engine "
+                             "applies them)")
         loop = asyncio.get_running_loop()
         fut = loop.create_future()
-        self.pending.append((req, fut, params, top))
+        self.pending.append((req, fut, params, top, pen))
         async with self.lock:
             if not fut.done():  # this task drains the queue for everyone that piled up behind the lock
                 batch, self.pending = self.pending[:self.slots], self.pending[self.slots:]
                 try:
                     results = await loop.run_in_executor(None, self._run_batch, [b[0] for b in batch],
                                                          [b[2] for b in batch] if self.sample else None,
-                                                         [b[3] for b in batch])
+                                                         [b[3] for b in batch], [b[4] for b in batch])
                 except Exception as e:  # every request of the failed batch gets the error, none is left waiting
                     for b in batch:
                         if not b[1].done():
@@ -219,6 +228,14 @@ class Engine:
             raise ValueError(f"top_logprobs must be an integer in 0..20, got {n!r}")
         return n
 
+    @staticmethod
+    def _penalties(req: ChatCompletionRequest):
+        """a request's PenaltyParams, None when both penalties are 0 (None counts as 0); a bad value raises"""
+        from .penalties import PenaltyParams
+        p = PenaltyParams(presence=0.0 if req.presence_penalty is None else req.presence_penalty,
+                          frequency=0.0 if req.frequency_penalty is None else req.frequency_penalty)
+        return None if p.off else p
+
     def _logprobs_content(self, ids: List[int], entries, n: int) -> List[Dict[str, Any]]:
         """OpenAI's logprobs.content: one entry per id the text was decoded from (the stop token excluded)"""
         tok = self.model.tokenizer
@@ -234,14 +251,15 @@ class Engine:
                 for e in entries[:len(ids)]]
 
     def _run_batch(self, reqs: List[ChatCompletionRequest], sampling: Optional[list] = None,
-                   top: Optional[list] = None) -> List[tuple]:
+                   top: Optional[list] = None, penalties: Optional[list] = None) -> List[tuple]:
         """sampling: one SamplingParams per request (Engine(sample=True)), or None for greedy decoding; top: each
-        request's top_logprobs count, None where it did not ask for logprobs.  -> (text, logprobs content or None) per
-        request"""
+        request's top_logprobs count, None where it did not ask for logprobs; penalties: each request's PenaltyParams,
+        None where it asked for none.  -> (text, logprobs content or None) per request"""
         m = self.model
         top = top if top is not None else [None] * len(reqs)
         want_lp = any(n is not None for n in top)
-        if (sampling is None and not self.prefix_cache and not want_lp
+        want_pen = penalties is not None and any(p is not None for p in penalties)
+        if (sampling is None and not self.prefix_cache and not want_lp and not want_pen
                 and (len(reqs) == 1 or not hasattr(m, "generate_batch"))):
             return [(m.generate_content(build_prompt(r.messages), generation_config=self._gen_config(r)), None)
                     for r in reqs]
@@ -254,6 +272,8 @@ class Engine:
             kw.update(prefix_cache=True, max_tokens_per_slot=self.max_tokens_per_slot)
         if want_lp:  # as kv_cache: only passed when asked for
             kw["logprobs"] = max(n for n in top if n is not None)
+        if want_pen:  # likewise
+            kw["penalties"] = list(penalties)
         res = m.generate_batch([{"input_ids": i, "media": md, "media_config": mc} for i, md, mc in prepared],
                                max_new_tokens=max(r.max_tokens or 512 for r in reqs), slots=self.slots, **kw)
         ids, lps = res if want_lp else (res, None)
@@ -278,6 +298,10 @@ class Engine:
         if req.logprobs or req.top_logprobs is not None:
             raise ValueError("logprobs are not supported with stream=true: the single-stream decoder that serves "
                              "streaming requests does not compute them yet; send the request without stream")
+        if self._penalties(req) is not None:
+            raise ValueError("presence / frequency penalties are not supported with stream=true: the single-stream "
+                             "decoder that serves streaming requests does not apply them yet; send the request "
+                             "without stream")
         gc = copy.copy(self.model.default_generation_config)
         gc.max_new_tokens = req.max_tokens
         gc.do_sample = False

@@ -37,7 +37,10 @@ tokens per byte by B.  Here:
     its uncached ids, since the donor's prefill may have run its GEMMs at another M;
   * with logprobs=n (vila_b200/logprobs.py) vila_token_logprobs reads each step's logits row once the token is chosen
     and writes the token's log-probability and its n best alternatives into per-slot history buffers beside `hist`;
-    the tokens are the same as without it.
+    the tokens are the same as without it;
+  * with penalties=True (vila_b200/penalties.py) each slot has its own presence / frequency penalty in device arrays,
+    and vila_apply_penalties writes the lm_head row with OpenAI's penalties over the slot's generated ids (`hist`) into
+    a second buffer that the greedy arg-max or vila_sample_batch reads; logprobs keep reading the raw row.
 """
 from __future__ import annotations
 
@@ -49,6 +52,7 @@ import torch
 
 from . import ops
 from .logprobs import TokenLogprob, check_top
+from .penalties import PenaltyParams
 from .prefix_cache import PrefixPages, random_keys
 from .sampling import SamplingParams, signed64
 
@@ -181,11 +185,16 @@ class BatchedDecoder:
     logprobs None (default) records no log-probabilities.  An int n in 0..20 keeps, beside `hist`, each token's
     log-probability under the raw model distribution (`lp_hist`) and its n most likely alternatives (`top_ids`,
     `top_lp`), written by vila_token_logprobs in every step graph and at admission; generated_logprobs(slot) reads
-    them."""
+    them.
+
+    penalties False (default) applies none.  True keeps per-slot fp32 `presence` / `frequency` arrays (admit() writes
+    them; a slot admitted without PenaltyParams gets 0 and 0) and a bf16 [slots, V] buffer `pen_logits`: every step
+    graph runs vila_apply_penalties on the lm_head output over the slot's generated ids, and the token is chosen from
+    `pen_logits`.  The first token, chosen from the prefill logits, has no history and is never penalised."""
 
     def __init__(self, llm, slots: int = 8, max_tokens_per_slot: int = 2048, max_new: int = 1024,
                  total_pages: Optional[int] = None, kv_cache: str = "bf16", sampling: bool = False,
-                 prefix_cache: bool = False, logprobs: Optional[int] = None):
+                 prefix_cache: bool = False, logprobs: Optional[int] = None, penalties: bool = False):
         if kv_cache not in KV_CACHE_FORMATS:
             raise ValueError(f"kv_cache must be one of {KV_CACHE_FORMATS}, got {kv_cache!r}")
         if prefix_cache and kv_cache == "fp8":
@@ -238,6 +247,11 @@ class BatchedDecoder:
             self.lp_hist = torch.zeros(slots, max_new + 8, dtype=torch.float32, device=dev)
             self.top_ids = torch.zeros(slots, max_new + 8, self.logprobs, dtype=torch.int32, device=dev)
             self.top_lp = torch.zeros(slots, max_new + 8, self.logprobs, dtype=torch.float32, device=dev)
+        self.penalties = bool(penalties)
+        if self.penalties:  # per-slot parameters of vila_apply_penalties (admit() writes them) and its output rows
+            self.presence = torch.zeros(slots, dtype=torch.float32, device=dev)
+            self.frequency = torch.zeros(slots, dtype=torch.float32, device=dev)
+            self.pen_logits = torch.zeros(slots, cfg.vocab_size, dtype=dt, device=dev)
         # attention configurations this slot size can need (attention_config): None, then ladder entries
         self.configs: List[Optional[int]] = [None] + [
             n for i, n in enumerate(SPLIT_LADDER)
@@ -268,10 +282,11 @@ class BatchedDecoder:
     def launches_per_step(self) -> int:
         """library kernels of one step in the configuration of the last run(): 7 per layer (9 with the bf16
         split-KV kernel: RoPE/append and attention added; always 7 with the fp8 KV cache) + final RMSNorm and
-        lm_head (+ vila_sample_batch with sampling, + vila_token_logprobs with logprobs)"""
+        lm_head (+ vila_sample_batch with sampling, + vila_token_logprobs with logprobs, + vila_apply_penalties with
+        penalties)"""
         per_layer = 7 if self.config is None or self.kv_cache == "fp8" else 9
         return (per_layer * self.llm.config.num_hidden_layers + 2 + (1 if self.sampling else 0)
-                + (0 if self.logprobs is None else 1))
+                + (0 if self.logprobs is None else 1) + (1 if self.penalties else 0))
 
     # ---- prefix cache ---------------------------------------------------------------------------
     def prefix_digests(self, inputs_embeds: torch.Tensor) -> np.ndarray:
@@ -303,16 +318,21 @@ class BatchedDecoder:
     # ---- admission ------------------------------------------------------------------------------
     @torch.inference_mode()
     def admit(self, slot: int, inputs_embeds: torch.Tensor, params: Optional[SamplingParams] = None, *,
-              digests: Optional[np.ndarray] = None) -> None:
+              digests: Optional[np.ndarray] = None, penalties: Optional[PenaltyParams] = None) -> None:
         """Prefill `inputs_embeds` [S, hidden] into the slot's pages and seed its decode state.  params: the slot's
         SamplingParams (sampling decoders only; None is greedy); its seed must be set.  digests: prefix_digests of
-        the prompt, if the caller has them already (prefix-caching decoders).
+        the prompt, if the caller has them already (prefix-caching decoders).  penalties: the slot's PenaltyParams
+        (decoders built with penalties=True only; None is 0 and 0).
 
         A prefix-caching decoder admits into an idle slot only (released, or never used), and if the admission raises
         it releases the slot again: the hit blocks are unpinned and the pages it took are returned, so a failed request
         leaves no page half-owned and no block registered over K/V that was not written."""
         if params is not None and not self.sampling:
             raise ValueError("admit(params=...) needs a decoder built with sampling=True")
+        if penalties is not None and not self.penalties:
+            raise ValueError("admit(penalties=...) needs a decoder built with penalties=True")
+        if penalties is not None and not isinstance(penalties, PenaltyParams):
+            raise ValueError(f"admit: penalties must be a PenaltyParams or None, got {type(penalties).__name__}")
         if self.sampling:
             params = params if params is not None else SamplingParams()
             if params.seed is None and not params.greedy:
@@ -320,7 +340,7 @@ class BatchedDecoder:
         S = inputs_embeds.shape[0]
         assert S + 1 <= self.pages_per_slot * PAGE, "prompt longer than a slot"
         if not self.prefix_cache:
-            self._fill(slot, inputs_embeds, params, 0, None)
+            self._fill(slot, inputs_embeds, params, 0, None, penalties)
             return
         if self.slot_pages[slot] or self._pos_host[slot] >= 0:
             raise ValueError(f"admit: slot {slot} is still in use: release() it first")
@@ -333,14 +353,14 @@ class BatchedDecoder:
             if hits:
                 self.page_tables[slot, :len(hits)] = torch.tensor(hits, dtype=torch.int32,
                                                                   device=self.page_tables.device)
-            self._fill(slot, inputs_embeds, params, PAGE * len(hits), digests)
+            self._fill(slot, inputs_embeds, params, PAGE * len(hits), digests, penalties)
         except BaseException:
             self.release(slot)
             raise
         self.allocator.stats["prefilled_tokens"] += S - PAGE * len(hits)
 
     def _fill(self, slot: int, inputs_embeds: torch.Tensor, params: Optional[SamplingParams], p0: int,
-              digests: Optional[np.ndarray]) -> None:
+              digests: Optional[np.ndarray], penalties: Optional[PenaltyParams]) -> None:
         """admit()'s work once the slot's first p0 // 128 pages hold the cached prefix: pages for the rest, the prefill
         of inputs_embeds[p0:], registration of the new full blocks (prefix caching) and the first token"""
         llm = self.llm
@@ -362,6 +382,10 @@ class BatchedDecoder:
         else:  # the mode's lm_head, as GraphDecoder.start
             h = ops.rmsnorm(hid[-1:].contiguous(), llm.model.norm.weight, llm.config.rms_norm_eps)
             logits = ops.gemv_batch(h, **self._weights(None))
+        if self.penalties:  # read by the step graphs only: token 0 has no history and is never penalised
+            pen = penalties if penalties is not None else PenaltyParams()
+            self.presence[slot] = pen.presence
+            self.frequency[slot] = pen.frequency
         if self.sampling:  # token 0 by the same kernel: M = 1, t = 0
             self.inv_temperature[slot] = params.inv_temperature
             self.top_k[slot] = params.top_k
@@ -464,11 +488,15 @@ class BatchedDecoder:
         else:
             logits = ops.linear(h, llm.lm_head.weight, static_w=True)
         active = self.positions >= 0
+        chosen_from = logits
+        if self.penalties:  # idle rows (position < 0) are not written
+            chosen_from = ops.apply_penalties(logits, self.hist, self.step_idx.view(-1), self.positions, self.presence,
+                                              self.frequency, out=self.pen_logits)
         if self.sampling:  # idle slots (position < 0) keep their token
-            ops.sample_batch(logits, self.inv_temperature, self.top_k, self.top_p, self.seed, self.step_idx.view(-1),
+            ops.sample_batch(chosen_from, self.inv_temperature, self.top_k, self.top_p, self.seed, self.step_idx.view(-1),
                              self.positions, out=self.tokens)
         else:
-            tok = torch.argmax(logits.float(), dim=-1)
+            tok = torch.argmax(chosen_from.float(), dim=-1)
             self.tokens.copy_(torch.where(active, tok, self.tokens))
         if self.logprobs is not None:  # idle slots (position < 0) are not written
             self._logprobs(logits, slice(None), self.step_idx.view(-1), self.positions)
@@ -545,13 +573,26 @@ def sampling_for_requests(sampling: Union[None, SamplingParams, Sequence[Samplin
     return out
 
 
+def penalties_for_requests(penalties: Union[None, PenaltyParams, Sequence[Optional[PenaltyParams]]],
+                           n: int) -> Optional[List[Optional[PenaltyParams]]]:
+    """generate_batch's `penalties` -> one PenaltyParams or None per request (None stays None)"""
+    if penalties is None:
+        return None
+    per = [penalties] * n if isinstance(penalties, PenaltyParams) else penalties
+    if (not isinstance(per, (list, tuple)) or len(per) != n
+            or not all(p is None or isinstance(p, PenaltyParams) for p in per)):
+        raise ValueError(f"penalties must be a PenaltyParams or a list of {n} PenaltyParams or None (one per request)")
+    return list(per)
+
+
 @torch.inference_mode()
 def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eos_token_ids: Sequence[int] = (),
                    slots: int = 8, max_tokens_per_slot: Optional[int] = None, check_every: int = 8,
                    decoder: Optional[BatchedDecoder] = None, total_pages: Optional[int] = None,
                    kv_cache: str = "bf16",
                    sampling: Union[None, SamplingParams, Sequence[SamplingParams]] = None,
-                   prefix_cache: bool = False, logprobs: Optional[int] = None
+                   prefix_cache: bool = False, logprobs: Optional[int] = None,
+                   penalties: Union[None, PenaltyParams, Sequence[Optional[PenaltyParams]]] = None
                    ) -> Union[List[List[int]], Tuple[List[List[int]], List[List[TokenLogprob]]]]:
     """Decode `prompts` (list of inputs_embeds [S_i, hidden]) with continuous batching: at most
     `slots` requests in flight; a finished request (EOS or max_new_tokens) frees its slot for the next
@@ -570,8 +611,15 @@ def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eo
     `decoder` with the other setting, or whose max_new is below max_new_tokens, is a ValueError.
     logprobs None: returns the ids.  An int n in 0..20: returns (ids, logprobs), logprobs[r] holding one TokenLogprob
     (the id, its log-probability under the raw model distribution and its n best alternatives) per id of ids[r]
-    (vila_b200/logprobs.py).  A passed-in `decoder` built without logprobs or with fewer than n is a ValueError."""
+    (vila_b200/logprobs.py).  A passed-in `decoder` built without logprobs or with fewer than n is a ValueError.
+    penalties None: no repetition penalties.  Otherwise one PenaltyParams for every request or a list with one
+    PenaltyParams or None (0 and 0) per request, applied on the device to every token after the first
+    (BatchedDecoder(penalties=True), vila_b200/penalties.py); logprobs stay those of the raw model distribution.  A
+    passed-in decoder built without penalties is a ValueError."""
     params = sampling_for_requests(sampling, len(prompts))
+    pens = penalties_for_requests(penalties, len(prompts))
+    if pens is not None and decoder is not None and not getattr(decoder, "penalties", False):
+        raise ValueError("penalties were requested but the decoder was built with penalties=False")
     if logprobs is not None:
         logprobs = check_top(logprobs)
         have = getattr(decoder, "logprobs", None) if decoder is not None else logprobs
@@ -599,7 +647,7 @@ def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eo
         decoder = BatchedDecoder(llm, slots, max_tokens_per_slot, max_new=max_new_tokens,
                                  total_pages=total_pages if total_pages is not None else pool_pages,
                                  kv_cache=kv_cache, sampling=params is not None, prefix_cache=prefix_cache,
-                                 logprobs=logprobs)
+                                 logprobs=logprobs, penalties=pens is not None)
     dec = decoder
     dec.capture()
     cap = dec.pages_per_slot * PAGE
@@ -637,6 +685,8 @@ def generate_batch(llm, prompts: Sequence[torch.Tensor], max_new_tokens: int, eo
                         break  # wait for a running request to finish and return its pages
                     r = queue.popleft()
                     kw = {"digests": digests.pop(r)} if prefix_cache else {}
+                    if pens is not None:
+                        kw["penalties"] = pens[r]
                     if params is None:
                         dec.admit(s, prompts[r], **kw)
                     else:
