@@ -452,6 +452,35 @@ typedef struct vila_logprobs_params {
 int vila_token_logprobs(const vila_logprobs_params* p, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * vila_token_logprobs_row — vila_token_logprobs' rule on the single-stream graph decoder's one row of bf16 logits
+ * [V], spread over the whole GPU: one CTA per 1152-entry chunk computes the chunk's max, its fp32 exp-sum and its top
+ * n into `workspace`; the last CTA to arrive (arrival `counter`, reset to 0 by that CTA, so replays of a captured
+ * graph need no memset) combines the chunks in chunk order.  The chosen token is *token and the history column is
+ * col = min(*step - 1, cols - 1): *step is the decoder's token counter, already advanced past the token (both int32
+ * [1]).  Writes lp_hist[col] (fp32), top_ids / top_lp [col * n + j] (int32 / fp32, j = 0 best) for j < k: k is
+ * min(*n_used, n) when n_used (a device int32 [1]) is given, else n, so n is the row stride and a captured graph
+ * serves every k up to n; entries j >= k are not written.  Top ids are exact,
+ * values within 1e-5 + 1e-6 |lp| of the rule in fp64, and the token's value equals its entry in top bit for bit;
+ * the bits do not depend on scheduling or on the device.  workspace: workspace_bytes >= ceil(V / 1152) * 168 bytes,
+ * 16-byte aligned; counter zero before the first launch.  1 <= V <= 327,680, 0 <= n <= 20 and n <= V (top_ids /
+ * top_lp may be NULL when n == 0), cols >= 1; the argument errors are reported before any device call.  PDL.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct vila_logprobs_row_params {
+  const void* logits;
+  const int32_t* token;
+  const int32_t* step;
+  float* lp_hist;
+  int32_t* top_ids;
+  float* top_lp;
+  const int32_t* n_used;
+  void* workspace;
+  int64_t workspace_bytes;
+  uint32_t* counter;
+  int32_t V, cols, n;
+} vila_logprobs_row_params;
+int vila_token_logprobs_row(const vila_logprobs_row_params* p, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * vila_apply_penalties — OpenAI's presence and frequency penalties on M rows of bf16 logits [M, V] (row stride ld),
  * written to out [M, V] (contiguous).  The rule (vila_b200/penalties.py states it in numpy), for row x with presence
  * p = presence[row], frequency f = frequency[row] and c_j the number of times id j occurs in history columns
@@ -476,6 +505,22 @@ typedef struct vila_penalty_params {
   int32_t M, V, cols;
 } vila_penalty_params;
 int vila_apply_penalties(const vila_penalty_params* p, void* stream);
+
+/* vila_apply_penalties_row — vila_apply_penalties' rule, bit for bit, on the single-stream graph decoder's one row of
+ * bf16 logits [V], written to out [V]: c_j counts id j in history[0 .. min(*step, cols) - 1] (int32 ids, int32 step
+ * counter = ids generated before this token; ids outside [0, V) are ignored), presence and frequency are fp32 device
+ * scalars.  Same kernel as vila_apply_penalties; 1 <= V <= 327,680, cols >= 1; the argument errors are reported
+ * before any device call.  PDL. */
+typedef struct vila_penalty_row_params {
+  const void* logits;
+  const int32_t* history;
+  const int32_t* step;
+  const float* presence;
+  const float* frequency;
+  void* out;
+  int32_t V, cols;
+} vila_penalty_row_params;
+int vila_apply_penalties_row(const vila_penalty_row_params* p, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * vila_prefix_block_hash — a 128-bit digest of every full 128-row block of a bf16 matrix x [rows, cols] (row

@@ -108,6 +108,22 @@ class PenaltyParams(C.Structure):
     ]
 
 
+class LogprobsRowParams(C.Structure):
+    _fields_ = [
+        ("logits", c_void_p), ("token", c_void_p), ("step", c_void_p), ("lp_hist", c_void_p), ("top_ids", c_void_p),
+        ("top_lp", c_void_p), ("n_used", c_void_p), ("workspace", c_void_p), ("workspace_bytes", c_i64),
+        ("counter", c_void_p),
+        ("V", C.c_int32), ("cols", C.c_int32), ("n", C.c_int32),
+    ]
+
+
+class PenaltyRowParams(C.Structure):
+    _fields_ = [
+        ("logits", c_void_p), ("history", c_void_p), ("step", c_void_p), ("presence", c_void_p),
+        ("frequency", c_void_p), ("out", c_void_p), ("V", C.c_int32), ("cols", C.c_int32),
+    ]
+
+
 # name -> argtypes; every function returns int (0 == ok) unless listed in _RESTYPES
 SIGNATURES = {
     "vila_abi_version": [],
@@ -157,6 +173,8 @@ SIGNATURES = {
     "vila_sample_finalize": [C.POINTER(SampleFinalizeParams), c_void_p],
     "vila_token_logprobs": [C.POINTER(LogprobsParams), c_void_p],
     "vila_apply_penalties": [C.POINTER(PenaltyParams), c_void_p],
+    "vila_token_logprobs_row": [C.POINTER(LogprobsRowParams), c_void_p],
+    "vila_apply_penalties_row": [C.POINTER(PenaltyRowParams), c_void_p],
     "vila_prefix_block_hash": [c_void_p, c_i64, c_i64, c_i64, C.c_uint64, C.c_uint64, c_void_p, c_void_p],
 }
 _RESTYPES = {"vila_last_error": C.c_char_p}

@@ -31,6 +31,7 @@ SOURCES = [
     "sample.cu",
     "prefix_hash.cu",
     "penalties.cu",
+    "logprobs_row.cu",
 ]
 HEADERS = ["common.cuh", "wgmma.cuh", "kernels.h", "../../include/vila_b200.h"]
 

@@ -465,6 +465,26 @@ int vila_token_logprobs(const vila_logprobs_params* p, void* stream) {
   return vb::token_logprobs(d, st(stream));
 }
 
+// the same for the single-stream graph decoder's one row
+int vila_token_logprobs_row(const vila_logprobs_row_params* p, void* stream) {
+  VB_CHECK(p != nullptr, "vila_token_logprobs_row: params are required");
+  vb::LogprobRowParams d;
+  d.logits = cb(p->logits);
+  d.token = p->token;
+  d.step = p->step;
+  d.lp_hist = p->lp_hist;
+  d.top_ids = p->top_ids;
+  d.top_lp = p->top_lp;
+  d.n_used = p->n_used;
+  d.workspace = p->workspace;
+  d.workspace_bytes = p->workspace_bytes;
+  d.counter = p->counter;
+  d.V = p->V; d.cols = p->cols; d.n = p->n;
+  if (int rc = vb::token_logprobs_row_check(d)) return rc;
+  VB_REQUIRE_DEVICE();
+  return vb::token_logprobs_row(d, st(stream));
+}
+
 // OpenAI presence_penalty / frequency_penalty for the batched engine (the reference serves neither)
 int vila_apply_penalties(const vila_penalty_params* p, void* stream) {
   VB_CHECK(p != nullptr, "vila_apply_penalties: params are required");
@@ -481,6 +501,22 @@ int vila_apply_penalties(const vila_penalty_params* p, void* stream) {
   if (int rc = vb::apply_penalties_check(d)) return rc;
   VB_REQUIRE_DEVICE();
   return vb::apply_penalties(d, st(stream));
+}
+
+// the same for the single-stream graph decoder's one row
+int vila_apply_penalties_row(const vila_penalty_row_params* p, void* stream) {
+  VB_CHECK(p != nullptr, "vila_apply_penalties_row: params are required");
+  vb::PenaltyRowParams d;
+  d.logits = cb(p->logits);
+  d.history = p->history;
+  d.step = p->step;
+  d.presence = p->presence;
+  d.frequency = p->frequency;
+  d.out = mb(p->out);
+  d.V = p->V; d.cols = p->cols;
+  if (int rc = vb::apply_penalties_row_check(d)) return rc;
+  VB_REQUIRE_DEVICE();
+  return vb::apply_penalties_row(d, st(stream));
 }
 
 // the reference prefills every request in full (serving/server.py:65-73, llava_arch.py:823-833): no seam

@@ -283,6 +283,24 @@ struct LogprobParams {
 };
 int token_logprobs_check(const LogprobParams& p);  // the argument errors, before any device call
 int token_logprobs(const LogprobParams& p, cudaStream_t stream);
+// the same rule on the single-stream decoder's one row, spread over one CTA per 1152-entry chunk
+// (logprobs_row.cu): written at column min(*step - 1, cols - 1), *step being the decoder's advanced counter
+struct LogprobRowParams {
+  const __nv_bfloat16* logits;  // [V]
+  const int32_t* token;         // [1] the chosen token
+  const int32_t* step;          // [1] tokens produced so far, this one included
+  float* lp_hist;               // [cols]
+  int32_t* top_ids;             // [cols, n] (null when n == 0)
+  float* top_lp;                // [cols, n] (null when n == 0)
+  const int32_t* n_used;        // [1] alternatives to compute, clamped to 0..n; null: n
+  void* workspace;              // token_logprobs_row_workspace_bytes(V) bytes, 16-byte aligned
+  int64_t workspace_bytes;
+  unsigned int* counter;        // zero before the first launch; each launch leaves it zero
+  int V, cols, n;
+};
+int64_t token_logprobs_row_workspace_bytes(int V);
+int token_logprobs_row_check(const LogprobRowParams& p);  // the argument errors, before any device call
+int token_logprobs_row(const LogprobRowParams& p, cudaStream_t stream);
 
 // ---- presence / frequency penalties in the batched engine (penalties.cu) --------------------------------
 // out = the rows of logits with vila_b200/penalties.py's rule applied, over history columns 0..min(step, cols) - 1
@@ -299,6 +317,19 @@ struct PenaltyParams {
 };
 int apply_penalties_check(const PenaltyParams& p);  // the argument errors, before any device call
 int apply_penalties(const PenaltyParams& p, cudaStream_t stream);
+// the same rule on the single-stream decoder's one row: its int32 history and int32 step counter, device-scalar
+// presence and frequency
+struct PenaltyRowParams {
+  const __nv_bfloat16* logits;  // [V]
+  const int32_t* history;       // [cols] generated ids
+  const int32_t* step;          // [1] ids generated before this token (t)
+  const float* presence;        // [1]
+  const float* frequency;       // [1]
+  __nv_bfloat16* out;           // [V]
+  int V, cols;
+};
+int apply_penalties_row_check(const PenaltyRowParams& p);  // the argument errors, before any device call
+int apply_penalties_row(const PenaltyRowParams& p, cudaStream_t stream);
 
 // ---- block digests for prefix caching in the batched engine (prefix_hash.cu) ----------------------------
 // out[b] = (d_0, d_1) of every full 128-row block b of x [rows, cols] bf16 (row stride ld elements); the rule is

@@ -1,5 +1,7 @@
-// OpenAI presence and frequency penalties on the device, for the continuous-batching engine (vila_b200/serving.py,
-// penalties=True): vila_apply_penalties.
+// OpenAI presence and frequency penalties on the device: vila_apply_penalties for the continuous-batching engine
+// (vila_b200/serving.py, penalties=True) and vila_apply_penalties_row for the single-stream graph decoder (GraphDecoder
+// with penalties, vila_b200/model/qwen2.py).  Both run the same kernel, templated on the type of the history and of
+// the step counter (int64 per row in the batched engine, int32 in the graph decoder).
 //
 // The rule (stated in numpy by vila_b200/penalties.py, which the tests use), for a row x of bf16 logits with presence
 // p, frequency f and c_j the number of times id j occurs among the ids the request generated before this token:
@@ -22,12 +24,13 @@ constexpr int kPenVec = 2;                              // 16-byte groups of 8 e
 constexpr int kPenChunk = kPenThreads * kPenVec * 8;    // 4096 entries per CTA: 38 CTAs per row at V = 152,064
 constexpr int kPenMaxVocab = 8 * 40960;                 // the samplers' limit: the penalised row goes to them
 
+template <typename Idx>
 struct PenaltyArgs {
   const __nv_bfloat16* logits;
   int64_t ld;
-  const int64_t* history;
-  const int64_t* step;
-  const int32_t* position;
+  const Idx* history;
+  const Idx* step;
+  const int32_t* position;  // null: every row is active
   const float* presence;
   const float* frequency;
   __nv_bfloat16* out;
@@ -38,12 +41,13 @@ __device__ __forceinline__ uint32_t bf_bits(const __nv_bfloat16* p) {
   return *reinterpret_cast<const unsigned short*>(p);
 }
 
-__global__ void __launch_bounds__(kPenThreads) apply_penalties_kernel(PenaltyArgs a) {
+template <typename Idx>
+__global__ void __launch_bounds__(kPenThreads) apply_penalties_kernel(PenaltyArgs<Idx> a) {
   __shared__ __align__(16) int count[kPenChunk];
   griddep_wait();
   griddep_launch_dependents();
   const int row = blockIdx.y;
-  if (a.position[row] < 0) return;  // idle row: its output row is left as it is
+  if (a.position && a.position[row] < 0) return;  // idle row: its output row is left as it is
   const int base = blockIdx.x * kPenChunk;
   const int n_local = min(kPenChunk, a.V - base);
   const __nv_bfloat16* x = a.logits + static_cast<int64_t>(row) * a.ld + base;
@@ -70,10 +74,10 @@ __global__ void __launch_bounds__(kPenThreads) apply_penalties_kernel(PenaltyArg
 
   for (int i = threadIdx.x; i < kPenChunk; i += kPenThreads) count[i] = 0;
   __syncthreads();
-  const int64_t n_hist = max(int64_t(0), min(a.step[row], static_cast<int64_t>(a.cols)));
-  const int64_t* h = a.history + static_cast<int64_t>(row) * a.cols;
+  const int64_t n_hist = max(int64_t(0), min(static_cast<int64_t>(a.step[row]), static_cast<int64_t>(a.cols)));
+  const Idx* h = a.history + static_cast<int64_t>(row) * a.cols;
   for (int64_t i = threadIdx.x; i < n_hist; i += kPenThreads) {
-    const int64_t id = h[i] - base;
+    const int64_t id = static_cast<int64_t>(h[i]) - base;
     if (id >= 0 && id < n_local) atomicAdd(&count[id], 1);  // ids outside [0, V) fall outside every chunk
   }
   __syncthreads();
@@ -127,8 +131,30 @@ int apply_penalties_check(const PenaltyParams& p) {
 
 int apply_penalties(const PenaltyParams& p, cudaStream_t stream) {
   if (int rc = apply_penalties_check(p)) return rc;
-  PenaltyArgs a{p.logits, p.ld, p.history, p.step, p.position, p.presence, p.frequency, p.out, p.V, p.cols};
-  VB_CUDA(launch_pdl(apply_penalties_kernel, dim3((p.V + kPenChunk - 1) / kPenChunk, p.M), dim3(kPenThreads), 0,
+  PenaltyArgs<int64_t> a{p.logits, p.ld, p.history, p.step, p.position, p.presence, p.frequency, p.out, p.V, p.cols};
+  VB_CUDA(launch_pdl(apply_penalties_kernel<int64_t>, dim3((p.V + kPenChunk - 1) / kPenChunk, p.M), dim3(kPenThreads),
+                     0, stream, a));
+  return 0;
+}
+
+int apply_penalties_row_check(const PenaltyRowParams& p) {
+  VB_CHECK(p.logits && p.history && p.step && p.presence && p.frequency && p.out,
+           "apply_penalties_row: logits, history, step, presence, frequency and out are required");
+  VB_CHECK(p.V >= 1 && p.V <= kPenMaxVocab, "apply_penalties_row: bad vocabulary size V=%d (1..%d)", p.V,
+           kPenMaxVocab);
+  VB_CHECK(p.cols >= 1, "apply_penalties_row: cols=%d must be >= 1", p.cols);
+  VB_CHECK((reinterpret_cast<uintptr_t>(p.logits) & 1) == 0 && (reinterpret_cast<uintptr_t>(p.out) & 1) == 0 &&
+               (reinterpret_cast<uintptr_t>(p.history) & 3) == 0 && (reinterpret_cast<uintptr_t>(p.step) & 3) == 0 &&
+               (reinterpret_cast<uintptr_t>(p.presence) & 3) == 0 &&
+               (reinterpret_cast<uintptr_t>(p.frequency) & 3) == 0,
+           "apply_penalties_row: misaligned pointer");
+  return 0;
+}
+
+int apply_penalties_row(const PenaltyRowParams& p, cudaStream_t stream) {
+  if (int rc = apply_penalties_row_check(p)) return rc;
+  PenaltyArgs<int32_t> a{p.logits, p.V, p.history, p.step, nullptr, p.presence, p.frequency, p.out, p.V, p.cols};
+  VB_CUDA(launch_pdl(apply_penalties_kernel<int32_t>, dim3((p.V + kPenChunk - 1) / kPenChunk, 1), dim3(kPenThreads), 0,
                      stream, a));
   return 0;
 }

@@ -729,3 +729,27 @@ class LlavaLlamaModel(nn.Module):
             text = self.tokenizer.decode(ids, skip_special_tokens=True)
             if text:
                 yield text
+
+    def stream_content(self, prompt: Union[str, List], generation_config=None, *, logprobs: Optional[int] = None,
+                       penalties=None, chunk_tokens: int = 8):
+        """generate_content(stream=True) with per-token logprobs and OpenAI presence / frequency penalties, as a
+        generator of (ids, entries) per chunk of up to chunk_tokens new ids (sampled on the device when the generation
+        config sets do_sample, as generate_content).  entries: one vila_b200.logprobs.TokenLogprob per id with
+        `logprobs` = n in 0..20 alternatives, else None.  penalties: a vila_b200.penalties.PenaltyParams, or None.  The
+        last chunk ends with the EOS id when one was generated; its entry is there too.  Both options run on the
+        device in the single-stream graph decoder (Qwen2ForCausalLM.stream_tokens).  Not with sequence-parallel
+        decoding (NotImplementedError)."""
+        from ..logprobs import check_top
+        if logprobs is not None:
+            check_top(logprobs)
+        if (logprobs is not None or (penalties is not None and not penalties.off)) and self._sp_runner() is not None:
+            raise NotImplementedError("stream_content: logprobs and penalties are not implemented with "
+                                      "sequence-parallel decoding")
+        with torch.inference_mode():
+            input_ids, media, media_config = self._prepare_content(prompt)
+            gc = generation_config or self.default_generation_config
+            inputs_embeds, _, _ = self._embed(input_ids, media, media_config, None, None)
+        sampling = sampling_for_generate(gc, 1)[0] if getattr(gc, "do_sample", False) else None
+        for out in self.llm.stream_tokens(inputs_embeds[0], gc, chunk_tokens=chunk_tokens, sampling=sampling,
+                                          logprobs=logprobs, penalties=penalties):
+            yield out if logprobs is not None else (out, None)

@@ -22,6 +22,8 @@ import torch
 from torch import nn
 
 from .. import ops
+from ..logprobs import MAX_TOP_LOGPROBS, TokenLogprob, check_top
+from ..penalties import PenaltyParams
 from ..sampling import SamplingParams, signed64
 from .configuration import Qwen2Config
 
@@ -253,6 +255,31 @@ def dequantize_w4_groups(packed: torch.Tensor, s: torch.Tensor, z: torch.Tensor)
     K = G * W4_GROUP
     q = _w4_unpack(packed, K)[:N].float().view(N, G, W4_GROUP)
     return ((q - z.float()[..., None]) * s.float()[..., None]).view(N, K)
+
+
+def _stream_logprobs(dec, max_new: int, chunk_tokens: int, eos_ids):
+    """stream_tokens' loop with logprobs, one chunk ahead: chunk k + 1 is enqueued before the host waits for chunk
+    k's rows (only those, in one copy) and builds its entries, so the device does not idle while the host works.
+    A chunk decoded past EOS is dropped."""
+    done, n = 0, min(chunk_tokens, max_new)
+    dec.run(n)
+    pending = dec.read_logprobs(n, start=0)
+    while True:
+        nxt = min(chunk_tokens, max_new - done - n)
+        if nxt > 0:
+            dec.run(nxt)
+        entries = pending()
+        if nxt > 0:
+            pending = dec.read_logprobs(done + n + nxt, start=done + n)
+        ids = [e.token for e in entries]
+        hit = [i for i, t in enumerate(ids) if t in eos_ids]
+        if hit:
+            yield ids[:hit[0] + 1], entries[:hit[0] + 1]
+            return
+        yield ids, entries
+        if nxt <= 0:
+            return
+        done, n = done + n, nxt
 
 
 class Qwen2ForCausalLM(nn.Module):
@@ -632,11 +659,19 @@ class Qwen2ForCausalLM(nn.Module):
         return self.stream_tokens(emb, generation_config, chunk_tokens, max_new_tokens)
 
     def stream_tokens(self, emb: torch.Tensor, generation_config=None, chunk_tokens: int = 8,
-                      max_new_tokens: Optional[int] = None, sampling: Optional[SamplingParams] = None):
+                      max_new_tokens: Optional[int] = None, sampling: Optional[SamplingParams] = None,
+                      logprobs: Optional[int] = None, penalties: Optional[PenaltyParams] = None):
         """stream_greedy, or with `sampling` (a SamplingParams with its seed set) the same loop sampled on the
-        device: the ids are those of generate(do_sample=True) with the same parameters and seed."""
+        device: the ids are those of generate(do_sample=True) with the same parameters and seed.
+        logprobs: None yields id lists; n in 0..20 yields (ids, [TokenLogprob ...]) per chunk, one entry per id (the
+        token's log-probability under the raw row and its n most likely alternatives, vila_b200/logprobs.py),
+        truncated at EOS as the ids are.  penalties: a PenaltyParams applies OpenAI's presence / frequency penalties
+        over the ids generated so far before each choice (vila_b200/penalties.py).  Both run on the device in the
+        graph decoder (GraphDecoder.start)."""
         if sampling is not None and not sampling.greedy and sampling.seed is None:
             raise ValueError("stream_tokens: sampling needs a seed")
+        if logprobs is not None:
+            check_top(logprobs)
         gc = generation_config or self.generation_config
         max_new = max_new_tokens or getattr(gc, "max_new_tokens", None)
         if max_new is None:
@@ -648,7 +683,13 @@ class Qwen2ForCausalLM(nn.Module):
             dec = self.decoder(max_new)
             cache = dec.cache_for(S + max_new)
             hid = self.prefill_hidden_graphed(emb, cache)
-            dec.start(hid[-1], cache, sampling)
+            if logprobs is None and penalties is None:
+                dec.start(hid[-1], cache, sampling)
+            else:
+                dec.start(hid[-1], cache, sampling, logprobs=logprobs, penalties=penalties)
+            if logprobs is not None:
+                yield from _stream_logprobs(dec, max_new, chunk_tokens, eos_ids)
+                return
             done = 0
             while done < max_new:
                 n = min(chunk_tokens, max_new - done)
@@ -660,6 +701,7 @@ class Qwen2ForCausalLM(nn.Module):
                     yield ids[:hit[0] + 1]
                     return
                 yield ids
+
 
     def _generate_eager(self, emb, max_new, eos_ids, sample, processors, temperature, top_p, top_k):
         """Non-graph path: logits come from the same kernels; the token choice (sampling /
@@ -711,6 +753,19 @@ class GraphDecoder:
     place of argmax_finalize.  Temperature, top-k, top-p and seed are device scalars that start() writes, so a
     new request's parameters replay the same graph.
 
+    Logprobs and presence / frequency penalties (start(..., logprobs=n, penalties=PenaltyParams)) run further step
+    graphs, captured on first use and keyed by (sampled, penalised, logprobs on) as well as the attention plan.  The
+    number of alternatives n is a device scalar that start() writes (the history rows hold 20), so one graph serves
+    every n:
+      greedy + logprobs   lm_head writes the bf16 row and keeps its fused argmax key; argmax_finalize; then
+                          vila_token_logprobs_row on the row (the ids are the greedy graph's)
+      sampled + logprobs  the sampled step, then vila_token_logprobs_row on the row
+      penalties           lm_head writes the row, vila_apply_penalties_row writes pen_logits over the decoder's own
+                          int32 history, vila_sample_finalize chooses from pen_logits (at inv_T = 0 the first index of
+                          the max: the greedy rule), then vila_token_logprobs_row on the raw row when logprobs are on
+    The rules are those of vila_b200/logprobs.py and vila_b200/penalties.py; token_logprobs() reads the entries back.
+    Their buffers are allocated on first use; a request with neither option runs exactly the graphs above.
+
     The decoder streams the weights of the LLM's decode-weight mode at construction
     (Qwen2ForCausalLM.set_decode_weights): in "fp8" mode every GEMV of start() and of each step, lm_head
     included, runs vila_gemv_fp8 on the e4m3 copies, so the first token is an fp8 lm_head result too.  In
@@ -745,6 +800,8 @@ class GraphDecoder:
         self.top_p = torch.ones(1, device=dev, dtype=torch.float32)
         self.seed = torch.zeros(1, device=dev, dtype=torch.int64)
         self.sampled = False  # mode of the current request (start())
+        self.penalised = False
+        self.top_n: Optional[int] = None  # logprobs: alternatives per token, None = off
         self.ws = torch.zeros(Hkv * self.MAX_SPLITS * (Hq // Hkv) * (D + 2), device=dev,
                               dtype=torch.float32)
         self.counters = torch.zeros(Hkv, device=dev, dtype=torch.int32)
@@ -755,16 +812,50 @@ class GraphDecoder:
         self.cache: Optional[PagedKVCache] = None
         self.graphs = {}  # (num_splits, split_tokens) -> captured CUDA graph of one decode step (for self.cache)
         self.sampled_graphs = {}  # the same for sampled steps
+        # (sampled, penalised, logprobs on, num_splits, split_tokens) -> step graph with logprobs or penalties
+        self.option_graphs = {}
+        # logprobs / penalties buffers, allocated on first use (_ensure_logprobs / _ensure_penalties)
+        self.lp_hist = self.top_ids = self.top_lp = self.lp_n = self.lp_ws = self.lp_counter = None
+        self.pen_logits = self.presence = self.frequency = None
+
+    @property
+    def _options(self) -> bool:
+        return self.penalised or self.top_n is not None
+
+    def _graph_dict_key(self):
+        plan = (self.num_splits, self.split_tokens)
+        if self._options:
+            return self.option_graphs, (self.sampled, self.penalised, self.top_n is not None) + plan
+        return (self.sampled_graphs if self.sampled else self.graphs), plan
 
     @property
     def graph(self):
-        return (self.sampled_graphs if self.sampled else self.graphs).get((self.num_splits, self.split_tokens))
+        graphs, key = self._graph_dict_key()
+        return graphs.get(key)
 
     @property
     def launches_per_step(self) -> int:
         """kernels of one decode step: 5 per layer (7 on the long-context path: RoPE/append, split-KV
-        attention, combine) + lm_head GEMV + finalize (argmax or sample), in either mode"""
-        return (7 if self.split_tokens else 5) * self.llm.config.num_hidden_layers + 2
+        attention, combine) + lm_head GEMV + finalize (argmax or sample), in either mode; + 1 with penalties
+        (vila_apply_penalties_row) and + 1 with logprobs (vila_token_logprobs_row)"""
+        return ((7 if self.split_tokens else 5) * self.llm.config.num_hidden_layers + 2 + int(self.penalised)
+                + int(self.top_n is not None))
+
+    def _ensure_logprobs(self) -> None:
+        if self.lp_hist is None:
+            dev, cols = self.llm.device, self.max_new + 8
+            self.lp_hist = torch.zeros(cols, device=dev, dtype=torch.float32)
+            self.top_ids = torch.zeros(cols, MAX_TOP_LOGPROBS, device=dev, dtype=torch.int32)
+            self.top_lp = torch.zeros(cols, MAX_TOP_LOGPROBS, device=dev, dtype=torch.float32)
+            self.lp_n = torch.zeros(1, device=dev, dtype=torch.int32)
+            self.lp_ws, self.lp_counter = ops.logprobs_row_workspace(self.logits.numel(), dev)
+
+    def _ensure_penalties(self) -> None:
+        if self.pen_logits is None:
+            dev = self.llm.device
+            self.pen_logits = torch.zeros_like(self.logits)
+            self.presence = torch.zeros(1, device=dev, dtype=torch.float32)
+            self.frequency = torch.zeros(1, device=dev, dtype=torch.float32)
 
     LONG_CTX = 1024  # above: the wgmma split-KV path
 
@@ -798,6 +889,7 @@ class GraphDecoder:
             self._order_key = order_key
             self.graphs = {}
             self.sampled_graphs = {}
+            self.option_graphs = {}
         self.cache.length = 0
         self.num_splits, self.split_tokens = self.pick_splits(self.cache.max_tokens if tokens > self.LONG_CTX
                                                               else tokens)
@@ -825,21 +917,32 @@ class GraphDecoder:
 
     def _lm_head(self):
         cfg = self.llm.config
-        if self.sampled:
+        if self.sampled or self.penalised:
             ops.gemv(self.x, norm_w=self.llm.model.norm.weight, norm_eps=cfg.rms_norm_eps, out=self.logits,
                      static_w=True, **self._weights(None))
+        elif self.top_n is not None:  # greedy + logprobs: the row and the fused argmax key from the same values
+            ops.gemv(self.x, norm_w=self.llm.model.norm.weight, norm_eps=cfg.rms_norm_eps, out=self.logits,
+                     argmax_key=self.key, static_w=True, **self._weights(None))
         else:
             ops.gemv(self.x, norm_w=self.llm.model.norm.weight, norm_eps=cfg.rms_norm_eps, argmax_key=self.key,
                      write_out=False, static_w=True, **self._weights(None))
 
     def _finalize(self):
-        """the token (arg-max, or the draw in sampled mode) -> history, step++, position++, next x"""
+        """the token (arg-max, or the draw in sampled mode; from the penalised row with penalties) -> history, step++,
+        position++, next x; then the token's logprobs on the raw row when they are on"""
         emb = self.llm.model.embed_tokens.weight
-        if self.sampled:
-            ops.sample_finalize(self.logits, self.inv_temperature, self.top_k, self.top_p, self.seed, self.step,
-                                self.token, self.hist, self.position, emb, self.x)
+        if self.penalised:
+            ops.apply_penalties_row(self.logits, self.hist, self.step, self.presence, self.frequency,
+                                    out=self.pen_logits)
+        if self.sampled or self.penalised:
+            ops.sample_finalize(self.pen_logits if self.penalised else self.logits, self.inv_temperature, self.top_k,
+                                self.top_p, self.seed, self.step, self.token, self.hist, self.position, emb, self.x)
         else:
             ops.argmax_finalize(self.key, self.token, self.hist, self.step, self.position, emb, self.x)
+        if self.top_n is not None:  # n = self.lp_n, a device scalar: one graph for every n
+            ops.token_logprobs_row(self.logits, self.token, self.step, lp_hist=self.lp_hist, workspace=self.lp_ws,
+                                   counter=self.lp_counter, top_ids=self.top_ids, top_lp=self.top_lp,
+                                   n_used=self.lp_n)
 
     def _step(self):
         llm, cfg, cache = self.llm, self.llm.config, self.cache
@@ -865,12 +968,32 @@ class GraphDecoder:
         self._lm_head()
         self._finalize()
 
-    def start(self, last_hidden: torch.Tensor, cache: PagedKVCache, params: Optional[SamplingParams] = None) -> None:
+    def start(self, last_hidden: torch.Tensor, cache: PagedKVCache, params: Optional[SamplingParams] = None, *,
+              logprobs: Optional[int] = None, penalties: Optional[PenaltyParams] = None) -> None:
         """Seed the loop from the prefill: first new token = argmax(lm_head(norm(last_hidden))), or with
         non-greedy `params` (seed set) the draw of token index 0 from those logits; the following steps
-        run the matching graph.  params None or greedy: exactly the greedy path."""
+        run the matching graph.  params None or greedy: exactly the greedy path.
+        logprobs: None, or n in 0..20: every token's log-probability and its n most likely alternatives under the raw
+        row (vila_b200/logprobs.py), entry 0 from this first row (token_logprobs()).  penalties: a PenaltyParams,
+        applied to every row before the choice (vila_b200/penalties.py; the first token's history is empty, so its row
+        is unchanged); None or both values 0 is the path without them.  Neither works with a sequence-parallel
+        cache (NotImplementedError)."""
         assert cache is self.cache
+        top_n = None if logprobs is None else check_top(logprobs)
+        penalised = penalties is not None and not penalties.off
+        if (top_n is not None or penalised) and getattr(self, "_order_key", None) is not None:
+            raise NotImplementedError("sequence-parallel decode: logprobs and penalties are not implemented")
+        self.top_n, self.penalised = top_n, penalised
+        if top_n is not None:
+            self._ensure_logprobs()
+            self.lp_n.fill_(top_n)
+        if penalised:
+            self._ensure_penalties()
+            self.presence.fill_(penalties.presence)
+            self.frequency.fill_(penalties.frequency)
         self.sampled = params is not None and not params.greedy
+        if penalised and not self.sampled:
+            self.inv_temperature.fill_(0.0)  # vila_sample_finalize's greedy rule on the penalised row
         if self.sampled:
             if params.seed is None:
                 raise ValueError("GraphDecoder.start: sampling needs a seed (serving.sampling_for_requests draws one)")
@@ -894,18 +1017,56 @@ class GraphDecoder:
             self._started = 2
         if n <= 0:
             return
-        graphs = self.sampled_graphs if self.sampled else self.graphs
-        g = graphs.get((self.num_splits, self.split_tokens))
+        graphs, key = self._graph_dict_key()
+        g = graphs.get(key)
         if g is None:
             # warm-up launch outside capture is not allowed to change state: capture directly
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
                 self._step()
-            graphs[(self.num_splits, self.split_tokens)] = g
+            graphs[key] = g
         for _ in range(n):
             g.replay()
         self.cache.length += n
 
     def tokens(self, n: int) -> List[int]:
         return self.hist[:n].tolist()
+
+    def token_logprobs(self, n_tokens: int, start: int = 0) -> List[TokenLogprob]:
+        """tokens start .. n_tokens - 1 of the current request with their logprobs and top alternatives (start() with
+        logprobs): only those rows are copied to the host, so a stream that reads each chunk's new tokens does work
+        in proportion to them.  ValueError without logprobs."""
+        return self.read_logprobs(n_tokens, start)()
+
+    def read_logprobs(self, n_tokens: int, start: int = 0):
+        """token_logprobs in two halves: enqueue the copy of rows start .. n_tokens - 1 to the host now, and return a
+        function that waits for that copy alone and builds the entries.  Steps enqueued in between run on the device
+        while the host waits and builds (the streaming loop reads chunk k while chunk k + 1 decodes)."""
+        if self.top_n is None:
+            raise ValueError("GraphDecoder.token_logprobs: the current request was started without logprobs")
+        n, cols = self.top_n, self.lp_hist.numel()
+        a, b = max(0, start), min(n_tokens, cols)
+        if a >= b:
+            return lambda: []
+        # one device-to-host copy: [id, logprob bits, top ids..., top logprob bits...] per token
+        rows = torch.cat([self.hist[a:b, None], self.lp_hist[a:b, None].view(torch.int32), self.top_ids[a:b, :n],
+                          self.top_lp[a:b, :n].view(torch.int32)], dim=1)
+        done = None
+        if rows.is_cuda:
+            host = torch.empty(rows.shape, dtype=torch.int32, pin_memory=True)
+            host.copy_(rows, non_blocking=True)
+            done = torch.cuda.Event()
+            done.record()
+            rows = host
+
+        def entries() -> List[TokenLogprob]:
+            if done is not None:
+                done.synchronize()
+            ids = rows[:, 0].tolist()
+            lps = rows[:, 1].view(torch.float32).tolist()
+            top_i = rows[:, 2:2 + n].tolist()
+            top_v = rows[:, 2 + n:].contiguous().view(torch.float32).tolist()
+            return [TokenLogprob(t, lp, list(zip(ti, tv))) for t, lp, ti, tv in zip(ids, lps, top_i, top_v)]
+
+        return entries
 

@@ -12,7 +12,8 @@ import torch
 
 from . import _lib
 from ._lib import (DecodeAttnFp8Params, DecodeAttnParams, DecodeAttnSplitParams, FmhaParams, GemvBatchParams,
-                   GemvParams, LogprobsParams, PenaltyParams, SampleFinalizeParams, SampleParams, check)
+                   GemvParams, LogprobsParams, LogprobsRowParams, PenaltyParams, PenaltyRowParams,
+                   SampleFinalizeParams, SampleParams, check)
 
 ACT_NONE, ACT_GELU_TANH, ACT_GELU_ERF, ACT_SILU = 0, 1, 2, 3
 
@@ -776,6 +777,97 @@ def apply_penalties(logits: torch.Tensor, history: torch.Tensor, step: torch.Ten
     p.presence, p.frequency, p.out = _p(presence), _p(frequency), _p(out)
     p.M, p.V, p.cols = M, V, history.shape[1]
     check(_lib.load().vila_apply_penalties(C.byref(p), _stream()), "vila_apply_penalties")
+    return out
+
+
+LOGPROBS_ROW_CHUNK = 1152  # entries per CTA of vila_token_logprobs_row
+
+
+def logprobs_row_workspace(V: int, device) -> tuple:
+    """-> (workspace, counter): the scratch of token_logprobs_row for rows of V entries (one chunk's max, exp-sum and
+    20 candidate keys per 1152 entries) and its zeroed arrival counter, which every launch leaves at zero"""
+    chunks = (V + LOGPROBS_ROW_CHUNK - 1) // LOGPROBS_ROW_CHUNK
+    return (torch.zeros(chunks * 21, dtype=torch.int64, device=device),
+            torch.zeros(1, dtype=torch.int32, device=device))
+
+
+def token_logprobs_row(logits: torch.Tensor, token: torch.Tensor, step: torch.Tensor, *, lp_hist: torch.Tensor,
+                       workspace: torch.Tensor, counter: torch.Tensor, top_ids: Optional[torch.Tensor] = None,
+                       top_lp: Optional[torch.Tensor] = None, n_used: Optional[torch.Tensor] = None) -> None:
+    """token_logprobs' rule on one row, spread over one CTA per 1152 entries (vila_token_logprobs_row, one launch),
+    for the single-stream graph decoder.  logits: a contiguous bf16 row [V]; token int32 [1] (the chosen token); step
+    int32 [1], the decoder's counter already advanced past the token: the outputs go to column min(step - 1, cols - 1)
+    of lp_hist fp32 [cols], top_ids int32 [cols, n] and top_lp fp32 [cols, n], best first (both None: n = 0).
+    n_used: optional int32 [1] on the device, the number k of alternatives this launch computes (clamped to 0..n; the
+    entries past k are not written), so that one captured launch serves every k up to n.
+    workspace / counter: logprobs_row_workspace(V)."""
+    _need(logits.dim() == 1 and logits.is_contiguous() and 1 <= logits.numel() <= SAMPLE_MAX_VOCAB,
+          f"token_logprobs_row: logits must be a contiguous [V] row with V in 1..{SAMPLE_MAX_VOCAB}, got "
+          f"{tuple(logits.shape)}")
+    V = logits.numel()
+    _need((top_ids is None) == (top_lp is None), "token_logprobs_row: top_ids and top_lp go together")
+    _need(lp_hist.dim() == 1 and lp_hist.numel() >= 1 and lp_hist.is_contiguous(),
+          f"token_logprobs_row: lp_hist must be a contiguous [cols] buffer, got {tuple(lp_hist.shape)}")
+    cols = lp_hist.numel()
+    n = 0 if top_ids is None else top_ids.shape[-1]
+    need_ws = (V + LOGPROBS_ROW_CHUNK - 1) // LOGPROBS_ROW_CHUNK * 168
+    arrays = [(logits, "logits", torch.bfloat16), (token, "token", torch.int32), (step, "step", torch.int32),
+              (lp_hist, "lp_hist", torch.float32), (workspace, "workspace", torch.int64),
+              (counter, "counter", torch.int32)]
+    if n_used is not None:
+        arrays.append((n_used, "n_used", torch.int32))
+    if top_ids is not None:
+        for t, name in ((top_ids, "top_ids"), (top_lp, "top_lp")):
+            _need(t.dim() == 2 and t.shape == (cols, n) and t.is_contiguous(),
+                  f"token_logprobs_row: {name} must be a contiguous [{cols}, n] buffer, got {tuple(t.shape)}")
+        _need(0 <= n <= 20 and n <= V, f"token_logprobs_row: n={n} must be in 0..20 and <= V={V}")
+        arrays += [(top_ids, "top_ids", torch.int32), (top_lp, "top_lp", torch.float32)]
+    for t, name, dt in arrays:
+        _need(t.dtype == dt, f"token_logprobs_row: {name} must be {dt}, got {t.dtype}")
+        if name in ("token", "step", "counter", "n_used"):
+            _need(t.numel() == 1, f"token_logprobs_row: {name} must be a single value, got {tuple(t.shape)}")
+    _need(workspace.is_contiguous() and workspace.numel() * 8 >= need_ws,
+          f"token_logprobs_row: workspace must be a contiguous buffer of at least {need_ws} bytes for V={V} "
+          f"(logprobs_row_workspace), got {workspace.numel() * workspace.element_size()}")
+    for t, name, _ in arrays:
+        _chk(t, name, t.dtype)
+    p = LogprobsRowParams()
+    p.logits, p.token, p.step, p.lp_hist = _p(logits), _p(token), _p(step), _p(lp_hist)
+    p.top_ids, p.top_lp = (_p(top_ids), _p(top_lp)) if n else (None, None)
+    p.n_used = _p(n_used)
+    p.workspace, p.workspace_bytes, p.counter = _p(workspace), workspace.numel() * 8, _p(counter)
+    p.V, p.cols, p.n = V, cols, n
+    check(_lib.load().vila_token_logprobs_row(C.byref(p), _stream()), "vila_token_logprobs_row")
+
+
+def apply_penalties_row(logits: torch.Tensor, history: torch.Tensor, step: torch.Tensor, presence: torch.Tensor,
+                        frequency: torch.Tensor, *, out: torch.Tensor) -> torch.Tensor:
+    """apply_penalties' rule, bit for bit, on the single-stream graph decoder's one row (vila_apply_penalties_row, one
+    launch).  logits: a contiguous bf16 row [V]; history int32 [cols] (contiguous) of generated ids; step int32 [1]
+    (t: history entries 0..min(t, cols) - 1 count); presence and frequency fp32 [1].  out: a contiguous bf16 [V]
+    buffer.  -> out"""
+    _need(logits.dim() == 1 and logits.is_contiguous() and 1 <= logits.numel() <= SAMPLE_MAX_VOCAB,
+          f"apply_penalties_row: logits must be a contiguous [V] row with V in 1..{SAMPLE_MAX_VOCAB}, got "
+          f"{tuple(logits.shape)}")
+    V = logits.numel()
+    _need(history.dim() == 1 and history.numel() >= 1 and history.is_contiguous(),
+          f"apply_penalties_row: history must be a contiguous [cols] buffer, got {tuple(history.shape)}")
+    _need(out.shape == (V,) and out.is_contiguous(),
+          f"apply_penalties_row: out must be a contiguous [{V}] buffer, got {tuple(out.shape)}")
+    arrays = [(logits, "logits", torch.bfloat16), (history, "history", torch.int32), (step, "step", torch.int32),
+              (presence, "presence", torch.float32), (frequency, "frequency", torch.float32),
+              (out, "out", torch.bfloat16)]
+    for t, name, dt in arrays:
+        _need(t.dtype == dt, f"apply_penalties_row: {name} must be {dt}, got {t.dtype}")
+        if name in ("step", "presence", "frequency"):
+            _need(t.numel() == 1, f"apply_penalties_row: {name} must be a single value, got {tuple(t.shape)}")
+    for t, name, _ in arrays:
+        _chk(t, name, t.dtype)
+    p = PenaltyRowParams()
+    p.logits, p.history, p.step, p.presence, p.frequency = (_p(logits), _p(history), _p(step), _p(presence),
+                                                           _p(frequency))
+    p.out, p.V, p.cols = _p(out), V, history.numel()
+    check(_lib.load().vila_apply_penalties_row(C.byref(p), _stream()), "vila_apply_penalties_row")
     return out
 
 

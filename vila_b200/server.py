@@ -13,11 +13,13 @@ the model keeps between batches together with the K/V pages of the prompt blocks
 like an earlier one (another question about the same video or image) prefills only what follows the shared blocks.
 A non-streaming request with `logprobs` (and optionally `top_logprobs`, 0..20) is always decoded by the batched engine,
 which computes each token's log-probability and its top alternatives on the device (vila_b200/logprobs.py); its
-choice carries OpenAI's `logprobs.content` list.  Streaming requests cannot have logprobs yet: the single-stream
-decoder does not compute them.  A non-streaming request with a non-zero `presence_penalty` or `frequency_penalty` (each
-in [-2, 2]) is likewise always decoded by the batched engine, which applies OpenAI's penalties over the request's
-generated ids on the device (vila_b200/penalties.py), greedily unless --sample is set.  Streaming requests cannot have
-penalties yet: the single-stream decoder does not apply them.
+choice carries OpenAI's `logprobs.content` list.  A non-streaming request with a non-zero `presence_penalty` or
+`frequency_penalty` (each in [-2, 2]) is likewise always decoded by the batched engine, which applies OpenAI's penalties
+over the request's generated ids on the device (vila_b200/penalties.py), greedily unless --sample is set.  A streaming
+request with logprobs or a non-zero penalty is decoded by the single-stream graph decoder through the model's
+`stream_content`, which computes both on the device as well: each SSE chunk carries `choices[0].logprobs.content` for
+the ids it was decoded from (every id once, in order, the stop token excluded), even when those ids decode to no text.
+With a model that has no `stream_content`, such streaming requests are refused.
 
     python -m vila_b200.server --model-path <dir> --port 8000
 """
@@ -295,13 +297,17 @@ class Engine:
         """a streamed request's generation config: a copy of the model's default with the request's max_tokens,
         and do_sample set explicitly: with --sample the request's temperature, top_p (top_k 0) and seed, else
         greedy whatever the checkpoint's config says.  Bad values raise."""
-        if req.logprobs or req.top_logprobs is not None:
-            raise ValueError("logprobs are not supported with stream=true: the single-stream decoder that serves "
-                             "streaming requests does not compute them yet; send the request without stream")
-        if self._penalties(req) is not None:
-            raise ValueError("presence / frequency penalties are not supported with stream=true: the single-stream "
-                             "decoder that serves streaming requests does not apply them yet; send the request "
-                             "without stream")
+        if not hasattr(self.model, "stream_content"):
+            if req.logprobs or req.top_logprobs is not None:
+                raise ValueError("logprobs are not supported with stream=true: the single-stream decoder that serves "
+                                 "streaming requests does not compute them yet; send the request without stream")
+            if self._penalties(req) is not None:
+                raise ValueError("presence / frequency penalties are not supported with stream=true: the "
+                                 "single-stream decoder that serves streaming requests does not apply them yet; send "
+                                 "the request without stream")
+        else:  # bad values fail the request here, before streaming starts
+            self._top_logprobs(req)
+            self._penalties(req)
         gc = copy.copy(self.model.default_generation_config)
         gc.max_new_tokens = req.max_tokens
         gc.do_sample = False
@@ -311,18 +317,39 @@ class Engine:
             gc.temperature, gc.top_k, gc.top_p, gc.seed = p.temperature, 0, p.top_p, p.seed
         return gc
 
+    @staticmethod
+    def _sse_chunk(req: ChatCompletionRequest, chunk_id: int, text: str, content=None) -> str:
+        """one streamed chat.completion.chunk event: the text delta, and OpenAI's logprobs.content when given"""
+        choice: Dict[str, Any] = {"delta": {"content": text}}
+        if content is not None:
+            choice["logprobs"] = {"content": content}
+        chunk = {"id": str(chunk_id), "object": "chat.completion.chunk", "created": int(time.time()),
+                 "model": req.model, "choices": [choice]}
+        return f"data: {json.dumps(chunk)}\n\n"
+
     async def stream(self, req: ChatCompletionRequest):
         if req.model != self.model_name:
             raise ValueError(f"The endpoint is configured to use the model {self.model_name}, "
                              f"but the request model is {req.model}")
         gc = self._stream_config(req)  # a bad value fails this request before it takes the lock
+        top, pen = self._top_logprobs(req), self._penalties(req)
+        if top is not None or pen is not None:
+            async with self.lock:
+                gen = self.model.stream_content(build_prompt(req.messages), generation_config=gc, logprobs=top,
+                                                penalties=pen)
+                for chunk_id, (ids, entries) in enumerate(gen):
+                    text = self.model.tokenizer.decode(ids, skip_special_tokens=True)
+                    content = None if top is None else self._logprobs_content(ids, entries, top)
+                    if text or content:  # a chunk with entries is sent even when its ids decode to no text
+                        yield self._sse_chunk(req, chunk_id, text, content)
+                    await asyncio.sleep(0)
+                yield "data: [DONE]\n\n"
+            return
         async with self.lock:
             gen = self.model.generate_content(build_prompt(req.messages), generation_config=gc, stream=True)
             for chunk_id, new_text in enumerate(gen):
                 if len(new_text):
-                    chunk = {"id": str(chunk_id), "object": "chat.completion.chunk", "created": int(time.time()),
-                             "model": req.model, "choices": [{"delta": {"content": new_text}}]}
-                    yield f"data: {json.dumps(chunk)}\n\n"
+                    yield self._sse_chunk(req, chunk_id, new_text)
                 await asyncio.sleep(0)
             yield "data: [DONE]\n\n"
 
