@@ -29,24 +29,55 @@ def test_library_exports_every_declared_symbol():
     assert lib.vila_abi_version() == 3
 
 
+# the ctypes class in vila_b200/_lib.py of every parameter struct the header declares
+STRUCT_CLASSES = {
+    "vila_fmha_params": "FmhaParams",
+    "vila_gemv_params": "GemvParams",
+    "vila_gemv_batch_params": "GemvBatchParams",
+    "vila_decode_attn_params": "DecodeAttnParams",
+    "vila_decode_attn_split_params": "DecodeAttnSplitParams",
+    "vila_decode_attn_fp8_params": "DecodeAttnFp8Params",
+    "vila_sample_params": "SampleParams",
+    "vila_sample_finalize_params": "SampleFinalizeParams",
+    "vila_logprobs_params": "LogprobsParams",
+    "vila_logprobs_row_params": "LogprobsRowParams",
+    "vila_penalty_params": "PenaltyParams",
+    "vila_penalty_row_params": "PenaltyRowParams",
+}
+SCALAR_CTYPES = {"int64_t": ctypes.c_int64, "int32_t": ctypes.c_int32, "float": ctypes.c_float}
+
+
+def header_struct_fields(body):
+    """(name, is_pointer, base type) of every field of a struct body of the header, in declaration order."""
+    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
+    fields = []
+    for decl in body.split(";"):
+        decl = decl.strip()
+        if not decl:
+            continue
+        first, *rest = decl.split(",")
+        tokens = first.replace("*", " * ").split()
+        base = " ".join(t for t in tokens[:-1] if t not in ("*", "const"))
+        fields.append((tokens[-1], "*" in tokens, base))
+        fields.extend((x.strip().lstrip("*"), x.strip().startswith("*"), base) for x in rest)
+    return fields
+
+
 def test_struct_layouts_match_header_field_order():
     from vila_b200 import _lib
     text = (ROOT / "include" / "vila_b200.h").read_text()
-    for cname, cls in (("vila_fmha_params", _lib.FmhaParams), ("vila_gemv_params", _lib.GemvParams),
-                       ("vila_decode_attn_params", _lib.DecodeAttnParams),
-                       ("vila_decode_attn_split_params", _lib.DecodeAttnSplitParams)):
-        body = re.search(r"typedef struct %s \{(.*?)\} %s;" % (cname, cname), text, flags=re.S).group(1)
-        body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
-        fields = []
-        for decl in body.split(";"):
-            decl = decl.strip()
-            if not decl:
-                continue
-            names = decl.split(",")
-            first = names[0].split()[-1].lstrip("*")
-            fields.append(first)
-            fields.extend(x.strip().lstrip("*") for x in names[1:])
-        assert fields == [f[0] for f in cls._fields_], (cname, fields)
+    structs = dict(re.findall(r"typedef struct (vila_\w+_params) \{(.*?)\} \1;", text, flags=re.S))
+    assert sorted(structs) == sorted(STRUCT_CLASSES), "every parameter struct of the header needs a ctypes class"
+    for cname, body in structs.items():
+        cls = getattr(_lib, STRUCT_CLASSES[cname])
+        fields = header_struct_fields(body)
+        assert [f[0] for f in fields] == [f[0] for f in cls._fields_], (cname, fields)
+        for (name, is_pointer, base), (_, ctype) in zip(fields, cls._fields_):
+            if is_pointer:
+                assert ctype is ctypes.c_void_p or issubclass(ctype, ctypes._Pointer), (cname, name, ctype)
+            else:
+                assert base in SCALAR_CTYPES, f"{cname}.{name}: {base} has no ctypes counterpart here"
+                assert ctype is SCALAR_CTYPES[base], (cname, name, base, ctype)
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="CPU-only behaviour")

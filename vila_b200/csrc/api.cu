@@ -97,36 +97,14 @@ int vila_rmsnorm(void* x_inout, const void* residual_add, const void* weight, vo
                           st(stream));
 }
 
-static vb::FmhaParams to_fmha(const vila_fmha_params* p) {
-  vb::FmhaParams q;
-  q.q = cb(p->q);
-  q.q_tok_stride = p->q_tok_stride;
-  q.q_head_stride = p->q_head_stride;
-  q.k = cb(p->k);
-  q.v = cb(p->v);
-  q.kv_page_stride = p->kv_page_stride;
-  q.kv_tok_stride = p->kv_tok_stride;
-  q.kv_head_stride = p->kv_head_stride;
-  q.kv_num_pages = p->kv_num_pages;
-  q.page_table = p->page_table;
-  q.page_table_stride = p->page_table_stride;
-  q.o = mb(p->o);
-  q.o_tok_stride = p->o_tok_stride;
-  q.o_head_stride = p->o_head_stride;
-  q.B = p->B; q.Sq = p->Sq; q.Sk = p->Sk; q.Hq = p->Hq; q.Hkv = p->Hkv; q.D = p->D;
-  q.causal = p->causal;
-  q.scale = p->scale;
-  return q;
-}
-
 int vila_fmha(const vila_fmha_params* p, void* stream) {
   VB_REQUIRE_DEVICE();
-  return vb::fmha_prefill(to_fmha(p), st(stream));
+  return vb::fmha_prefill(*p, st(stream));
 }
 
 int vila_fmha_cfg(int variant, const vila_fmha_params* p, void* stream) {
   VB_REQUIRE_DEVICE();
-  return vb::fmha_prefill_cfg(variant, to_fmha(p), st(stream));
+  return vb::fmha_prefill_cfg(variant, *p, st(stream));
 }
 
 int vila_patch_im2col(const void* pixels, void* out, int B, int C, int H, int W, int patch,
@@ -258,28 +236,11 @@ int vila_gemv_w4a16(const vila_gemv_params* p, const void* w_scale, const uint8_
   return vb::gemv_tma_w4a16(to_gemv(p), cb(w_scale), w_zero, st(stream));
 }
 
-static vb::GemvBatchArgs to_gemv_batch(const vila_gemv_batch_params* p) {
-  vb::GemvBatchArgs g;
-  g.x = cb(p->x);
-  g.ldx = p->ldx;
-  g.w = p->w;
-  g.bias = cb(p->bias);
-  g.residual = cb(p->residual);
-  g.ld_res = p->ld_res;
-  g.y = mb(p->y);
-  g.ldy = p->ldy;
-  g.M = p->M;
-  g.N = p->N;
-  g.K = p->K;
-  g.flags = p->flags;
-  return g;
-}
-
 // the Linear layers of a batched decode step (modeling_qwen2.py:81-95,164-176,223-226) on e4m3 weights
 int vila_gemv_batch_fp8(const vila_gemv_batch_params* p, const float* w_scale, void* stream) {
   VB_REQUIRE_DEVICE();
   VB_CHECK(p != nullptr, "vila_gemv_batch_fp8: params are required");
-  return vb::gemv_batch_fp8(to_gemv_batch(p), w_scale, st(stream));
+  return vb::gemv_batch_fp8(*p, w_scale, st(stream));
 }
 
 // the TinyChat W4A16 GEMM of the reference's 4-bit deployment (README "Quantization and Deployment")
@@ -287,7 +248,7 @@ int vila_gemv_batch_w4a16(const vila_gemv_batch_params* p, const void* w_scale, 
                           void* stream) {
   VB_REQUIRE_DEVICE();
   VB_CHECK(p != nullptr, "vila_gemv_batch_w4a16: params are required");
-  return vb::gemv_batch_w4a16(to_gemv_batch(p), cb(w_scale), w_zero, st(stream));
+  return vb::gemv_batch_w4a16(*p, cb(w_scale), w_zero, st(stream));
 }
 
 int vila_gemv_batch_partition(int N, int K, int fp8, int32_t* out) {
@@ -305,76 +266,28 @@ int vila_argmax_finalize(unsigned long long* key, int32_t* token_out, int32_t* t
 
 int vila_decode_attention(const vila_decode_attn_params* p, void* stream) {
   VB_REQUIRE_DEVICE();
-  vb::DecodeAttnParams d;
-  d.qkv = mb(p->qkv);
-  d.position = p->position;
-  d.k_pool = mb(p->k_pool);
-  d.v_pool = mb(p->v_pool);
-  d.page_table = p->page_table;
-  d.out = mb(p->out);
-  d.ws = p->ws;
-  d.counters = p->counters;
-  d.inv_freq = p->inv_freq;
-  d.Hq = p->Hq; d.Hkv = p->Hkv; d.D = p->D; d.num_splits = p->num_splits;
-  d.scale = p->scale;
-  return vb::decode_attention(d, st(stream));
+  return vb::decode_attention(*p, st(stream));
 }
 
 int vila_decode_attention_batch(const vila_decode_attn_params* p, int batch, int qkv_stride,
                                 int out_stride, int pt_stride, int max_pages, void* stream) {
   VB_REQUIRE_DEVICE();
-  vb::DecodeAttnParams d;
-  d.qkv = mb(p->qkv);
-  d.position = p->position;
-  d.k_pool = mb(p->k_pool);
-  d.v_pool = mb(p->v_pool);
-  d.page_table = p->page_table;
-  d.out = mb(p->out);
+  vila_decode_attn_params d = *p;  // the batched kernel has no split: ws, counters and num_splits are ignored
   d.ws = nullptr;
   d.counters = nullptr;
-  d.inv_freq = p->inv_freq;
-  d.Hq = p->Hq; d.Hkv = p->Hkv; d.D = p->D; d.num_splits = 0;
-  d.scale = p->scale;
+  d.num_splits = 0;
   return vb::decode_attention_batch(d, batch, qkv_stride, out_stride, pt_stride, max_pages, st(stream));
 }
 
 int vila_decode_attention_split(const vila_decode_attn_split_params* p, void* stream) {
   VB_REQUIRE_DEVICE();
-  vb::DecodeAttnSplitParams d;
-  d.qkv = mb(p->qkv);
-  d.position = p->position;
-  d.k_pool = mb(p->k_pool);
-  d.v_pool = mb(p->v_pool);
-  d.page_table = p->page_table;
-  d.kv_num_pages = p->kv_num_pages;
-  d.out = mb(p->out);
-  d.o_partial = p->o_partial;
-  d.lse = p->lse;
-  d.counters = p->counters;
-  d.inv_freq = p->inv_freq;
-  d.Hq = p->Hq; d.Hkv = p->Hkv; d.D = p->D; d.num_splits = p->num_splits; d.split_tokens = p->split_tokens;
-  d.scale = p->scale;
-  return vb::decode_attention_split(d, st(stream));
+  return vb::decode_attention_split(*p, st(stream));
 }
 
 int vila_decode_attention_split_batch(const vila_decode_attn_split_params* p, int batch, int qkv_stride,
                                       int out_stride, int pt_stride, void* stream) {
   VB_REQUIRE_DEVICE();
-  vb::DecodeAttnSplitParams d;
-  d.qkv = mb(p->qkv);
-  d.position = p->position;
-  d.k_pool = mb(p->k_pool);
-  d.v_pool = mb(p->v_pool);
-  d.page_table = p->page_table;
-  d.kv_num_pages = p->kv_num_pages;
-  d.out = mb(p->out);
-  d.o_partial = p->o_partial;
-  d.lse = p->lse;
-  d.counters = p->counters;
-  d.inv_freq = p->inv_freq;
-  d.Hq = p->Hq; d.Hkv = p->Hkv; d.D = p->D; d.num_splits = p->num_splits; d.split_tokens = p->split_tokens;
-  d.scale = p->scale;
-  return vb::decode_attention_split_batch(d, batch, qkv_stride, out_stride, pt_stride, st(stream));
+  return vb::decode_attention_split_batch(*p, batch, qkv_stride, out_stride, pt_stride, st(stream));
 }
 
 // DynamicCache.update + flash-attn decode (modeling_qwen2.py:99-160,262-310) over an e4m3 KV pool
@@ -388,135 +301,54 @@ int vila_kv_quantize_fp8(const void* src, int64_t src_tokens, void* dst, float* 
 int vila_decode_attention_fp8_batch(const vila_decode_attn_fp8_params* p, void* stream) {
   VB_REQUIRE_DEVICE();
   VB_CHECK(p != nullptr, "vila_decode_attention_fp8_batch: params are required");
-  vb::DecodeAttnFp8Params d;
-  d.qkv = cb(p->qkv);
-  d.position = p->position;
-  d.k_pool = static_cast<uint8_t*>(p->k_pool);
-  d.v_pool = static_cast<uint8_t*>(p->v_pool);
-  d.k_scale = p->k_scale;
-  d.v_scale = p->v_scale;
-  d.page_table = p->page_table;
-  d.out = mb(p->out);
-  d.ws = p->ws;
-  d.counters = p->counters;
-  d.inv_freq = p->inv_freq;
-  d.Hq = p->Hq; d.Hkv = p->Hkv; d.D = p->D; d.batch = p->batch;
-  d.qkv_stride = p->qkv_stride; d.out_stride = p->out_stride; d.pt_stride = p->pt_stride;
-  d.num_splits = p->num_splits; d.split_tokens = p->split_tokens;
-  d.scale = p->scale;
-  return vb::decode_attention_fp8_batch(d, st(stream));
+  return vb::decode_attention_fp8_batch(*p, st(stream));
 }
 
 // HF Temperature / TopK / TopP LogitsWarper + torch.multinomial (GenerationMixin._sample)
 int vila_sample_batch(const vila_sample_params* p, void* stream) {
   VB_REQUIRE_DEVICE();
   VB_CHECK(p != nullptr, "vila_sample_batch: params are required");
-  vb::SampleParams d;
-  d.logits = cb(p->logits);
-  d.ld = p->ld;
-  d.inv_temperature = p->inv_temperature;
-  d.top_k = p->top_k;
-  d.top_p = p->top_p;
-  d.seed = p->seed;
-  d.step = p->step;
-  d.position = p->position;
-  d.tokens = p->tokens;
-  d.n_kept = p->n_kept;
-  d.M = p->M; d.V = p->V;
-  return vb::sample_batch(d, st(stream));
+  return vb::sample_batch(*p, st(stream));
 }
 
 // GenerationMixin._sample's warpers + torch.multinomial for the single-stream graph decoder
 int vila_sample_finalize(const vila_sample_finalize_params* p, void* stream) {
   VB_CHECK(p != nullptr, "vila_sample_finalize: params are required");
-  vb::SampleFinalizeParams d;
-  d.logits = cb(p->logits);
-  d.inv_temperature = p->inv_temperature;
-  d.top_k = p->top_k;
-  d.top_p = p->top_p;
-  d.seed = p->seed;
-  d.step = p->step;
-  d.position = p->position;
-  d.token_out = p->token_out;
-  d.token_hist = p->token_hist;
-  d.embed_table = cb(p->embed_table);
-  d.x_next = mb(p->x_next);
-  d.V = p->V; d.hidden = p->hidden;
-  if (int rc = vb::sample_finalize_check(d)) return rc;
+  if (int rc = vb::sample_finalize_check(*p)) return rc;
   VB_REQUIRE_DEVICE();
-  return vb::sample_finalize(d, st(stream));
+  return vb::sample_finalize(*p, st(stream));
 }
 
 // HF generate(output_scores=True) + torch.log_softmax / OpenAI logprobs for the batched engine
 int vila_token_logprobs(const vila_logprobs_params* p, void* stream) {
   VB_CHECK(p != nullptr, "vila_token_logprobs: params are required");
-  vb::LogprobParams d;
-  d.logits = cb(p->logits);
-  d.ld = p->ld;
-  d.tokens = p->tokens;
-  d.step = p->step;
-  d.position = p->position;
-  d.lp_hist = p->lp_hist;
-  d.top_ids = p->top_ids;
-  d.top_lp = p->top_lp;
-  d.M = p->M; d.V = p->V; d.cols = p->cols; d.n = p->n;
-  if (int rc = vb::token_logprobs_check(d)) return rc;
+  if (int rc = vb::token_logprobs_check(*p)) return rc;
   VB_REQUIRE_DEVICE();
-  return vb::token_logprobs(d, st(stream));
+  return vb::token_logprobs(*p, st(stream));
 }
 
 // the same for the single-stream graph decoder's one row
 int vila_token_logprobs_row(const vila_logprobs_row_params* p, void* stream) {
   VB_CHECK(p != nullptr, "vila_token_logprobs_row: params are required");
-  vb::LogprobRowParams d;
-  d.logits = cb(p->logits);
-  d.token = p->token;
-  d.step = p->step;
-  d.lp_hist = p->lp_hist;
-  d.top_ids = p->top_ids;
-  d.top_lp = p->top_lp;
-  d.n_used = p->n_used;
-  d.workspace = p->workspace;
-  d.workspace_bytes = p->workspace_bytes;
-  d.counter = p->counter;
-  d.V = p->V; d.cols = p->cols; d.n = p->n;
-  if (int rc = vb::token_logprobs_row_check(d)) return rc;
+  if (int rc = vb::token_logprobs_row_check(*p)) return rc;
   VB_REQUIRE_DEVICE();
-  return vb::token_logprobs_row(d, st(stream));
+  return vb::token_logprobs_row(*p, st(stream));
 }
 
 // OpenAI presence_penalty / frequency_penalty for the batched engine (the reference serves neither)
 int vila_apply_penalties(const vila_penalty_params* p, void* stream) {
   VB_CHECK(p != nullptr, "vila_apply_penalties: params are required");
-  vb::PenaltyParams d;
-  d.logits = cb(p->logits);
-  d.ld = p->ld;
-  d.history = p->history;
-  d.step = p->step;
-  d.position = p->position;
-  d.presence = p->presence;
-  d.frequency = p->frequency;
-  d.out = mb(p->out);
-  d.M = p->M; d.V = p->V; d.cols = p->cols;
-  if (int rc = vb::apply_penalties_check(d)) return rc;
+  if (int rc = vb::apply_penalties_check(*p)) return rc;
   VB_REQUIRE_DEVICE();
-  return vb::apply_penalties(d, st(stream));
+  return vb::apply_penalties(*p, st(stream));
 }
 
 // the same for the single-stream graph decoder's one row
 int vila_apply_penalties_row(const vila_penalty_row_params* p, void* stream) {
   VB_CHECK(p != nullptr, "vila_apply_penalties_row: params are required");
-  vb::PenaltyRowParams d;
-  d.logits = cb(p->logits);
-  d.history = p->history;
-  d.step = p->step;
-  d.presence = p->presence;
-  d.frequency = p->frequency;
-  d.out = mb(p->out);
-  d.V = p->V; d.cols = p->cols;
-  if (int rc = vb::apply_penalties_row_check(d)) return rc;
+  if (int rc = vb::apply_penalties_row_check(*p)) return rc;
   VB_REQUIRE_DEVICE();
-  return vb::apply_penalties_row(d, st(stream));
+  return vb::apply_penalties_row(*p, st(stream));
 }
 
 // the reference prefills every request in full (serving/server.py:65-73, llava_arch.py:823-833): no seam

@@ -255,8 +255,12 @@ constexpr int kMaxG = 8;  // query heads per kv head
 
 template <int D, int G, bool kCluster>
 __global__ void __launch_bounds__(kDaThreads)
-decode_attn_kernel(DecodeAttnParams p) {
+decode_attn_kernel(vila_decode_attn_params p) {
   const float* __restrict__ inv_freq = p.inv_freq;
+  __nv_bfloat16* qkv = static_cast<__nv_bfloat16*>(p.qkv);
+  __nv_bfloat16* k_pool = static_cast<__nv_bfloat16*>(p.k_pool);
+  __nv_bfloat16* v_pool = static_cast<__nv_bfloat16*>(p.v_pool);
+  __nv_bfloat16* out = static_cast<__nv_bfloat16*>(p.out);
   static_assert(D == 128, "decode attention is specialised for head_dim 128");
   constexpr int VPT = 8;             // elements per lane (16 bytes)
   constexpr int LPT = D / VPT;       // lanes per token (16)
@@ -285,8 +289,8 @@ decode_attn_kernel(DecodeAttnParams p) {
       if (t < t1 && t != pos) {
         const int page = p.page_table[t >> 7];
         const size_t o = ((static_cast<size_t>(page) * 128 + (t & 127)) * p.Hkv + hk) * D + dl * VPT;
-        kreg[i] = ldg_v4(p.k_pool + o);
-        vreg[i] = ldg_v4(p.v_pool + o);
+        kreg[i] = ldg_v4(k_pool + o);
+        vreg[i] = ldg_v4(v_pool + o);
       }
     }
   };
@@ -307,7 +311,7 @@ decode_attn_kernel(DecodeAttnParams p) {
   for (int idx = threadIdx.x; idx < (G + 1) * (D / 2); idx += blockDim.x) {
     const int hh = idx / (D / 2), i = idx % (D / 2);
     const __nv_bfloat16* src =
-        hh < G ? p.qkv + (hk * G + hh) * D : p.qkv + (p.Hq + hk) * D;
+        hh < G ? qkv + (hk * G + hh) * D : qkv + (p.Hq + hk) * D;
     const float x0 = __bfloat162float(src[i]), x1 = __bfloat162float(src[i + D / 2]);
     const float ang = (float)pos * inv_freq[i];
     float sn, cs;
@@ -324,14 +328,14 @@ decode_attn_kernel(DecodeAttnParams p) {
       knew_s[i + D / 2] = __float2bfloat16(y1);
     }
   }
-  for (int i = threadIdx.x; i < D; i += blockDim.x) vnew_s[i] = p.qkv[(p.Hq + p.Hkv + hk) * D + i];
+  for (int i = threadIdx.x; i < D; i += blockDim.x) vnew_s[i] = qkv[(p.Hq + p.Hkv + hk) * D + i];
   __syncthreads();
   if (split == 0) {  // KV append (DynamicCache.update)
     const int page = p.page_table[pos >> 7];
     const size_t o = ((static_cast<size_t>(page) * 128 + (pos & 127)) * p.Hkv + hk) * D;
     for (int i = threadIdx.x; i < D; i += blockDim.x) {
-      p.k_pool[o + i] = knew_s[i];
-      p.v_pool[o + i] = vnew_s[i];
+      k_pool[o + i] = knew_s[i];
+      v_pool[o + i] = vnew_s[i];
     }
   }
 
@@ -440,7 +444,7 @@ decode_attn_kernel(DecodeAttnParams p) {
         ll += cluster.map_shared_rank(&part_l[0], s)[g] * w;
         oo += cluster.map_shared_rank(&part_o[0][0], s)[g * D + d] * w;
       }
-      p.out[(hk * G + g) * D + d] = __float2bfloat16(oo / ll);
+      out[(hk * G + g) * D + d] = __float2bfloat16(oo / ll);
     }
     cluster.sync();  // peers may still be reading this CTA's shared memory
     return;
@@ -489,7 +493,7 @@ decode_attn_kernel(DecodeAttnParams p) {
       ll += ws_l[base] * w;
       oo += ws_o[base * D + d] * w;
     }
-    p.out[(hk * G + g) * D + d] = __float2bfloat16(oo / ll);
+    out[(hk * G + g) * D + d] = __float2bfloat16(oo / ll);
   }
 }
 
@@ -510,8 +514,23 @@ constexpr int kDhMaxPages = 32;  // <= 4096 tokens per sequence
 // Batched form (continuous batching over ONE shared paged pool, vila_b200/serving.py): blockIdx.y is
 // the sequence; each has its own row of qkv / out, its own position and its own page-table row.
 // positions[b] < 0 marks an idle slot (the CTA exits).  The single-sequence entry point is batch 1.
+// The kernel reads vila_decode_attn_params through typed pointers, in a struct of the same layout filled by
+// head_args(): offsetting the C-ABI struct's void pointers inside the kernel compiles to different code.
+struct DecodeAttnHeadParams {
+  __nv_bfloat16* qkv;
+  const int32_t* position;
+  __nv_bfloat16* k_pool;
+  __nv_bfloat16* v_pool;
+  const int32_t* page_table;
+  __nv_bfloat16* out;
+  float* ws;
+  int32_t* counters;
+  const float* inv_freq;
+  int Hq, Hkv, D, num_splits;
+  float scale;
+};
 struct DecodeAttnBatchArgs {
-  DecodeAttnParams p;  // qkv / out / position / page_table point at sequence 0
+  DecodeAttnHeadParams p;  // qkv / out / position / page_table point at sequence 0
   int batch;
   int qkv_stride, out_stride, pt_stride;  // elements between consecutive sequences
   int max_pages;                          // valid entries per page-table row (<= kDhMaxPages)
@@ -522,7 +541,7 @@ __global__ void __launch_bounds__(kDhThreads)
 decode_attn_head_kernel(DecodeAttnBatchArgs args) {
   static_assert(D == 128, "head_dim 128");
   constexpr int VPT = 8, LPT = D / VPT;
-  DecodeAttnParams p = args.p;
+  DecodeAttnHeadParams p = args.p;
   {
     const int b = blockIdx.y;
     p.qkv += static_cast<size_t>(b) * args.qkv_stride;
@@ -715,6 +734,14 @@ __global__ void decode_combine_kernel(const float* __restrict__ o_partial, const
   }
 }
 
+DecodeAttnBatchArgs head_args(const vila_decode_attn_params& p, int batch, int qkv_stride, int out_stride,
+                              int pt_stride, int max_pages) {
+  using bf = __nv_bfloat16;
+  return {{static_cast<bf*>(p.qkv), p.position, static_cast<bf*>(p.k_pool), static_cast<bf*>(p.v_pool), p.page_table,
+           static_cast<bf*>(p.out), p.ws, p.counters, p.inv_freq, p.Hq, p.Hkv, p.D, p.num_splits, p.scale},
+          batch, qkv_stride, out_stride, pt_stride, max_pages};
+}
+
 }  // namespace
 
 int gemv_bf16(const GemvParams& p, cudaStream_t stream) {
@@ -753,14 +780,14 @@ int argmax_finalize(unsigned long long* key, int32_t* token_out, int32_t* token_
   return 0;
 }
 
-int decode_attention(const DecodeAttnParams& p, cudaStream_t stream) {
+int decode_attention(const vila_decode_attn_params& p, cudaStream_t stream) {
   VB_CHECK(p.D == 128, "decode_attention: head_dim must be 128 (got %d)", p.D);
   VB_CHECK(p.Hq % p.Hkv == 0, "decode_attention: Hq %% Hkv != 0");
   VB_CHECK(p.num_splits >= 0 && p.num_splits <= 64, "decode_attention: bad num_splits %d",
            p.num_splits);
   if (p.num_splits == 0) {
     // one CTA per query head, no split: contexts of at most 1024 tokens (8 pages), see the kernel
-    DecodeAttnBatchArgs a{p, 1, 0, 0, 0, 8};
+    const DecodeAttnBatchArgs a = head_args(p, 1, 0, 0, 0, 8);
     VB_CUDA(launch_pdl(decode_attn_head_kernel<128, 4>, dim3(p.Hq), dim3(kDhThreads), 0, stream, a));
     return 0;
   }
@@ -802,16 +829,17 @@ int decode_attention(const DecodeAttnParams& p, cudaStream_t stream) {
 //      producer / MMA / softmax pipeline on every SM
 //   3. the combine: by the last split CTA of every KV head inside (2) when `counters` is given, else
 //      decode_combine_kernel
-int decode_attention_split(const DecodeAttnSplitParams& p, cudaStream_t stream) {
+int decode_attention_split(const vila_decode_attn_split_params& p, cudaStream_t stream) {
   VB_CHECK(p.D == 128, "decode_attention_split: head_dim must be 128 (got %d)", p.D);
   VB_CHECK(p.Hq % p.Hkv == 0, "decode_attention_split: Hq %% Hkv != 0");
   VB_CHECK(p.num_splits >= 1 && p.split_tokens > 0 && p.split_tokens % 128 == 0,
            "decode_attention_split: bad split configuration (%d x %d)", p.num_splits, p.split_tokens);
   const int G = p.Hq / p.Hkv;
-  int rc = rope_kv_append(p.qkv, p.position, 1, p.Hq, p.Hkv, p.D, p.inv_freq, p.k_pool, p.v_pool,
+  int rc = rope_kv_append(static_cast<__nv_bfloat16*>(p.qkv), p.position, 1, p.Hq, p.Hkv, p.D, p.inv_freq,
+                          static_cast<__nv_bfloat16*>(p.k_pool), static_cast<__nv_bfloat16*>(p.v_pool),
                           p.page_table, -1, stream);
   if (rc) return rc;
-  FmhaParams f;
+  vila_fmha_params f;
   f.q = p.qkv;
   f.q_tok_stride = p.D;                       // "token" = query head g of the group
   f.q_head_stride = static_cast<int64_t>(G) * p.D;   // "head" = KV head
@@ -839,8 +867,8 @@ int decode_attention_split(const DecodeAttnSplitParams& p, cudaStream_t stream) 
   if (p.counters != nullptr) return 0;  // combined by the last split CTA of every KV head
   VB_CHECK(p.num_splits <= kCombineMaxSplits, "decode_attention_split: at most %d splits", kCombineMaxSplits);
   VB_CUDA(launch_pdl(decode_combine_kernel, dim3(p.Hq), dim3(128), 0, stream,
-                     static_cast<const float*>(p.o_partial), static_cast<const float*>(p.lse), p.out,
-                     p.Hq, p.D, p.num_splits));
+                     static_cast<const float*>(p.o_partial), static_cast<const float*>(p.lse),
+                     static_cast<__nv_bfloat16*>(p.out), p.Hq, p.D, p.num_splits));
   return 0;
 }
 
@@ -848,7 +876,7 @@ int decode_attention_split(const DecodeAttnSplitParams& p, cudaStream_t stream) 
 // Batched long-context decode attention (continuous batching at video contexts): the two launches of
 // decode_attention_split with the fused combine, over `batch` sequences at once.  Sequence b's output is
 // bit-identical to decode_attention_split on that sequence alone with the same split configuration.
-int decode_attention_split_batch(const DecodeAttnSplitParams& p, int batch, int qkv_stride, int out_stride,
+int decode_attention_split_batch(const vila_decode_attn_split_params& p, int batch, int qkv_stride, int out_stride,
                                  int pt_stride, cudaStream_t stream) {
   VB_CHECK(p.D == 128, "decode_attention_split_batch: head_dim must be 128 (got %d)", p.D);
   VB_CHECK(p.Hq % p.Hkv == 0, "decode_attention_split_batch: Hq %% Hkv != 0");
@@ -861,10 +889,11 @@ int decode_attention_split_batch(const DecodeAttnSplitParams& p, int batch, int 
            "decode_attention_split_batch: bad strides (qkv %d, out %d, page table %d)", qkv_stride, out_stride,
            pt_stride);
   const int G = p.Hq / p.Hkv;
-  int rc = rope_kv_append_decode_batch(p.qkv, qkv_stride, p.position, batch, p.Hq, p.Hkv, p.D, p.inv_freq,
-                                       p.k_pool, p.v_pool, p.page_table, pt_stride, stream);
+  int rc = rope_kv_append_decode_batch(static_cast<__nv_bfloat16*>(p.qkv), qkv_stride, p.position, batch, p.Hq,
+                                       p.Hkv, p.D, p.inv_freq, static_cast<__nv_bfloat16*>(p.k_pool),
+                                       static_cast<__nv_bfloat16*>(p.v_pool), p.page_table, pt_stride, stream);
   if (rc) return rc;
-  FmhaParams f;
+  vila_fmha_params f;
   f.q = p.qkv;
   f.q_tok_stride = p.D;
   f.q_head_stride = static_cast<int64_t>(G) * p.D;
@@ -891,14 +920,14 @@ int decode_attention_split_batch(const DecodeAttnSplitParams& p, int batch, int 
                            qkv_stride, out_stride);
 }
 
-int decode_attention_batch(const DecodeAttnParams& p, int batch, int qkv_stride, int out_stride,
+int decode_attention_batch(const vila_decode_attn_params& p, int batch, int qkv_stride, int out_stride,
                            int pt_stride, int max_pages, cudaStream_t stream) {
   VB_CHECK(p.D == 128, "decode_attention_batch: head_dim must be 128 (got %d)", p.D);
   VB_CHECK(p.Hq % p.Hkv == 0, "decode_attention_batch: Hq %% Hkv != 0");
   VB_CHECK(batch >= 1 && batch <= 65535, "decode_attention_batch: bad batch %d", batch);
   VB_CHECK(max_pages >= 1 && max_pages <= kDhMaxPages && max_pages <= pt_stride,
            "decode_attention_batch: 1 <= max_pages (%d) <= min(%d, pt_stride %d)", max_pages, kDhMaxPages, pt_stride);
-  DecodeAttnBatchArgs a{p, batch, qkv_stride, out_stride, pt_stride, max_pages};
+  const DecodeAttnBatchArgs a = head_args(p, batch, qkv_stride, out_stride, pt_stride, max_pages);
   VB_CUDA(launch_pdl(decode_attn_head_kernel<128, 4>, dim3(p.Hq, batch), dim3(kDhThreads), 0, stream, a));
   return 0;
 }

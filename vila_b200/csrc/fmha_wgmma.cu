@@ -403,7 +403,7 @@ struct SplitArgs {
 };
 
 template <int DP, int CW, int kPolyEvery = 0>
-int launch_fmha(const FmhaParams& p, cudaStream_t stream, const SplitArgs* split = nullptr) {
+int launch_fmha(const vila_fmha_params& p, cudaStream_t stream, const SplitArgs* split = nullptr) {
   using C = FmhaCfg<DP, CW>;
   CUtensorMap tq, tk, tv;
   const int batch = split ? split->batch : 0;
@@ -433,7 +433,7 @@ int launch_fmha(const FmhaParams& p, cudaStream_t stream, const SplitArgs* split
     if (make_tmap_nd_bf16(&tv, p.v, 4, dims, str, box, C::kSwizzleBytes)) return 1;
   }
   FmhaKernelArgs a;
-  a.o = p.o;
+  a.o = static_cast<__nv_bfloat16*>(p.o);
   a.o_tok_stride = p.o_tok_stride;
   a.o_head_stride = p.o_head_stride;
   a.page_table = p.page_table;
@@ -460,7 +460,7 @@ int launch_fmha(const FmhaParams& p, cudaStream_t stream, const SplitArgs* split
 }
 
 template <int kPolyEvery>
-int launch_fmha_for_head_dim(const FmhaParams& p, cudaStream_t stream) {
+int launch_fmha_for_head_dim(const vila_fmha_params& p, cudaStream_t stream) {
   if (p.D == 128) return launch_fmha<128, 64, kPolyEvery>(p, stream);
   if (p.D <= 96 && p.D > 64) return launch_fmha<96, 32, kPolyEvery>(p, stream);
   if (p.D == 64) return launch_fmha<64, 64, kPolyEvery>(p, stream);
@@ -470,7 +470,7 @@ int launch_fmha_for_head_dim(const FmhaParams& p, cudaStream_t stream) {
 
 }  // namespace
 
-int fmha_prefill(const FmhaParams& p, cudaStream_t stream) { return fmha_prefill_cfg(0, p, stream); }
+int fmha_prefill(const vila_fmha_params& p, cudaStream_t stream) { return fmha_prefill_cfg(0, p, stream); }
 
 // Split-KV attention of ONE long sequence for a handful of query rows (decode: the G query heads of a
 // KV group are the "rows" of the 128-row tile, the KV heads are the "heads"): p.B = number of KV
@@ -482,7 +482,7 @@ int fmha_prefill(const FmhaParams& p, cudaStream_t stream) { return fmha_prefill
 // (< 0: idle), queries at p.q + s*q_seq_stride, page-table row p.page_table + s*p.page_table_stride,
 // partials / lse / counters the s-th block of [B][Hq][Sq][D] / [B][Hq][Sq] / [Hq], output at
 // p.o + s*o_seq_stride; the fused combine (counters) is required.
-int fmha_decode_split(const FmhaParams& p, const int32_t* n_tok_minus_1, int split_tokens,
+int fmha_decode_split(const vila_fmha_params& p, const int32_t* n_tok_minus_1, int split_tokens,
                       float* o_partial, float* lse, int* counters, cudaStream_t stream,
                       int batch, int64_t q_seq_stride, int64_t o_seq_stride) {
   VB_CHECK(p.D == 128, "fmha_decode_split: head dim must be 128");
@@ -500,7 +500,7 @@ int fmha_decode_split(const FmhaParams& p, const int32_t* n_tok_minus_1, int spl
 
 // variant: 0 = default, 1 / 2 = the wgmma kernel (kept as separate selectors so callers can pin a
 // kernel), 3 / 4 = the same kernel with every 4th / 2nd exp2 computed by the FMA-pipe polynomial.
-int fmha_prefill_cfg(int variant, const FmhaParams& p, cudaStream_t stream) {
+int fmha_prefill_cfg(int variant, const vila_fmha_params& p, cudaStream_t stream) {
   VB_CHECK(variant >= 0 && variant <= 4, "fmha: unknown variant %d", variant);
   VB_CHECK(p.B > 0 && p.Sq > 0 && p.Sk > 0, "fmha: empty problem");
   VB_CHECK(p.Hq % p.Hkv == 0, "fmha: Hq (%d) must be a multiple of Hkv (%d)", p.Hq, p.Hkv);

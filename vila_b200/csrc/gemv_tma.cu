@@ -668,33 +668,36 @@ __device__ __forceinline__ float ld_dsmem_f32(uint32_t cluster_addr) {
 // epilogue of one output element (row n, x row m), with the rounding points of gemv_epilogue; sc: the row
 // scales of the row block staged in shared memory, row n at sc[n - row0]
 template <bool kFp8>
-__device__ __forceinline__ void batch_finish(const GemvBatchArgs& p, const float* sc, int row0, int n, int m,
+__device__ __forceinline__ void batch_finish(const vila_gemv_batch_params& p, const float* sc, int row0, int n, int m,
                                              float v) {
+  const __nv_bfloat16* bias = static_cast<const __nv_bfloat16*>(p.bias);
+  const __nv_bfloat16* residual = static_cast<const __nv_bfloat16*>(p.residual);
   if constexpr (kFp8) v *= sc[n - row0];
-  if (p.bias) v += __bfloat162float(p.bias[n]);
+  if (bias) v += __bfloat162float(bias[n]);
   v = bf16_round(v);
-  if (p.residual) v = bf16_round(v + __bfloat162float(p.residual[m * p.ld_res + n]));
-  p.y[m * p.ldy + n] = __float2bfloat16(v);
+  if (residual) v = bf16_round(v + __bfloat162float(residual[m * p.ld_res + n]));
+  static_cast<__nv_bfloat16*>(p.y)[m * p.ldy + n] = __float2bfloat16(v);
 }
 template <bool kFp8>
-__device__ __forceinline__ void batch_finish_swiglu(const GemvBatchArgs& p, const float* sc, int row0, int n,
-                                                    int m, float g, float u) {  // n even: gate n, up n + 1
+__device__ __forceinline__ void batch_finish_swiglu(const vila_gemv_batch_params& p, const float* sc, int row0,
+                                                    int n, int m, float g, float u) {  // n even: gate n, up n + 1
+  const __nv_bfloat16* bias = static_cast<const __nv_bfloat16*>(p.bias);
   if constexpr (kFp8) {
     g *= sc[n - row0];
     u *= sc[n + 1 - row0];
   }
-  if (p.bias) {
-    g += __bfloat162float(p.bias[n]);
-    u += __bfloat162float(p.bias[n + 1]);
+  if (bias) {
+    g += __bfloat162float(bias[n]);
+    u += __bfloat162float(bias[n + 1]);
   }
   g = bf16_round(g);
   u = bf16_round(u);
-  p.y[m * p.ldy + (n >> 1)] = __float2bfloat16(bf16_round(silu_f(g)) * u);
+  static_cast<__nv_bfloat16*>(p.y)[m * p.ldy + (n >> 1)] = __float2bfloat16(bf16_round(silu_f(g)) * u);
 }
 
 template <bool kFp8, int kNT>
 __global__ void __launch_bounds__(kThreads, 1)
-gemv_batch_kernel(GemvBatchArgs p, const void* __restrict__ w_scale, const uint8_t* __restrict__ w_zero,
+gemv_batch_kernel(vila_gemv_batch_params p, const void* __restrict__ w_scale, const uint8_t* __restrict__ w_zero,
                   BatchLayout L) {
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t* xs = smem + L.x_off;                                             // [16][x_pitch]
@@ -789,7 +792,8 @@ gemv_batch_kernel(GemvBatchArgs p, const void* __restrict__ w_scale, const uint8
   if (warp == 0) {
     if (lane == 0) mbar_arrive_expect_tx(x_bar, p.M * x_bytes);
     __syncwarp();
-    if (lane < p.M) bulk_g2s(xs + lane * L.x_pitch, p.x + lane * p.ldx + k0, x_bytes, x_bar);
+    if (lane < p.M)
+      bulk_g2s(xs + lane * L.x_pitch, static_cast<const __nv_bfloat16*>(p.x) + lane * p.ldx + k0, x_bytes, x_bar);
   }
   for (int i = threadIdx.x; i < (8 * kNT - p.M) * (L.x_pitch >> 4); i += kThreads)
     reinterpret_cast<uint4*>(xs + p.M * L.x_pitch)[i] = make_uint4(0, 0, 0, 0);
@@ -1028,7 +1032,7 @@ int batch_partition(int N, int K, bool fp8, BatchLayout& L) {
 }
 
 template <bool kFp8, int kNT>
-int gemv_batch_launch(const GemvBatchArgs& p, const void* w_scale, const uint8_t* w_zero, const BatchLayout& L,
+int gemv_batch_launch(const vila_gemv_batch_params& p, const void* w_scale, const uint8_t* w_zero, const BatchLayout& L,
                       cudaStream_t stream) {
   if (batch_set_smem_attr<kFp8, kNT>() != 0) return 2;
   const int tiles = (p.N + kW4TileRows - 1) / kW4TileRows;
@@ -1038,7 +1042,8 @@ int gemv_batch_launch(const GemvBatchArgs& p, const void* w_scale, const uint8_t
   return 0;
 }
 
-int gemv_batch(const GemvBatchArgs& p, const void* w_scale, const uint8_t* w_zero, bool fp8, cudaStream_t stream) {
+int gemv_batch(const vila_gemv_batch_params& p, const void* w_scale, const uint8_t* w_zero, bool fp8,
+               cudaStream_t stream) {
   const char* name = fp8 ? "gemv_batch_fp8" : "gemv_batch_w4a16";
   const int unit = fp8 ? 16 : kW4Group;
   VB_CHECK(p.M >= 1 && p.M <= kBatchMaxRows, "%s: M=%d outside 1..%d", name, p.M, kBatchMaxRows);
@@ -1102,10 +1107,10 @@ int gemv_tma_w4a16(const GemvParams& p, const __nv_bfloat16* w_gscale, const uin
 }
 
 // batched forms: this kernel or an error, never a fallback
-int gemv_batch_fp8(const GemvBatchArgs& p, const float* w_scale, cudaStream_t stream) {
+int gemv_batch_fp8(const vila_gemv_batch_params& p, const float* w_scale, cudaStream_t stream) {
   return gemv_batch(p, w_scale, nullptr, true, stream);
 }
-int gemv_batch_w4a16(const GemvBatchArgs& p, const __nv_bfloat16* w_gscale, const uint8_t* w_zero,
+int gemv_batch_w4a16(const vila_gemv_batch_params& p, const __nv_bfloat16* w_gscale, const uint8_t* w_zero,
                      cudaStream_t stream) {
   return gemv_batch(p, w_gscale, w_zero, false, stream);
 }

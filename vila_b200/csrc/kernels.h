@@ -1,9 +1,12 @@
 // Internal (C++) launcher declarations shared between the .cu translation units.
-// The public surface is the C-ABI in include/vila_b200.h (implemented in api.cu).
+// The public surface is the C-ABI in include/vila_b200.h (implemented in api.cu); launchers that take a
+// parameter struct take that header's struct and cast its untyped pointers where they use them.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "../../include/vila_b200.h"
 
 namespace vb {
 
@@ -44,31 +47,13 @@ int gemm_bf16_cfg(int block_n, const __nv_bfloat16* A, int lda, const __nv_bfloa
                   cudaStream_t stream);
 
 // ---- attention (prefill / ViT) -----------------------------------------------------------------
-struct FmhaParams {
-  const __nv_bfloat16* q;  // [B*Sq, Hq, D] view: element (t, h, d) at q + t*q_tok_stride + h*q_head_stride + d
-  int64_t q_tok_stride, q_head_stride;
-  // K/V are addressed as pages of 128 tokens: page p, token r, head h at
-  //   k + p*kv_page_stride + r*kv_tok_stride + h*kv_head_stride
-  const __nv_bfloat16* k;
-  const __nv_bfloat16* v;
-  int64_t kv_page_stride, kv_tok_stride, kv_head_stride;
-  int64_t kv_num_pages;        // extent of the page dimension (TMA bound)
-  const int32_t* page_table;   // [B, max_pages_per_seq] or nullptr (then page = b*pages_per_seq + j)
-  int page_table_stride;
-  __nv_bfloat16* o;            // [B*Sq, Hq, D] same addressing scheme as q (o_tok_stride, o_head_stride)
-  int64_t o_tok_stride, o_head_stride;
-  int B, Sq, Sk, Hq, Hkv;
-  int D;            // real head dim (72 or 128); padded internally by TMA zero fill
-  int causal;       // 1: kv <= q + (Sk - Sq)
-  float scale;      // softmax scale (1/sqrt(D))
-};
-int fmha_prefill(const FmhaParams& p, cudaStream_t stream);
+int fmha_prefill(const vila_fmha_params& p, cudaStream_t stream);
 // variant: 0 default, 1 / 2 the wgmma kernel, 3 / 4 with every 4th / 2nd exp2 on the FMA pipe
-int fmha_prefill_cfg(int variant, const FmhaParams& p, cudaStream_t stream);
+int fmha_prefill_cfg(int variant, const vila_fmha_params& p, cudaStream_t stream);
 // split-KV mode of the attention kernel for decode at long context (see fmha_wgmma.cu)
 // counters != nullptr ([Hq] ints, zero-initialised once): the last split CTA of a head combines into p.o
 // batch > 0: that many sequences in one launch (per-sequence lengths, page-table rows, work buffers)
-int fmha_decode_split(const FmhaParams& p, const int32_t* n_tok_minus_1, int split_tokens,
+int fmha_decode_split(const vila_fmha_params& p, const int32_t* n_tok_minus_1, int split_tokens,
                       float* o_partial, float* lse, int* counters, cudaStream_t stream,
                       int batch = 0, int64_t q_seq_stride = 0, int64_t o_seq_stride = 0);
 
@@ -150,19 +135,8 @@ int gemv_tma_fp8(const GemvParams& p, cudaStream_t stream);   // e4m3 weights, K
 // points [N, K / 128]; K % 128 == 0
 int gemv_tma_w4a16(const GemvParams& p, const __nv_bfloat16* w_gscale, const uint8_t* w_zero, cudaStream_t stream);
 // M <= 16 activation rows against the same quantized copies (gemv_batch_kernel): y[m] = epilogue(W x[m])
-struct GemvBatchArgs {
-  const __nv_bfloat16* x;         // [M, ldx]
-  int64_t ldx;
-  const void* w;                  // e4m3 [N, K], or the packed 4-bit codes
-  const __nv_bfloat16* bias;      // [N] or null
-  const __nv_bfloat16* residual;  // [M, ld_res] or null; may alias y
-  int64_t ld_res;
-  __nv_bfloat16* y;               // [M, ldy]: N (or N/2 with SwiGLU) values per row
-  int64_t ldy;
-  int M, N, K, flags;             // flags: bit0 SwiGLU, bit1 static weights
-};
-int gemv_batch_fp8(const GemvBatchArgs& p, const float* w_scale, cudaStream_t stream);
-int gemv_batch_w4a16(const GemvBatchArgs& p, const __nv_bfloat16* w_gscale, const uint8_t* w_zero,
+int gemv_batch_fp8(const vila_gemv_batch_params& p, const float* w_scale, cudaStream_t stream);
+int gemv_batch_w4a16(const vila_gemv_batch_params& p, const __nv_bfloat16* w_gscale, const uint8_t* w_zero,
                      cudaStream_t stream);
 // out: {cluster size, CTAs, tiles per cluster, k-parts per slice, max active clusters, dynamic smem bytes}
 int gemv_batch_partition(int N, int K, int fp8, int32_t* out);
@@ -171,45 +145,17 @@ int argmax_finalize(unsigned long long* key, int32_t* token_out, int32_t* token_
                     int32_t* step_counter, int32_t* position, const __nv_bfloat16* embed_table,
                     __nv_bfloat16* x_next, int hidden, cudaStream_t stream);
 
-struct DecodeAttnParams {
-  __nv_bfloat16* qkv;          // [ (Hq+2Hkv)*D ] pre-RoPE, current token
-  const int32_t* position;     // device scalar: position id of the current token (== cache length)
-  __nv_bfloat16* k_pool;       // this layer's K pages [P,128,Hkv,D]
-  __nv_bfloat16* v_pool;
-  const int32_t* page_table;   // [max_pages]
-  __nv_bfloat16* out;          // [Hq*D]
-  float* ws;                   // split-KV workspace
-  int32_t* counters;           // [Hkv] zero-initialised arrival counters
-  const float* inv_freq;       // [D/2] fp32 (HF rotary inv_freq, computed on the host like HF does)
-  int Hq, Hkv, D, num_splits;
-  float scale;
-};
-int decode_attention(const DecodeAttnParams& p, cudaStream_t stream);
+int decode_attention(const vila_decode_attn_params& p, cudaStream_t stream);
 // batch of sequences over ONE shared paged pool (continuous batching): sequence b uses qkv + b*qkv_stride,
 // out + b*out_stride, position[b] (< 0: idle slot) and page_table + b*pt_stride (max_pages valid entries,
 // <= 32 = 4096 tokens); one CTA per (query head, sequence)
-int decode_attention_batch(const DecodeAttnParams& p, int batch, int qkv_stride, int out_stride,
+int decode_attention_batch(const vila_decode_attn_params& p, int batch, int qkv_stride, int out_stride,
                            int pt_stride, int max_pages, cudaStream_t stream);
-struct DecodeAttnSplitParams {
-  __nv_bfloat16* qkv;          // [(Hq+2Hkv)*D] pre-RoPE, current token (q / k rotated in place)
-  const int32_t* position;     // device scalar: position id of the current token == tokens cached so far
-  __nv_bfloat16* k_pool;       // this layer's K pages [P,128,Hkv,D]
-  __nv_bfloat16* v_pool;
-  const int32_t* page_table;
-  int64_t kv_num_pages;
-  __nv_bfloat16* out;          // [Hq*D]
-  float* o_partial;            // [num_splits, Hq, D] fp32
-  float* lse;                  // [num_splits, Hq]
-  int32_t* counters;           // [Hkv] zero-initialised once (self-cleaning), or null: separate combine launch
-  const float* inv_freq;
-  int Hq, Hkv, D, num_splits, split_tokens;
-  float scale;
-};
-int decode_attention_split(const DecodeAttnSplitParams& p, cudaStream_t stream);
+int decode_attention_split(const vila_decode_attn_split_params& p, cudaStream_t stream);
 // batch of sequences over ONE shared paged pool, long contexts: sequence b uses qkv + b*qkv_stride,
 // out + b*out_stride, position[b] (< 0: idle) and page_table + b*pt_stride; o_partial / lse / counters
 // hold `batch` blocks of the single-sequence sizes; counters are required (fused combine)
-int decode_attention_split_batch(const DecodeAttnSplitParams& p, int batch, int qkv_stride, int out_stride,
+int decode_attention_split_batch(const vila_decode_attn_split_params& p, int batch, int qkv_stride, int out_stride,
                                  int pt_stride, cudaStream_t stream);
 
 // ---- opt-in e4m3 KV cache of the batched engine (kv_fp8.cu) -------------------------------------
@@ -217,119 +163,33 @@ int decode_attention_split_batch(const DecodeAttnSplitParams& p, int batch, int 
 // [L, 2, dst_pages, 128, Hkv, 128] and fp32 scales [L, 2, dst_pages, 128, Hkv] through one page-table row
 int kv_quantize_fp8(const __nv_bfloat16* src, int64_t src_tokens, uint8_t* dst, float* dst_scale, int64_t dst_pages,
                     const int32_t* page_table, int pt_len, int L, int Hkv, int D, int S, cudaStream_t stream);
-struct DecodeAttnFp8Params {
-  const __nv_bfloat16* qkv;    // [batch, qkv_stride] pre-RoPE, current token (not modified)
-  const int32_t* position;     // [batch] position of the new token == tokens cached (< 0: idle slot)
-  uint8_t* k_pool;             // this layer's e4m3 K pages [P, 128, Hkv, 128]
-  uint8_t* v_pool;
-  float* k_scale;              // [P, 128, Hkv]
-  float* v_scale;
-  const int32_t* page_table;   // [batch, pt_stride]
-  __nv_bfloat16* out;          // [batch, out_stride]
-  float* ws;                   // >= batch * Hkv * num_splits * G * (D + 2) floats
-  int32_t* counters;           // [batch * Hkv], zero before the first launch (self-cleaning)
-  const float* inv_freq;       // [D/2]
-  int Hq, Hkv, D, batch, qkv_stride, out_stride, pt_stride, num_splits, split_tokens;
-  float scale;
-};
-int decode_attention_fp8_batch(const DecodeAttnFp8Params& p, cudaStream_t stream);
+int decode_attention_fp8_batch(const vila_decode_attn_fp8_params& p, cudaStream_t stream);
 
 // ---- temperature / top-k / top-p sampling of the batched engine (sample.cu) ----------------------
-struct SampleParams {
-  const __nv_bfloat16* logits;   // [M, ld]
-  int64_t ld;                    // row stride (elements), >= V
-  const float* inv_temperature;  // [M] 1/T (0: greedy)
-  const int32_t* top_k;          // [M] 0 or >= V: off
-  const float* top_p;            // [M] 1: off
-  const int64_t* seed;           // [M]
-  const int64_t* step;           // [M] index t of the token being drawn
-  const int32_t* position;       // [M] < 0: idle row, tokens[row] untouched
-  int64_t* tokens;               // [M] out
-  int32_t* n_kept;               // [M] out (size of the kept set) or null
-  int M, V;
-};
-int sample_batch(const SampleParams& p, cudaStream_t stream);
+int sample_batch(const vila_sample_params& p, cudaStream_t stream);
 // the single-stream decoder's end of a sampled step: one row, device-scalar parameters, t = *step; then
 // token_out = token, token_hist[t] = token (if given), step + 1, position + 1 (if given), x_next = embed_table[token]
 // (if given).  Bit-identical to sample_batch with M = 1 on the same row, parameters, seed and t.
-struct SampleFinalizeParams {
-  const __nv_bfloat16* logits;   // [V]
-  const float* inv_temperature;  // device scalars, as sample_batch's per-row arrays
-  const int32_t* top_k;
-  const float* top_p;
-  const int64_t* seed;
-  int32_t* step;                 // t; incremented
-  int32_t* position;             // incremented, or null
-  int32_t* token_out;
-  int32_t* token_hist;           // or null
-  const __nv_bfloat16* embed_table;  // [*, hidden] with x_next, or both null
-  __nv_bfloat16* x_next;
-  int V, hidden;
-};
-int sample_finalize_check(const SampleFinalizeParams& p);  // the argument errors, before any device call
-int sample_finalize(const SampleFinalizeParams& p, cudaStream_t stream);
+int sample_finalize_check(const vila_sample_finalize_params& p);  // the argument errors, before any device call
+int sample_finalize(const vila_sample_finalize_params& p, cudaStream_t stream);
 // per-row log-probability of the chosen token and the n best tokens (vila_b200/logprobs.py's rule), written at
 // column min(step[row], cols - 1) of the engine's history buffers
-struct LogprobParams {
-  const __nv_bfloat16* logits;  // [M, ld]
-  int64_t ld;                   // row stride (elements), >= V
-  const int64_t* tokens;        // [M] the chosen token of each row
-  const int64_t* step;          // [M] history column
-  const int32_t* position;      // [M] < 0: idle row, nothing written
-  float* lp_hist;               // [M, cols]
-  int32_t* top_ids;             // [M, cols, n] (null when n == 0)
-  float* top_lp;                // [M, cols, n] (null when n == 0)
-  int M, V, cols, n;
-};
-int token_logprobs_check(const LogprobParams& p);  // the argument errors, before any device call
-int token_logprobs(const LogprobParams& p, cudaStream_t stream);
+int token_logprobs_check(const vila_logprobs_params& p);  // the argument errors, before any device call
+int token_logprobs(const vila_logprobs_params& p, cudaStream_t stream);
 // the same rule on the single-stream decoder's one row, spread over one CTA per 1152-entry chunk
 // (logprobs_row.cu): written at column min(*step - 1, cols - 1), *step being the decoder's advanced counter
-struct LogprobRowParams {
-  const __nv_bfloat16* logits;  // [V]
-  const int32_t* token;         // [1] the chosen token
-  const int32_t* step;          // [1] tokens produced so far, this one included
-  float* lp_hist;               // [cols]
-  int32_t* top_ids;             // [cols, n] (null when n == 0)
-  float* top_lp;                // [cols, n] (null when n == 0)
-  const int32_t* n_used;        // [1] alternatives to compute, clamped to 0..n; null: n
-  void* workspace;              // token_logprobs_row_workspace_bytes(V) bytes, 16-byte aligned
-  int64_t workspace_bytes;
-  unsigned int* counter;        // zero before the first launch; each launch leaves it zero
-  int V, cols, n;
-};
 int64_t token_logprobs_row_workspace_bytes(int V);
-int token_logprobs_row_check(const LogprobRowParams& p);  // the argument errors, before any device call
-int token_logprobs_row(const LogprobRowParams& p, cudaStream_t stream);
+int token_logprobs_row_check(const vila_logprobs_row_params& p);  // the argument errors, before any device call
+int token_logprobs_row(const vila_logprobs_row_params& p, cudaStream_t stream);
 
 // ---- presence / frequency penalties in the batched engine (penalties.cu) --------------------------------
 // out = the rows of logits with vila_b200/penalties.py's rule applied, over history columns 0..min(step, cols) - 1
-struct PenaltyParams {
-  const __nv_bfloat16* logits;  // [M, ld]
-  int64_t ld;                   // row stride (elements), >= V
-  const int64_t* history;       // [M, cols] generated ids
-  const int64_t* step;          // [M] ids generated so far (t)
-  const int32_t* position;      // [M] < 0: idle row, its output row is not written
-  const float* presence;        // [M]
-  const float* frequency;       // [M]
-  __nv_bfloat16* out;           // [M, V]
-  int M, V, cols;
-};
-int apply_penalties_check(const PenaltyParams& p);  // the argument errors, before any device call
-int apply_penalties(const PenaltyParams& p, cudaStream_t stream);
+int apply_penalties_check(const vila_penalty_params& p);  // the argument errors, before any device call
+int apply_penalties(const vila_penalty_params& p, cudaStream_t stream);
 // the same rule on the single-stream decoder's one row: its int32 history and int32 step counter, device-scalar
 // presence and frequency
-struct PenaltyRowParams {
-  const __nv_bfloat16* logits;  // [V]
-  const int32_t* history;       // [cols] generated ids
-  const int32_t* step;          // [1] ids generated before this token (t)
-  const float* presence;        // [1]
-  const float* frequency;       // [1]
-  __nv_bfloat16* out;           // [V]
-  int V, cols;
-};
-int apply_penalties_row_check(const PenaltyRowParams& p);  // the argument errors, before any device call
-int apply_penalties_row(const PenaltyRowParams& p, cudaStream_t stream);
+int apply_penalties_row_check(const vila_penalty_row_params& p);  // the argument errors, before any device call
+int apply_penalties_row(const vila_penalty_row_params& p, cudaStream_t stream);
 
 // ---- block digests for prefix caching in the batched engine (prefix_hash.cu) ----------------------------
 // out[b] = (d_0, d_1) of every full 128-row block b of x [rows, cols] bf16 (row stride ld elements); the rule is

@@ -97,8 +97,26 @@ __global__ void __launch_bounds__(256) kv_quantize_kernel(KvQuantArgs a) {
 //   C  thread (4 d = tid % 32, token group = warp): o_g[d] = o_g[d] * alpha + sum_r pb_g[r] * float(vcode[r, d])
 //      over tokens r = warp, warp + 8, ...; the 8 token groups are added in order after the last chunk.
 // K / V are read with plain L2 loads: the CTA that holds `pos` writes the new row first and reads it back.
+// vila_decode_attn_fp8_params with typed pointers, filled by launch_fa(): offsetting the C-ABI struct's void
+// pointers inside the kernel compiles to different code.  Same layout.
+struct FaArgs {
+  const __nv_bfloat16* qkv;
+  const int32_t* position;
+  uint8_t* k_pool;
+  uint8_t* v_pool;
+  float* k_scale;
+  float* v_scale;
+  const int32_t* page_table;
+  __nv_bfloat16* out;
+  float* ws;
+  int32_t* counters;
+  const float* inv_freq;
+  int Hq, Hkv, D, batch, qkv_stride, out_stride, pt_stride, num_splits, split_tokens;
+  float scale;
+};
+
 template <int G>
-__global__ void __launch_bounds__(kFaThreads, G <= 8 ? 2 : 1) decode_attn_fp8_kernel(DecodeAttnFp8Params p) {
+__global__ void __launch_bounds__(kFaThreads, G <= 8 ? 2 : 1) decode_attn_fp8_kernel(FaArgs p) {
   constexpr int D = 128;
   constexpr int GP = (G + 3) & ~3;  // pb_s row width (float4 reads)
   extern __shared__ __align__(16) float fa_smem[];
@@ -350,12 +368,16 @@ size_t fa_smem_bytes() {
 }
 
 template <int G>
-int launch_fa(const DecodeAttnFp8Params& p, cudaStream_t stream) {
+int launch_fa(const vila_decode_attn_fp8_params& p, cudaStream_t stream) {
+  const FaArgs a{static_cast<const __nv_bfloat16*>(p.qkv), p.position, static_cast<uint8_t*>(p.k_pool),
+                 static_cast<uint8_t*>(p.v_pool), p.k_scale, p.v_scale, p.page_table,
+                 static_cast<__nv_bfloat16*>(p.out), p.ws, p.counters, p.inv_freq, p.Hq, p.Hkv, p.D, p.batch,
+                 p.qkv_stride, p.out_stride, p.pt_stride, p.num_splits, p.split_tokens, p.scale};
   auto kern = decode_attn_fp8_kernel<G>;
   const size_t smem = fa_smem_bytes<G>();
   static PerDeviceOnce attr_once;
   if (attr_once.first()) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  VB_CUDA(launch_pdl(kern, dim3(p.num_splits, p.Hkv, p.batch), dim3(kFaThreads), smem, stream, p));
+  VB_CUDA(launch_pdl(kern, dim3(p.num_splits, p.Hkv, p.batch), dim3(kFaThreads), smem, stream, a));
   return 0;
 }
 
@@ -382,7 +404,7 @@ int kv_quantize_fp8(const __nv_bfloat16* src, int64_t src_tokens, uint8_t* dst, 
   return 0;
 }
 
-int decode_attention_fp8_batch(const DecodeAttnFp8Params& p, cudaStream_t stream) {
+int decode_attention_fp8_batch(const vila_decode_attn_fp8_params& p, cudaStream_t stream) {
   VB_CHECK(p.D == 128, "decode_attention_fp8_batch: head_dim must be 128 (got %d)", p.D);
   VB_CHECK(p.Hq >= 1 && p.Hkv >= 1 && p.Hq % p.Hkv == 0, "decode_attention_fp8_batch: Hq %d is not a multiple of Hkv %d",
            p.Hq, p.Hkv);

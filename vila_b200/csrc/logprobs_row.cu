@@ -234,7 +234,7 @@ int64_t token_logprobs_row_workspace_bytes(int V) {
   return chunks * (kRowMaxTop * static_cast<int64_t>(sizeof(u64)) + static_cast<int64_t>(sizeof(float2)));
 }
 
-int token_logprobs_row_check(const LogprobRowParams& p) {
+int token_logprobs_row_check(const vila_logprobs_row_params& p) {
   VB_CHECK(p.logits && p.token && p.step && p.lp_hist && p.workspace && p.counter,
            "token_logprobs_row: logits, token, step, lp_hist, workspace and counter are required");
   VB_CHECK(p.V >= 1 && p.V <= kRowMaxVocab, "token_logprobs_row: bad vocabulary size V=%d (1..%d)", p.V,
@@ -255,13 +255,13 @@ int token_logprobs_row_check(const LogprobRowParams& p) {
   return 0;
 }
 
-int token_logprobs_row(const LogprobRowParams& p, cudaStream_t stream) {
+int token_logprobs_row(const vila_logprobs_row_params& p, cudaStream_t stream) {
   if (int rc = token_logprobs_row_check(p)) return rc;
   const int chunks = (p.V + kRowChunk - 1) / kRowChunk;
   u64* keys = static_cast<u64*>(p.workspace);
-  RowArgs a{p.logits, p.token, p.step, p.lp_hist, p.top_ids, p.top_lp, p.n_used, keys,
-            reinterpret_cast<float2*>(keys + static_cast<int64_t>(chunks) * kRowMaxTop), p.counter, p.V, p.cols, p.n,
-            chunks};
+  RowArgs a{static_cast<const __nv_bfloat16*>(p.logits), p.token, p.step, p.lp_hist, p.top_ids, p.top_lp, p.n_used,
+            keys, reinterpret_cast<float2*>(keys + static_cast<int64_t>(chunks) * kRowMaxTop), p.counter, p.V, p.cols,
+            p.n, chunks};
   // at most 285 x 20 keys = 45,600 bytes: within the default dynamic shared-memory limit (sized for n, the most
   // alternatives a launch may compute)
   const size_t smem = static_cast<size_t>(chunks) * p.n * sizeof(u64);

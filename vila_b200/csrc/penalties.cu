@@ -113,7 +113,7 @@ __global__ void __launch_bounds__(kPenThreads) apply_penalties_kernel(PenaltyArg
 
 }  // namespace
 
-int apply_penalties_check(const PenaltyParams& p) {
+int apply_penalties_check(const vila_penalty_params& p) {
   VB_CHECK(p.logits && p.history && p.step && p.position && p.presence && p.frequency && p.out,
            "apply_penalties: logits, history, step, position, presence, frequency and out are required");
   VB_CHECK(p.M >= 1 && p.M <= 65535, "apply_penalties: bad row count M=%d (1..65535)", p.M);
@@ -129,15 +129,16 @@ int apply_penalties_check(const PenaltyParams& p) {
   return 0;
 }
 
-int apply_penalties(const PenaltyParams& p, cudaStream_t stream) {
+int apply_penalties(const vila_penalty_params& p, cudaStream_t stream) {
   if (int rc = apply_penalties_check(p)) return rc;
-  PenaltyArgs<int64_t> a{p.logits, p.ld, p.history, p.step, p.position, p.presence, p.frequency, p.out, p.V, p.cols};
+  PenaltyArgs<int64_t> a{static_cast<const __nv_bfloat16*>(p.logits), p.ld, p.history, p.step, p.position, p.presence,
+                         p.frequency, static_cast<__nv_bfloat16*>(p.out), p.V, p.cols};
   VB_CUDA(launch_pdl(apply_penalties_kernel<int64_t>, dim3((p.V + kPenChunk - 1) / kPenChunk, p.M), dim3(kPenThreads),
                      0, stream, a));
   return 0;
 }
 
-int apply_penalties_row_check(const PenaltyRowParams& p) {
+int apply_penalties_row_check(const vila_penalty_row_params& p) {
   VB_CHECK(p.logits && p.history && p.step && p.presence && p.frequency && p.out,
            "apply_penalties_row: logits, history, step, presence, frequency and out are required");
   VB_CHECK(p.V >= 1 && p.V <= kPenMaxVocab, "apply_penalties_row: bad vocabulary size V=%d (1..%d)", p.V,
@@ -151,9 +152,10 @@ int apply_penalties_row_check(const PenaltyRowParams& p) {
   return 0;
 }
 
-int apply_penalties_row(const PenaltyRowParams& p, cudaStream_t stream) {
+int apply_penalties_row(const vila_penalty_row_params& p, cudaStream_t stream) {
   if (int rc = apply_penalties_row_check(p)) return rc;
-  PenaltyArgs<int32_t> a{p.logits, p.V, p.history, p.step, nullptr, p.presence, p.frequency, p.out, p.V, p.cols};
+  PenaltyArgs<int32_t> a{static_cast<const __nv_bfloat16*>(p.logits), p.V, p.history, p.step, nullptr, p.presence,
+                         p.frequency, static_cast<__nv_bfloat16*>(p.out), p.V, p.cols};
   VB_CUDA(launch_pdl(apply_penalties_kernel<int32_t>, dim3((p.V + kPenChunk - 1) / kPenChunk, 1), dim3(kPenThreads), 0,
                      stream, a));
   return 0;

@@ -659,7 +659,7 @@ int slice_for(int V, int cluster) { return ((V + cluster - 1) / cluster + 3) & ~
 
 }  // namespace
 
-int sample_batch(const SampleParams& p, cudaStream_t stream) {
+int sample_batch(const vila_sample_params& p, cudaStream_t stream) {
   VB_CHECK(p.logits && p.inv_temperature && p.top_k && p.top_p && p.seed && p.step && p.position && p.tokens,
            "sample_batch: logits, the five parameter arrays, position and tokens are required");
   VB_CHECK(p.M >= 1 && p.M <= 65535, "sample_batch: bad row count M=%d (1..65535)", p.M);
@@ -673,8 +673,8 @@ int sample_batch(const SampleParams& p, cudaStream_t stream) {
                (reinterpret_cast<uintptr_t>(p.n_kept) & 3) == 0,
            "sample_batch: misaligned pointer");
   const int slice = slice_for(p.V, kSampCluster);
-  SampleArgs a{p.logits, p.ld, p.inv_temperature, p.top_k, p.top_p, p.seed, p.step, p.position, p.tokens, p.n_kept,
-               p.V, slice};
+  SampleArgs a{static_cast<const __nv_bfloat16*>(p.logits), p.ld, p.inv_temperature, p.top_k, p.top_p, p.seed, p.step,
+               p.position, p.tokens, p.n_kept, p.V, slice};
   static PerDeviceOnce attr_once;
   if (attr_once.first())
     VB_CUDA(cudaFuncSetAttribute(sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -684,7 +684,7 @@ int sample_batch(const SampleParams& p, cudaStream_t stream) {
   return 0;
 }
 
-int sample_finalize_check(const SampleFinalizeParams& p) {
+int sample_finalize_check(const vila_sample_finalize_params& p) {
   VB_CHECK(p.logits && p.inv_temperature && p.top_k && p.top_p && p.seed && p.step && p.token_out,
            "sample_finalize: logits, the four parameter scalars, step and token_out are required");
   VB_CHECK(p.V >= 1 && p.V <= kSampCluster * kSampMaxSlice, "sample_finalize: bad vocabulary size V=%d (1..%d)", p.V,
@@ -703,12 +703,12 @@ int sample_finalize_check(const SampleFinalizeParams& p) {
   return 0;
 }
 
-int sample_finalize(const SampleFinalizeParams& p, cudaStream_t stream) {
+int sample_finalize(const vila_sample_finalize_params& p, cudaStream_t stream) {
   if (int rc = sample_finalize_check(p)) return rc;
   const int slice = slice_for(p.V, kFinCluster);
-  FinalizeArgs a{p.logits, p.inv_temperature, p.top_k, p.top_p, p.seed, p.step, p.position, p.token_out,
-                 p.token_hist, reinterpret_cast<const uint4*>(p.embed_table), reinterpret_cast<uint4*>(p.x_next),
-                 p.hidden / 8, p.V, slice};
+  FinalizeArgs a{static_cast<const __nv_bfloat16*>(p.logits), p.inv_temperature, p.top_k, p.top_p, p.seed, p.step,
+                 p.position, p.token_out, p.token_hist, static_cast<const uint4*>(p.embed_table),
+                 static_cast<uint4*>(p.x_next), p.hidden / 8, p.V, slice};
   auto kern = sample_finalize_kernel<kFinCluster>;
   static PerDeviceOnce attr_once;
   if (attr_once.first())
@@ -719,7 +719,7 @@ int sample_finalize(const SampleFinalizeParams& p, cudaStream_t stream) {
   return 0;
 }
 
-int token_logprobs_check(const LogprobParams& p) {
+int token_logprobs_check(const vila_logprobs_params& p) {
   VB_CHECK(p.logits && p.tokens && p.step && p.position && p.lp_hist,
            "token_logprobs: logits, tokens, step, position and lp_hist are required");
   VB_CHECK(p.M >= 1 && p.M <= 65535, "token_logprobs: bad row count M=%d (1..65535)", p.M);
@@ -738,11 +738,11 @@ int token_logprobs_check(const LogprobParams& p) {
   return 0;
 }
 
-int token_logprobs(const LogprobParams& p, cudaStream_t stream) {
+int token_logprobs(const vila_logprobs_params& p, cudaStream_t stream) {
   if (int rc = token_logprobs_check(p)) return rc;
   const int slice = slice_for(p.V, kSampCluster);
-  LogprobArgs a{p.logits, p.ld, p.tokens, p.step, p.position, p.lp_hist, p.top_ids, p.top_lp, p.V, slice, p.cols,
-                p.n};
+  LogprobArgs a{static_cast<const __nv_bfloat16*>(p.logits), p.ld, p.tokens, p.step, p.position, p.lp_hist, p.top_ids,
+                p.top_lp, p.V, slice, p.cols, p.n};
   static PerDeviceOnce attr_once;
   if (attr_once.first())
     VB_CUDA(cudaFuncSetAttribute(token_logprobs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
