@@ -153,15 +153,15 @@ class _StandInDecoder:
     def cache_for(self, n):
         return "cache"
 
-    def start(self, last_hidden, cache, params=None):
+    def start(self, last_hidden, cache, params=None, *, logprobs=None, penalties=None):
         self.calls.append(("start", params))
         self.base = 100 if params is None or params.greedy else 200
 
     def run(self, n):
         pass
 
-    def tokens(self, n):
-        return [self.base + i for i in range(n)]
+    def read(self, n, start=0):
+        return lambda: ([self.base + i for i in range(start, n)], None)
 
 
 def _generate(llm, **kw):
@@ -222,7 +222,7 @@ def test_row_seeds_replay_and_a_config_seed_wins():
     assert torch.equal(torch.get_rng_state(), state)  # a config seed draws nothing
 
 
-def test_stream_tokens_passes_the_parameters():
+def test_stream_tokens_starts_the_decoder_with_the_parameters():
     llm = _StandInLLM()
     gc = SimpleNamespace(eos_token_id=None)
     p = SamplingParams(0.9, top_p=0.8, seed=3)

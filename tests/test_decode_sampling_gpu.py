@@ -150,7 +150,7 @@ def test_decoder_sampled_teacher_forced(cuda, kind):
     assert compared >= 2 * steps / 3
 
 
-def test_same_ids_on_every_route(cuda, monkeypatch):
+def test_same_ids_and_graphs_on_every_route(cuda, monkeypatch):
     from vila_b200 import _lib, ops
     from vila_b200.sampling import SamplingParams
     model = _model("tiny")[0]
@@ -200,10 +200,11 @@ def test_same_ids_on_every_route(cuda, monkeypatch):
             got = [t for c in llm.stream_tokens(emb, SimpleNamespace(eos_token_id=None), max_new_tokens=n,
                                                  sampling=q) for t in c]
             assert len(got) == n and got != ref
-        assert llm.decoder(n) is dec and len(dec.sampled_graphs) == 1 and len(dec.graphs) == 1
+        modes = [k[:3] for k in dec.graphs]  # one greedy and one sampled graph
+        assert llm.decoder(n) is dec and sorted(modes) == [(False, False, False), (True, False, False)]
         long_emb = _prompt(llm, 700, seed=700)
         list(llm.stream_tokens(long_emb, SimpleNamespace(eos_token_id=None), max_new_tokens=n, sampling=p))
-        assert len(dec.sampled_graphs) == 2
+        assert [k[:3] for k in dec.graphs].count((True, False, False)) == 2 and len(dec.graphs) == 3
         # launches per step and the finalize kernel of each mode
         names = {"sample_finalize": 0, "argmax_finalize": 0, "sample_batch": 0}
         for name in names:

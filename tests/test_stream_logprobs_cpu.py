@@ -164,42 +164,53 @@ def _decoder():
     return dec
 
 
-def test_decoder_modes_select_their_graphs_and_buffers(recorded):
+def test_decoder_modes_select_their_graph_keys_and_buffers(recorded):
     from vila_b200.sampling import SamplingParams
     dec = _decoder()
     base = dec.launches_per_step
     assert base == 5 * 2 + 2
+
+    def head(call):  # the lm_head GEMV as ops.gemv reads its arguments: (writes the row, keeps the argmax key)
+        kw = call[1]
+        return kw.get("out") is dec.logits and kw.get("write_out", True), kw.get("argmax_key") is dec.key
+
     dec.start(torch.zeros(8), dec.cache)
-    assert [c[0] for c in recorded] == ["gemv", "argmax_finalize"]
+    assert [c[0] for c in recorded] == ["gemv", "argmax_finalize"] and head(recorded[0]) == (False, True)
     assert dec.lp_hist is None and dec.pen_logits is None  # nothing allocated without the options
-    assert dec._graph_dict_key() == (dec.graphs, (dec.num_splits, dec.split_tokens))
+    plan = (dec.num_splits, dec.split_tokens)
+    assert dec._graph_key() == (False, False, False) + plan
     dec.start(torch.zeros(8), dec.cache, penalties=PenaltyParams(0.0, 0.0))  # .off: the base graph
-    assert dec._graph_dict_key()[0] is dec.graphs and dec.pen_logits is None and dec.launches_per_step == base
+    assert dec._graph_key() == (False, False, False) + plan and dec.pen_logits is None
+    assert dec.launches_per_step == base
     recorded.clear()
     dec.start(torch.zeros(8), dec.cache, logprobs=5)
     assert [c[0] for c in recorded] == ["gemv", "argmax_finalize", "token_logprobs_row"]
     assert recorded[0][1]["argmax_key"] is dec.key and recorded[0][1]["out"] is dec.logits  # row and key together
+    assert head(recorded[0]) == (True, True)
     assert dec.lp_hist.shape == (24,) and dec.top_ids.shape == (24, 20) and dec.pen_logits is None
     assert recorded[2][1]["top_ids"] is dec.top_ids and recorded[2][1]["n_used"] is dec.lp_n and dec.lp_n.item() == 5
-    graphs, key = dec._graph_dict_key()
-    assert graphs is dec.option_graphs and key[:3] == (False, False, True) and dec.launches_per_step == base + 1
+    key = dec._graph_key()
+    assert key == (False, False, True) + plan and dec.launches_per_step == base + 1
     dec.start(torch.zeros(8), dec.cache, logprobs=17)  # another n: the same graph, n is a device scalar
-    assert dec._graph_dict_key() == (graphs, key) and dec.lp_n.item() == 17
+    assert dec._graph_key() == key and dec.lp_n.item() == 17
     recorded.clear()
     dec.inv_temperature.fill_(0.5)
     dec.start(torch.zeros(8), dec.cache, penalties=PenaltyParams(0.5, -1.0), logprobs=0)
     assert [c[0] for c in recorded] == ["gemv", "apply_penalties_row", "sample_finalize", "token_logprobs_row"]
     assert float(dec.inv_temperature) == 0.0  # greedy on the penalised row
     assert dec.presence.item() == 0.5 and dec.frequency.item() == -1.0
-    assert recorded[2][0] == "sample_finalize"
-    assert dec._graph_dict_key()[1][:3] == (False, True, True) and dec.launches_per_step == base + 2
+    assert recorded[2][0] == "sample_finalize" and head(recorded[0]) == (True, False)
+    assert dec._graph_key() == (False, True, True) + plan and dec.launches_per_step == base + 2
     assert dec.lp_n.item() == 0
     recorded.clear()
     dec.start(torch.zeros(8), dec.cache, SamplingParams(0.7, seed=3), penalties=PenaltyParams(1.0, 0.0))
     assert [c[0] for c in recorded] == ["gemv", "apply_penalties_row", "sample_finalize"]
-    assert dec._graph_dict_key()[1][:3] == (True, True, False) and dec.launches_per_step == base + 1
+    assert head(recorded[0]) == (True, False)
+    assert dec._graph_key() == (True, True, False) + plan and dec.launches_per_step == base + 1
+    recorded.clear()
     dec.start(torch.zeros(8), dec.cache, SamplingParams(0.7, seed=3))
-    assert dec._graph_dict_key()[0] is dec.sampled_graphs and dec.launches_per_step == base
+    assert [c[0] for c in recorded] == ["gemv", "sample_finalize"] and head(recorded[0]) == (True, False)
+    assert dec._graph_key() == (True, False, False) + plan and dec.launches_per_step == base
     with pytest.raises(ValueError, match="started without logprobs"):
         dec.token_logprobs(3)
     with pytest.raises(ValueError, match="logprobs must be"):
@@ -227,6 +238,10 @@ def test_decoder_token_logprobs_reads_its_buffers(recorded):
     assert got == [TokenLogprob(4, -0.5, [(4, -0.5), (1, -2.0)]), TokenLogprob(5, -1.0, [(5, -1.0), (2, -3.0)]),
                    TokenLogprob(6, -1.5, [(6, -1.5), (3, -4.0)])]
     assert dec.token_logprobs(3, start=1) == got[1:] and dec.token_logprobs(3, start=3) == []
+    assert dec.read(3, start=1)() == ([5, 6], got[1:])
+    dec.start(torch.zeros(8), dec.cache)  # without logprobs: the ids alone
+    dec.hist[:3] = torch.tensor([4, 5, 6], dtype=torch.int32)
+    assert dec.read(3, start=1)() == ([5, 6], None) and dec.read(3, start=3)() == ([], None)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -246,16 +261,16 @@ class _LpDecoder:
     def run(self, n):
         self.log.append(("run", n))
 
-    def tokens(self, n):
-        return [100 + i for i in range(n)]
-
-    def read_logprobs(self, n, start=0):
+    def read(self, n, start=0):
         assert start % 4 == 0 and n - start <= 4  # only the chunk's new rows are asked for
-        def entries():
-            self.log.append(("wait", start))
-            return [TokenLogprob(100 + i, -i / 8, [(100 + i, -i / 8)]) for i in range(start, n)]
+        lp = self.started["logprobs"] is not None
 
-        return entries
+        def wait():
+            self.log.append(("wait", start))
+            return [100 + i for i in range(start, n)], [TokenLogprob(100 + i, -i / 8, [(100 + i, -i / 8)])
+                                                        for i in range(start, n)] if lp else None
+
+        return wait
 
 
 def _stream_llm():
@@ -264,7 +279,7 @@ def _stream_llm():
                            dec=dec)
 
 
-def test_stream_tokens_chunks_and_eos_truncation():
+def test_stream_tokens_chunk_reads_and_eos_truncation():
     llm = _stream_llm()
     gc = SimpleNamespace(max_new_tokens=10, eos_token_id=[106])
     pen = PenaltyParams(0.5, 0.5)
@@ -279,10 +294,19 @@ def test_stream_tokens_chunks_and_eos_truncation():
     out = list(Qwen2ForCausalLM.stream_tokens(llm, torch.zeros(3, 8), gc_all, chunk_tokens=4, logprobs=1))
     assert [ids for ids, _ in out] == [[100, 101, 102, 103], [104, 105, 106, 107], [108, 109]]
     assert llm.dec.log == [("run", 4), ("run", 4), ("wait", 0), ("run", 2), ("wait", 4), ("wait", 8)]
+    llm.dec.log.clear()
     plain = list(Qwen2ForCausalLM.stream_tokens(llm, torch.zeros(3, 8), gc, chunk_tokens=4))
-    assert plain == [[100, 101, 102, 103], [104, 105, 106]] and llm.dec.started == {}
+    assert plain == [[100, 101, 102, 103], [104, 105, 106]] and llm.dec.started == dict(logprobs=None, penalties=None)
+    # no read-ahead without logprobs: each chunk's rows are read before the next chunk runs, none after EOS
+    assert llm.dec.log == [("run", 4), ("wait", 0), ("run", 4), ("wait", 4)]
+    llm.dec.log.clear()
     pen_only = list(Qwen2ForCausalLM.stream_tokens(llm, torch.zeros(3, 8), gc, chunk_tokens=4, penalties=pen))
     assert pen_only == plain and llm.dec.started == dict(logprobs=None, penalties=pen)
+    assert llm.dec.log == [("run", 4), ("wait", 0), ("run", 4), ("wait", 4)]
+    llm.dec.log.clear()
+    plain_all = list(Qwen2ForCausalLM.stream_tokens(llm, torch.zeros(3, 8), gc_all, chunk_tokens=4))
+    assert plain_all == [ids for ids, _ in out]
+    assert llm.dec.log == [("run", 4), ("wait", 0), ("run", 4), ("wait", 4), ("run", 2), ("wait", 8)]
     with pytest.raises(ValueError, match="logprobs must be"):
         list(Qwen2ForCausalLM.stream_tokens(llm, torch.zeros(3, 8), gc, logprobs=30))
 

@@ -327,7 +327,7 @@ def test_decoder_greedy_penalised_ids_against_the_oracle(cuda):
              "ok": True})
 
 
-def test_requests_without_options_are_unchanged(cuda):
+def test_requests_without_options_replay_their_graph(cuda):
     from vila_b200.penalties import PenaltyParams
     from vila_b200.sampling import SamplingParams
     llm = _model("tiny")[0].llm
@@ -337,18 +337,22 @@ def test_requests_without_options_are_unchanged(cuda):
     dec = llm._decoder
     base = dec.launches_per_step
     assert base == 5 * llm.config.num_hidden_layers + 2
-    assert len(dec.graphs) == 1 and not dec.sampled_graphs and not dec.option_graphs
+    plan = (dec.num_splits, dec.split_tokens)
+    assert list(dec.graphs) == [(False, False, False) + plan]
+    plain_graph = dec.graphs[(False, False, False) + plan]
     assert dec.lp_hist is None and dec.pen_logits is None  # nothing allocated for the options
     _stream(llm, emb, 10, logprobs=2, penalties=PenaltyParams(0.5, 0.5))
-    assert dec.launches_per_step == base + 2 and len(dec.option_graphs) == 1
+    assert dec.launches_per_step == base + 2 and list(dec.graphs)[1:] == [(False, True, True) + plan]
     _stream(llm, emb, 10, sampling=SamplingParams(0.7, seed=1), logprobs=2)
-    assert dec.launches_per_step == base + 1 and len(dec.option_graphs) == 2
+    assert dec.launches_per_step == base + 1 and list(dec.graphs)[2:] == [(True, False, True) + plan]
     a = _stream(llm, emb, 10, logprobs=7)  # another top count: the greedy + logprobs graph is reused
     b = _stream(llm, emb, 10, logprobs=3)
-    assert len(dec.option_graphs) == 3 and a[0] == b[0] == plain
+    assert list(dec.graphs)[3:] == [(False, False, True) + plan] and a[0] == b[0] == plain
     assert [e.top[:3] for e in a[1]] == [e.top for e in b[1]] and all(len(e.top) == 7 for e in a[1])
     again, _ = _stream(llm, emb, 10)
-    assert again == plain and dec.launches_per_step == base and len(dec.graphs) == 1 and not dec.sampled_graphs
+    # the plain request after the option requests replays the graph it replayed first: no greedy or sampled recapture
+    assert again == plain and dec.launches_per_step == base and len(dec.graphs) == 4
+    assert dec.graphs[(False, False, False) + plan] is plain_graph
 
 
 def test_llava_stream_content_end_to_end(cuda):

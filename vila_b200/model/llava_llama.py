@@ -720,12 +720,7 @@ class LlavaLlamaModel(nn.Module):
     def _generate_content_stream(self, prompt, generation_config, response_format, chunk_tokens: int = 8):
         if response_format is not None:
             raise NotImplementedError("streaming + constrained decoding: use stream=False")
-        with torch.inference_mode():
-            input_ids, media, media_config = self._prepare_content(prompt)
-            gc = generation_config or self.default_generation_config
-            inputs_embeds, _, _ = self._embed(input_ids, media, media_config, None, None)
-        sampling = sampling_for_generate(gc, 1)[0] if getattr(gc, "do_sample", False) else None
-        for ids in self.llm.stream_tokens(inputs_embeds[0], gc, chunk_tokens=chunk_tokens, sampling=sampling):
+        for ids, _ in self.stream_content(prompt, generation_config, chunk_tokens=chunk_tokens):
             text = self.tokenizer.decode(ids, skip_special_tokens=True)
             if text:
                 yield text

@@ -15,6 +15,7 @@ Arithmetic spec: in-tree copy llava/eval/vision_niah_vila/zigzag_ring_attn/model
 """
 from __future__ import annotations
 
+from collections import deque
 from types import SimpleNamespace
 from typing import List, Optional, Sequence
 
@@ -257,29 +258,28 @@ def dequantize_w4_groups(packed: torch.Tensor, s: torch.Tensor, z: torch.Tensor)
     return ((q - z.float()[..., None]) * s.float()[..., None]).view(N, K)
 
 
-def _stream_logprobs(dec, max_new: int, chunk_tokens: int, eos_ids):
-    """stream_tokens' loop with logprobs, one chunk ahead: chunk k + 1 is enqueued before the host waits for chunk
-    k's rows (only those, in one copy) and builds its entries, so the device does not idle while the host works.
-    A chunk decoded past EOS is dropped."""
-    done, n = 0, min(chunk_tokens, max_new)
-    dec.run(n)
-    pending = dec.read_logprobs(n, start=0)
-    while True:
-        nxt = min(chunk_tokens, max_new - done - n)
-        if nxt > 0:
-            dec.run(nxt)
-        entries = pending()
-        if nxt > 0:
-            pending = dec.read_logprobs(done + n + nxt, start=done + n)
-        ids = [e.token for e in entries]
-        hit = [i for i, t in enumerate(ids) if t in eos_ids]
-        if hit:
-            yield ids[:hit[0] + 1], entries[:hit[0] + 1]
+def _decode_chunks(dec, max_new: int, chunk_tokens: int, eos_ids, ahead: bool):
+    """Run a started GraphDecoder for up to max_new tokens in chunks of chunk_tokens and yield (ids, entries or None)
+    per chunk, cut after the first EOS id.  Each chunk's rows alone are read back, in one copy (GraphDecoder.read).
+    ahead: chunk k + 1 is enqueued before the host waits for chunk k, so the device decodes while the host builds the
+    logprob entries; a chunk decoded past EOS is then dropped.  Without it each chunk is read before the next runs, so
+    nothing is decoded past the chunk that holds EOS."""
+    reads = deque()
+    done = 0
+    while done < max_new or reads:
+        if done < max_new:
+            n = min(chunk_tokens, max_new - done)
+            dec.run(n)
+            reads.append(dec.read(done + n, start=done))
+            done += n
+            if ahead and len(reads) == 1 and done < max_new:
+                continue
+        ids, entries = reads.popleft()()
+        hit = next((i + 1 for i, t in enumerate(ids) if t in eos_ids), None)
+        if hit is not None:
+            yield ids[:hit], None if entries is None else entries[:hit]
             return
         yield ids, entries
-        if nxt <= 0:
-            return
-        done, n = done + n, nxt
 
 
 class Qwen2ForCausalLM(nn.Module):
@@ -638,18 +638,9 @@ class Qwen2ForCausalLM(nn.Module):
             cache = dec.cache_for(S + max_new)
             hid = self.prefill_hidden_graphed(emb, cache)
             dec.start(hid[-1], cache, sampling)
-        done = 0
-        ids: List[int] = []
-        while done < max_new:
-            n = min(check_every, max_new - done)
-            dec.run(n)
-            done += n
-            if eos_ids:
-                ids = dec.tokens(done)
-                hit = [i for i, t in enumerate(ids) if t in eos_ids]
-                if hit:
-                    return ids[:hit[0] + 1]
-        return dec.tokens(done)
+        # without EOS ids nothing is read until the end: one chunk of max_new
+        chunks = _decode_chunks(dec, max_new, check_every if eos_ids else max_new, eos_ids, ahead=False)
+        return [t for ids, _ in chunks for t in ids]
 
     def stream_greedy(self, emb: torch.Tensor, generation_config=None, chunk_tokens: int = 8,
                       max_new_tokens: Optional[int] = None):
@@ -683,25 +674,11 @@ class Qwen2ForCausalLM(nn.Module):
             dec = self.decoder(max_new)
             cache = dec.cache_for(S + max_new)
             hid = self.prefill_hidden_graphed(emb, cache)
-            if logprobs is None and penalties is None:
-                dec.start(hid[-1], cache, sampling)
-            else:
-                dec.start(hid[-1], cache, sampling, logprobs=logprobs, penalties=penalties)
-            if logprobs is not None:
-                yield from _stream_logprobs(dec, max_new, chunk_tokens, eos_ids)
-                return
-            done = 0
-            while done < max_new:
-                n = min(chunk_tokens, max_new - done)
-                dec.run(n)
-                ids = dec.tokens(done + n)[done:]
-                done += n
-                hit = [i for i, t in enumerate(ids) if t in eos_ids]
-                if hit:
-                    yield ids[:hit[0] + 1]
-                    return
-                yield ids
-
+            dec.start(hid[-1], cache, sampling, logprobs=logprobs, penalties=penalties)
+            # read-ahead only with logprobs: it overlaps building their entries with decoding, and would otherwise
+            # only add a chunk of decoding past EOS
+            for ids, entries in _decode_chunks(dec, max_new, chunk_tokens, eos_ids, ahead=logprobs is not None):
+                yield ids if logprobs is None else (ids, entries)
 
     def _generate_eager(self, emb, max_new, eos_ids, sample, processors, temperature, top_p, top_k):
         """Non-graph path: logits come from the same kernels; the token choice (sampling /
@@ -747,16 +724,16 @@ class GraphDecoder:
     graph and replayed without host synchronisation (the reference runs ~400 launches and one D2H
     stopping-criteria sync per token, SURVEY §3.1 HOT LOOP C).
 
-    Sampled decoding (start(..., params) with non-greedy SamplingParams) runs a second graph per
-    configuration, with the same number of launches: lm_head writes the bf16 logits row and
-    vila_sample_finalize draws the token from it (the rule of vila_b200/sampling.py, t = the step counter) in
-    place of argmax_finalize.  Temperature, top-k, top-p and seed are device scalars that start() writes, so a
-    new request's parameters replay the same graph.
+    `graphs` holds one step graph per mode and attention plan, captured on first use and keyed by (sampled,
+    penalised, logprobs on, num_splits, split_tokens) (_graph_key).  A request's parameters are device scalars that
+    start() writes, so every request of one mode and plan replays the same graph.
 
-    Logprobs and presence / frequency penalties (start(..., logprobs=n, penalties=PenaltyParams)) run further step
-    graphs, captured on first use and keyed by (sampled, penalised, logprobs on) as well as the attention plan.  The
-    number of alternatives n is a device scalar that start() writes (the history rows hold 20), so one graph serves
-    every n:
+    Sampled decoding (start(..., params) with non-greedy SamplingParams) has the same number of launches as greedy:
+    lm_head writes the bf16 logits row and vila_sample_finalize draws the token from it (the rule of
+    vila_b200/sampling.py, t = the step counter) in place of argmax_finalize.
+
+    Logprobs and presence / frequency penalties (start(..., logprobs=n, penalties=PenaltyParams)) add a launch each.
+    The number of alternatives n is a device scalar (the history rows hold 20), so one graph serves every n:
       greedy + logprobs   lm_head writes the bf16 row and keeps its fused argmax key; argmax_finalize; then
                           vila_token_logprobs_row on the row (the ids are the greedy graph's)
       sampled + logprobs  the sampled step, then vila_token_logprobs_row on the row
@@ -764,7 +741,7 @@ class GraphDecoder:
                           int32 history, vila_sample_finalize chooses from pen_logits (at inv_T = 0 the first index of
                           the max: the greedy rule), then vila_token_logprobs_row on the raw row when logprobs are on
     The rules are those of vila_b200/logprobs.py and vila_b200/penalties.py; token_logprobs() reads the entries back.
-    Their buffers are allocated on first use; a request with neither option runs exactly the graphs above.
+    Their buffers are allocated on first use; a request with neither option runs the greedy or sampled graph.
 
     The decoder streams the weights of the LLM's decode-weight mode at construction
     (Qwen2ForCausalLM.set_decode_weights): in "fp8" mode every GEMV of start() and of each step, lm_head
@@ -810,28 +787,14 @@ class GraphDecoder:
         self.lse = torch.zeros(self.MAX_SPLITS * Hq, device=dev, dtype=torch.float32)
         self.split_tokens = 0  # > 0: the long-context path is active for the current cache
         self.cache: Optional[PagedKVCache] = None
-        self.graphs = {}  # (num_splits, split_tokens) -> captured CUDA graph of one decode step (for self.cache)
-        self.sampled_graphs = {}  # the same for sampled steps
-        # (sampled, penalised, logprobs on, num_splits, split_tokens) -> step graph with logprobs or penalties
-        self.option_graphs = {}
+        self.graphs = {}  # _graph_key() -> captured CUDA graph of one decode step (for self.cache)
         # logprobs / penalties buffers, allocated on first use (_ensure_logprobs / _ensure_penalties)
         self.lp_hist = self.top_ids = self.top_lp = self.lp_n = self.lp_ws = self.lp_counter = None
         self.pen_logits = self.presence = self.frequency = None
 
-    @property
-    def _options(self) -> bool:
-        return self.penalised or self.top_n is not None
-
-    def _graph_dict_key(self):
-        plan = (self.num_splits, self.split_tokens)
-        if self._options:
-            return self.option_graphs, (self.sampled, self.penalised, self.top_n is not None) + plan
-        return (self.sampled_graphs if self.sampled else self.graphs), plan
-
-    @property
-    def graph(self):
-        graphs, key = self._graph_dict_key()
-        return graphs.get(key)
+    def _graph_key(self):
+        """what a step graph depends on besides the cache: the current request's mode and the attention plan"""
+        return self.sampled, self.penalised, self.top_n is not None, self.num_splits, self.split_tokens
 
     @property
     def launches_per_step(self) -> int:
@@ -888,8 +851,6 @@ class GraphDecoder:
             self.cache = self.llm.new_cache(n_tok, order)
             self._order_key = order_key
             self.graphs = {}
-            self.sampled_graphs = {}
-            self.option_graphs = {}
         self.cache.length = 0
         self.num_splits, self.split_tokens = self.pick_splits(self.cache.max_tokens if tokens > self.LONG_CTX
                                                               else tokens)
@@ -916,16 +877,13 @@ class GraphDecoder:
                                          layer.mlp.down_proj.weight))
 
     def _lm_head(self):
-        cfg = self.llm.config
-        if self.sampled or self.penalised:
-            ops.gemv(self.x, norm_w=self.llm.model.norm.weight, norm_eps=cfg.rms_norm_eps, out=self.logits,
-                     static_w=True, **self._weights(None))
-        elif self.top_n is not None:  # greedy + logprobs: the row and the fused argmax key from the same values
-            ops.gemv(self.x, norm_w=self.llm.model.norm.weight, norm_eps=cfg.rms_norm_eps, out=self.logits,
-                     argmax_key=self.key, static_w=True, **self._weights(None))
-        else:
-            ops.gemv(self.x, norm_w=self.llm.model.norm.weight, norm_eps=cfg.rms_norm_eps, argmax_key=self.key,
-                     write_out=False, static_w=True, **self._weights(None))
+        """the bf16 row when a kernel after lm_head reads it, the fused argmax key when argmax_finalize chooses (greedy
+        + logprobs: both, from the same values)"""
+        chooses_from_row = self.sampled or self.penalised
+        row = chooses_from_row or self.top_n is not None
+        ops.gemv(self.x, norm_w=self.llm.model.norm.weight, norm_eps=self.llm.config.rms_norm_eps,
+                 out=self.logits if row else None, write_out=row,
+                 argmax_key=None if chooses_from_row else self.key, static_w=True, **self._weights(None))
 
     def _finalize(self):
         """the token (arg-max, or the draw in sampled mode; from the penalised row with penalties) -> history, step++,
@@ -1017,14 +975,14 @@ class GraphDecoder:
             self._started = 2
         if n <= 0:
             return
-        graphs, key = self._graph_dict_key()
-        g = graphs.get(key)
+        key = self._graph_key()
+        g = self.graphs.get(key)
         if g is None:
             # warm-up launch outside capture is not allowed to change state: capture directly
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
                 self._step()
-            graphs[key] = g
+            self.graphs[key] = g
         for _ in range(n):
             g.replay()
         self.cache.length += n
@@ -1036,18 +994,22 @@ class GraphDecoder:
         """tokens start .. n_tokens - 1 of the current request with their logprobs and top alternatives (start() with
         logprobs): only those rows are copied to the host, so a stream that reads each chunk's new tokens does work
         in proportion to them.  ValueError without logprobs."""
-        return self.read_logprobs(n_tokens, start)()
-
-    def read_logprobs(self, n_tokens: int, start: int = 0):
-        """token_logprobs in two halves: enqueue the copy of rows start .. n_tokens - 1 to the host now, and return a
-        function that waits for that copy alone and builds the entries.  Steps enqueued in between run on the device
-        while the host waits and builds (the streaming loop reads chunk k while chunk k + 1 decodes)."""
         if self.top_n is None:
             raise ValueError("GraphDecoder.token_logprobs: the current request was started without logprobs")
-        n, cols = self.top_n, self.lp_hist.numel()
-        a, b = max(0, start), min(n_tokens, cols)
+        return self.read(n_tokens, start)()[1]
+
+    def read(self, n_tokens: int, start: int = 0):
+        """Tokens start .. n_tokens - 1 of the current request as a function returning (ids, entries): entries are their
+        TokenLogprobs with logprobs, else None.  Only their rows are copied to the host, in one copy.  With logprobs
+        that copy is enqueued now and the function waits for it alone, so steps enqueued in between decode while the
+        host builds the entries (_decode_chunks reads chunk k while chunk k + 1 runs).  Ids alone, which no caller
+        reads ahead, are copied by the function with a plain blocking copy."""
+        n = self.top_n
+        a, b = max(0, start), min(n_tokens, self.hist.numel())
+        if n is None:
+            return lambda: (self.hist[a:b].tolist(), None)
         if a >= b:
-            return lambda: []
+            return lambda: ([], [])
         # one device-to-host copy: [id, logprob bits, top ids..., top logprob bits...] per token
         rows = torch.cat([self.hist[a:b, None], self.lp_hist[a:b, None].view(torch.int32), self.top_ids[a:b, :n],
                           self.top_lp[a:b, :n].view(torch.int32)], dim=1)
@@ -1059,14 +1021,14 @@ class GraphDecoder:
             done.record()
             rows = host
 
-        def entries() -> List[TokenLogprob]:
+        def wait():
             if done is not None:
                 done.synchronize()
             ids = rows[:, 0].tolist()
             lps = rows[:, 1].view(torch.float32).tolist()
             top_i = rows[:, 2:2 + n].tolist()
             top_v = rows[:, 2 + n:].contiguous().view(torch.float32).tolist()
-            return [TokenLogprob(t, lp, list(zip(ti, tv))) for t, lp, ti, tv in zip(ids, lps, top_i, top_v)]
+            return ids, [TokenLogprob(t, lp, list(zip(ti, tv))) for t, lp, ti, tv in zip(ids, lps, top_i, top_v)]
 
-        return entries
+        return wait
 
