@@ -523,6 +523,20 @@ typedef struct vila_penalty_row_params {
 int vila_apply_penalties_row(const vila_penalty_row_params* p, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * vila_apply_token_bitmask_row — grammar-constrained decoding: the single-stream graph decoder's one row of bf16
+ * logits [V], masked by a grammar matcher's token bitmask, written to out [V].  Replaces xgrammar's HF
+ * LogitsProcessor (xgr.contrib.hf.LogitsProcessor -> apply_token_bitmask_inplace), which the reference builds from
+ * `response_format` (llava_arch.py:802-821) and runs on the host-driven eager decode loop.  The rule
+ * (vila_b200/grammar.py states it in numpy), for token j with bitmask int32 [ceil(V / 32)] in xgrammar's layout:
+ *   bit j % 32 of bitmask[j / 32] set:  out_j = logits_j, bit for bit
+ *   otherwise:                          out_j = -inf (0xFF80)
+ * Bits at or above V are ignored.  logits == out (in place) is allowed; otherwise the rows must not overlap.  Any
+ * V >= 1, rows of any 2-byte alignment, bitmask 4-byte aligned; the argument errors are reported before any device
+ * call.  The arguments are passed directly, as vila_prefix_block_hash's are.  One thread per 8 entries, PDL.
+ * ------------------------------------------------------------------------------------------- */
+int vila_apply_token_bitmask_row(const void* logits, const int32_t* bitmask, void* out, int32_t V, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * vila_prefix_block_hash — a 128-bit digest of every full 128-row block of a bf16 matrix x [rows, cols] (row
  * stride ld elements), for prefix caching in the continuous-batching engine: out [rows / 128][2] (uint64).  The
  * reference has no counterpart: it prefills every request in full (serving/server.py:65-73, llava_arch.py:823-833).

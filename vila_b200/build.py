@@ -32,6 +32,7 @@ SOURCES = [
     "prefix_hash.cu",
     "penalties.cu",
     "logprobs_row.cu",
+    "token_bitmask.cu",
 ]
 HEADERS = ["common.cuh", "wgmma.cuh", "kernels.h", "../../include/vila_b200.h"]
 

@@ -351,6 +351,13 @@ int vila_apply_penalties_row(const vila_penalty_row_params* p, void* stream) {
   return vb::apply_penalties_row(*p, st(stream));
 }
 
+// xgrammar's HF LogitsProcessor (llava_arch.py:802-821) for the single-stream graph decoder's one row
+int vila_apply_token_bitmask_row(const void* logits, const int32_t* bitmask, void* out, int32_t V, void* stream) {
+  if (int rc = vb::apply_token_bitmask_row_check(logits, bitmask, out, V)) return rc;
+  VB_REQUIRE_DEVICE();
+  return vb::apply_token_bitmask_row(logits, bitmask, out, V, st(stream));
+}
+
 // the reference prefills every request in full (serving/server.py:65-73, llava_arch.py:823-833): no seam
 int vila_prefix_block_hash(const void* x, int64_t ld, int64_t rows, int64_t cols, uint64_t key0, uint64_t key1,
                            uint64_t* out, void* stream) {

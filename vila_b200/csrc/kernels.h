@@ -191,6 +191,12 @@ int apply_penalties(const vila_penalty_params& p, cudaStream_t stream);
 int apply_penalties_row_check(const vila_penalty_row_params& p);  // the argument errors, before any device call
 int apply_penalties_row(const vila_penalty_row_params& p, cudaStream_t stream);
 
+// ---- grammar-constrained decoding in the single-stream decoder (token_bitmask.cu) -------------------------------
+// out = in where the token bitmask allows the id, -inf elsewhere (vila_b200/grammar.py's rule); in == out allowed
+// the argument errors, before any device call
+int apply_token_bitmask_row_check(const void* logits, const int32_t* bitmask, const void* out, int V);
+int apply_token_bitmask_row(const void* logits, const int32_t* bitmask, void* out, int V, cudaStream_t stream);
+
 // ---- block digests for prefix caching in the batched engine (prefix_hash.cu) ----------------------------
 // out[b] = (d_0, d_1) of every full 128-row block b of x [rows, cols] bf16 (row stride ld elements); the rule is
 // vila_b200/prefix_cache.py's.  The check reports the argument errors before any device call.

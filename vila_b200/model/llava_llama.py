@@ -653,19 +653,32 @@ class LlavaLlamaModel(nn.Module):
             gc.eos_token_id = self.tokenizer.stop_token_ids
         return gc
 
-    def get_xgr_logits_processor(self, response_format) -> List[Any]:
-        """llava_arch.py:802-821: compile `response_format` (type json_object | json_schema) with
-        xgrammar into an HF-style logits processor (needs a HF tokenizer; host-side plumbing that the
-        eager decode loop calls once per token)."""
+    def compile_response_format(self, response_format):
+        """llava_arch.py:802-821: compile `response_format` with xgrammar: type json_schema -> its schema (indent 2),
+        any other type -> the builtin JSON grammar.  self.grammar_compiler is built from the HF tokenizer on first use
+        (a caller may install one built from an explicit vocabulary first) and caches what it compiles.  A schema
+        xgrammar cannot compile raises."""
         import xgrammar as xgr
         if getattr(self, "grammar_compiler", None) is None:
             self.grammar_compiler = xgr.GrammarCompiler(
                 xgr.TokenizerInfo.from_huggingface(self.tokenizer, vocab_size=self.vocab_size))
         if response_format.type == "json_schema":
-            compiled = self.grammar_compiler.compile_json_schema(response_format.json_schema.schema_, indent=2)
-        else:
-            compiled = self.grammar_compiler.compile_builtin_json_grammar()
-        return [xgr.contrib.hf.LogitsProcessor(compiled)]
+            return self.grammar_compiler.compile_json_schema(response_format.json_schema.schema_, indent=2)
+        return self.grammar_compiler.compile_builtin_json_grammar()
+
+    def get_xgr_logits_processor(self, response_format) -> List[Any]:
+        """llava_arch.py:802-821: `response_format` as an HF-style logits processor, for the eager decode loop
+        (Qwen2ForCausalLM.generate(logits_processor=...)), which calls it once per token on the host."""
+        import xgrammar as xgr
+        return [xgr.contrib.hf.LogitsProcessor(self.compile_response_format(response_format))]
+
+    def grammar_matcher(self, response_format, stop_token_ids):
+        """`response_format` as a fresh xgrammar GrammarMatcher for the graph decoder (GraphDecoder.start(grammar=)),
+        whose stop tokens are the decode's EOS ids: the grammar allows them once the document is complete, and
+        accepting one terminates the matcher."""
+        import xgrammar as xgr
+        return xgr.GrammarMatcher(self.compile_response_format(response_format),
+                                  override_stop_tokens=list(stop_token_ids))
 
     def _prepare_content(self, prompt: Union[str, List]):
         """prompt -> (input_ids [1,T], media, media_config): the host half of generate_content
@@ -695,56 +708,77 @@ class LlavaLlamaModel(nn.Module):
                          response_format=None, stream: bool = False):
         """llava_arch.py:835-948: prompt = str or list of (str | image tensor [3,H,W] | PIL image).
         Image tensors must already be normalised; PIL images go through `media.process_image`.
-        response_format: xgrammar-constrained decoding (llava_arch.py:846-849).
+        response_format: xgrammar-constrained decoding (llava_arch.py:846-849), streamed or not: the graph decoder
+        masks every row with the grammar's token bitmask on the device (stream_content).
         stream=True (serving/server.py:259-264 calls it that way): returns an iterator of text
         chunks; the decode stays on the device and is drained every few tokens.  Both forms sample on the
         device when the generation config sets do_sample (its temperature, top_k, top_p and `seed`), with the
         same ids for the same seed."""
         if stream:
             return self._generate_content_stream(prompt, generation_config, response_format)
+        if response_format:
+            gc = generation_config or self.default_generation_config
+
+            def constrained():
+                return [t for ids, _ in self.stream_content(prompt, gc, response_format=response_format,
+                                                             chunk_tokens=16) for t in ids]
+            try:
+                output_ids = constrained()
+            except ValueError:
+                if not getattr(gc, "do_sample", False):
+                    raise
+                gc.do_sample = False  # the reference's fallback: retry greedily (llava_arch.py:932-944)
+                output_ids = constrained()
+            return self.tokenizer.decode(output_ids, skip_special_tokens=True).strip()
         with torch.inference_mode():
-            processors = self.get_xgr_logits_processor(response_format) if response_format else None
             input_ids, media, media_config = self._prepare_content(prompt)
             gc = generation_config or self.default_generation_config
             try:
                 output_ids = self.generate(input_ids=input_ids, media=media, media_config=media_config,
-                                           generation_config=gc, logits_processor=processors)
+                                           generation_config=gc)
             except ValueError:
                 if not getattr(gc, "do_sample", False):
                     raise
                 gc.do_sample = False  # the reference's fallback: retry greedily (llava_arch.py:932-944)
                 output_ids = self.generate(input_ids=input_ids, media=media, media_config=media_config,
-                                           generation_config=gc, logits_processor=processors)
+                                           generation_config=gc)
             return self.tokenizer.decode(output_ids[0], skip_special_tokens=True).strip()
 
     def _generate_content_stream(self, prompt, generation_config, response_format, chunk_tokens: int = 8):
-        if response_format is not None:
-            raise NotImplementedError("streaming + constrained decoding: use stream=False")
-        for ids, _ in self.stream_content(prompt, generation_config, chunk_tokens=chunk_tokens):
+        kw = {} if response_format is None else {"response_format": response_format}
+        for ids, _ in self.stream_content(prompt, generation_config, chunk_tokens=chunk_tokens, **kw):
             text = self.tokenizer.decode(ids, skip_special_tokens=True)
             if text:
                 yield text
 
     def stream_content(self, prompt: Union[str, List], generation_config=None, *, logprobs: Optional[int] = None,
-                       penalties=None, chunk_tokens: int = 8):
+                       penalties=None, chunk_tokens: int = 8, response_format=None):
         """generate_content(stream=True) with per-token logprobs and OpenAI presence / frequency penalties, as a
         generator of (ids, entries) per chunk of up to chunk_tokens new ids (sampled on the device when the generation
         config sets do_sample, as generate_content).  entries: one vila_b200.logprobs.TokenLogprob per id with
         `logprobs` = n in 0..20 alternatives, else None.  penalties: a vila_b200.penalties.PenaltyParams, or None.  The
         last chunk ends with the EOS id when one was generated; its entry is there too.  Both options run on the
-        device in the single-stream graph decoder (Qwen2ForCausalLM.stream_tokens).  Not with sequence-parallel
-        decoding (NotImplementedError)."""
+        device in the single-stream graph decoder (Qwen2ForCausalLM.stream_tokens).  response_format: a ResponseFormat
+        (generate_content's mapping of its types, compile_response_format); every id is then one the grammar allows,
+        and the stream ends when the grammar terminates (its stop tokens are the config's EOS ids).  Not with
+        sequence-parallel decoding (NotImplementedError)."""
         from ..logprobs import check_top
         if logprobs is not None:
             check_top(logprobs)
-        if (logprobs is not None or (penalties is not None and not penalties.off)) and self._sp_runner() is not None:
-            raise NotImplementedError("stream_content: logprobs and penalties are not implemented with "
-                                      "sequence-parallel decoding")
+        if ((logprobs is not None or (penalties is not None and not penalties.off) or response_format is not None)
+                and self._sp_runner() is not None):
+            raise NotImplementedError("stream_content: logprobs, penalties and response_format are not implemented "
+                                      "with sequence-parallel decoding")
         with torch.inference_mode():
             input_ids, media, media_config = self._prepare_content(prompt)
             gc = generation_config or self.default_generation_config
             inputs_embeds, _, _ = self._embed(input_ids, media, media_config, None, None)
         sampling = sampling_for_generate(gc, 1)[0] if getattr(gc, "do_sample", False) else None
+        kw = {}
+        if response_format is not None:
+            eos = getattr(gc, "eos_token_id", None)
+            kw["grammar"] = self.grammar_matcher(response_format, [] if eos is None else
+                                                 [eos] if isinstance(eos, int) else list(eos))
         for out in self.llm.stream_tokens(inputs_embeds[0], gc, chunk_tokens=chunk_tokens, sampling=sampling,
-                                          logprobs=logprobs, penalties=penalties):
+                                          logprobs=logprobs, penalties=penalties, **kw):
             yield out if logprobs is not None else (out, None)

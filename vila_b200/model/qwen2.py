@@ -22,6 +22,7 @@ from typing import List, Optional, Sequence
 import torch
 from torch import nn
 
+from .. import grammar as grammar_rule
 from .. import ops
 from ..logprobs import MAX_TOP_LOGPROBS, TokenLogprob, check_top
 from ..penalties import PenaltyParams
@@ -263,23 +264,28 @@ def _decode_chunks(dec, max_new: int, chunk_tokens: int, eos_ids, ahead: bool):
     per chunk, cut after the first EOS id.  Each chunk's rows alone are read back, in one copy (GraphDecoder.read).
     ahead: chunk k + 1 is enqueued before the host waits for chunk k, so the device decodes while the host builds the
     logprob entries; a chunk decoded past EOS is then dropped.  Without it each chunk is read before the next runs, so
-    nothing is decoded past the chunk that holds EOS."""
+    nothing is decoded past the chunk that holds EOS.  A chunk shorter than asked for ends the stream: the decoder
+    stopped because its grammar terminated."""
     reads = deque()
     done = 0
     while done < max_new or reads:
         if done < max_new:
             n = min(chunk_tokens, max_new - done)
             dec.run(n)
-            reads.append(dec.read(done + n, start=done))
+            reads.append((n, dec.read(done + n, start=done)))
             done += n
             if ahead and len(reads) == 1 and done < max_new:
                 continue
-        ids, entries = reads.popleft()()
+        want, read = reads.popleft()
+        ids, entries = read()
         hit = next((i + 1 for i, t in enumerate(ids) if t in eos_ids), None)
         if hit is not None:
             yield ids[:hit], None if entries is None else entries[:hit]
             return
-        yield ids, entries
+        if ids:
+            yield ids, entries
+        if len(ids) < want:
+            return
 
 
 class Qwen2ForCausalLM(nn.Module):
@@ -614,9 +620,12 @@ class Qwen2ForCausalLM(nn.Module):
 
     def _generate_greedy(self, emb: torch.Tensor, max_new: int, eos_ids: List[int],
                          check_every: int = 16, sp_runner=None,
-                         sampling: Optional[SamplingParams] = None) -> List[int]:
-        """The graph decoder's loop: greedy, or sampled on the device with `sampling` (its seed set)."""
+                         sampling: Optional[SamplingParams] = None, grammar=None) -> List[int]:
+        """The graph decoder's loop: greedy, or sampled on the device with `sampling` (its seed set); constrained by
+        `grammar` (a matcher with xgrammar's GrammarMatcher interface, GraphDecoder.start) when given."""
         S = emb.shape[0]
+        if sp_runner is not None and grammar is not None:
+            raise NotImplementedError("sequence-parallel decode: grammar-constrained decoding is not implemented")
         dec = self.decoder(max_new)
         if sp_runner is not None:
             # sequence-parallel prefill (vila_b200/sp.py): every rank ends with the COMPLETE K/V in
@@ -637,7 +646,7 @@ class Qwen2ForCausalLM(nn.Module):
         else:
             cache = dec.cache_for(S + max_new)
             hid = self.prefill_hidden_graphed(emb, cache)
-            dec.start(hid[-1], cache, sampling)
+            dec.start(hid[-1], cache, sampling, **({} if grammar is None else {"grammar": grammar}))
         # without EOS ids nothing is read until the end: one chunk of max_new
         chunks = _decode_chunks(dec, max_new, check_every if eos_ids else max_new, eos_ids, ahead=False)
         return [t for ids, _ in chunks for t in ids]
@@ -651,14 +660,15 @@ class Qwen2ForCausalLM(nn.Module):
 
     def stream_tokens(self, emb: torch.Tensor, generation_config=None, chunk_tokens: int = 8,
                       max_new_tokens: Optional[int] = None, sampling: Optional[SamplingParams] = None,
-                      logprobs: Optional[int] = None, penalties: Optional[PenaltyParams] = None):
+                      logprobs: Optional[int] = None, penalties: Optional[PenaltyParams] = None, grammar=None):
         """stream_greedy, or with `sampling` (a SamplingParams with its seed set) the same loop sampled on the
         device: the ids are those of generate(do_sample=True) with the same parameters and seed.
         logprobs: None yields id lists; n in 0..20 yields (ids, [TokenLogprob ...]) per chunk, one entry per id (the
         token's log-probability under the raw row and its n most likely alternatives, vila_b200/logprobs.py),
         truncated at EOS as the ids are.  penalties: a PenaltyParams applies OpenAI's presence / frequency penalties
-        over the ids generated so far before each choice (vila_b200/penalties.py).  Both run on the device in the
-        graph decoder (GraphDecoder.start)."""
+        over the ids generated so far before each choice (vila_b200/penalties.py).  grammar: a matcher with xgrammar's
+        GrammarMatcher interface, whose token bitmask constrains every choice (vila_b200/grammar.py); the stream ends
+        when it terminates.  All run on the device in the graph decoder (GraphDecoder.start)."""
         if sampling is not None and not sampling.greedy and sampling.seed is None:
             raise ValueError("stream_tokens: sampling needs a seed")
         if logprobs is not None:
@@ -674,7 +684,8 @@ class Qwen2ForCausalLM(nn.Module):
             dec = self.decoder(max_new)
             cache = dec.cache_for(S + max_new)
             hid = self.prefill_hidden_graphed(emb, cache)
-            dec.start(hid[-1], cache, sampling, logprobs=logprobs, penalties=penalties)
+            dec.start(hid[-1], cache, sampling, logprobs=logprobs, penalties=penalties,
+                      **({} if grammar is None else {"grammar": grammar}))
             # read-ahead only with logprobs: it overlaps building their entries with decoding, and would otherwise
             # only add a chunk of decoding past EOS
             for ids, entries in _decode_chunks(dec, max_new, chunk_tokens, eos_ids, ahead=logprobs is not None):
@@ -743,6 +754,17 @@ class GraphDecoder:
     The rules are those of vila_b200/logprobs.py and vila_b200/penalties.py; token_logprobs() reads the entries back.
     Their buffers are allocated on first use; a request with neither option runs the greedy or sampled graph.
 
+    Grammar-constrained decoding (start(..., grammar=matcher), the rule of vila_b200/grammar.py) needs the matcher's
+    token bitmask on the device before each choice, and the matcher needs each id on the host before it can fill the
+    next mask.  So a constrained step is two graphs, keyed by _graph_key() + ("body",) / ("choose",):
+      body    the layers and lm_head writing the bf16 row
+      choose  [vila_apply_penalties_row] + vila_apply_token_bitmask_row + vila_sample_finalize (at inv_T = 0 the greedy
+              rule over the allowed ids) + [vila_token_logprobs_row on the raw row]
+    and the host loop for token t is: replay body(t); accept_token(t - 1); fill_next_token_bitmask into a pinned buffer
+    and copy it to the device; replay choose(t); copy the token back; replay body(t + 1); wait for the token.  The
+    matcher's host work overlaps the body, and the host's wait overlaps the next body (_run_constrained).  The loop
+    stops when the matcher terminates (the body replayed for the step after the stop token is not used).  A request without a grammar runs exactly its unconstrained graph.
+
     The decoder streams the weights of the LLM's decode-weight mode at construction
     (Qwen2ForCausalLM.set_decode_weights): in "fp8" mode every GEMV of start() and of each step, lm_head
     included, runs vila_gemv_fp8 on the e4m3 copies, so the first token is an fp8 lm_head result too.  In
@@ -791,6 +813,12 @@ class GraphDecoder:
         # logprobs / penalties buffers, allocated on first use (_ensure_logprobs / _ensure_penalties)
         self.lp_hist = self.top_ids = self.top_lp = self.lp_n = self.lp_ws = self.lp_counter = None
         self.pen_logits = self.presence = self.frequency = None
+        # grammar-constrained requests: the matcher, its mask buffers (allocated on first use, _ensure_grammar), the
+        # ids chosen so far (on the host) and whether the matcher has terminated
+        self.grammar = None
+        self.mask = self.mask_host = self.mask_np = self.masked = self.token_host = self.token_ready = None
+        self.grammar_ids: List[int] = []
+        self.finished = False
 
     def _graph_key(self):
         """what a step graph depends on besides the cache: the current request's mode and the attention plan"""
@@ -800,9 +828,10 @@ class GraphDecoder:
     def launches_per_step(self) -> int:
         """kernels of one decode step: 5 per layer (7 on the long-context path: RoPE/append, split-KV
         attention, combine) + lm_head GEMV + finalize (argmax or sample), in either mode; + 1 with penalties
-        (vila_apply_penalties_row) and + 1 with logprobs (vila_token_logprobs_row)"""
+        (vila_apply_penalties_row), + 1 with logprobs (vila_token_logprobs_row) and + 1 with a grammar
+        (vila_apply_token_bitmask_row)"""
         return ((7 if self.split_tokens else 5) * self.llm.config.num_hidden_layers + 2 + int(self.penalised)
-                + int(self.top_n is not None))
+                + int(self.top_n is not None) + int(self.grammar is not None))
 
     def _ensure_logprobs(self) -> None:
         if self.lp_hist is None:
@@ -819,6 +848,35 @@ class GraphDecoder:
             self.pen_logits = torch.zeros_like(self.logits)
             self.presence = torch.zeros(1, device=dev, dtype=torch.float32)
             self.frequency = torch.zeros(1, device=dev, dtype=torch.float32)
+
+    def _ensure_grammar(self) -> None:
+        if self.mask is None:
+            dev, W = self.llm.device, grammar_rule.bitmask_words(self.logits.numel())
+            self.mask = torch.zeros(W, device=dev, dtype=torch.int32)
+            self.mask_host = torch.zeros(1, W, dtype=torch.int32, pin_memory=True)
+            self.mask_np = self.mask_host.numpy()
+            self.masked = torch.zeros_like(self.logits)
+            self.token_host = torch.zeros(1, dtype=torch.int32, pin_memory=True)
+            self.token_ready = torch.cuda.Event()
+
+    def _fill_mask(self) -> None:
+        """the matcher's bitmask for the next token -> the device (asynchronous copy from pinned memory; the pinned
+        buffer is refilled only after _wait_token has waited for the step that follows this copy)"""
+        self.grammar.fill_next_token_bitmask(self.mask_host)
+        if not grammar_rule.any_allowed(self.mask_np, self.logits.numel()):
+            raise ValueError(f"GraphDecoder: the grammar allows no token after {len(self.grammar_ids)} tokens "
+                             "(an all-zero bitmask)")
+        self.mask.copy_(self.mask_host[0], non_blocking=True)
+
+    def _copy_token(self) -> None:
+        """enqueue the copy of the token just chosen to pinned memory, and an event after it"""
+        self.token_host.copy_(self.token, non_blocking=True)
+        self.token_ready.record()
+
+    def _wait_token(self) -> None:
+        """wait for _copy_token's event -> grammar_ids"""
+        self.token_ready.synchronize()
+        self.grammar_ids.append(int(self.token_host[0]))
 
     LONG_CTX = 1024  # above: the wgmma split-KV path
 
@@ -879,22 +937,24 @@ class GraphDecoder:
     def _lm_head(self):
         """the bf16 row when a kernel after lm_head reads it, the fused argmax key when argmax_finalize chooses (greedy
         + logprobs: both, from the same values)"""
-        chooses_from_row = self.sampled or self.penalised
+        chooses_from_row = self.sampled or self.penalised or self.grammar is not None
         row = chooses_from_row or self.top_n is not None
         ops.gemv(self.x, norm_w=self.llm.model.norm.weight, norm_eps=self.llm.config.rms_norm_eps,
                  out=self.logits if row else None, write_out=row,
                  argmax_key=None if chooses_from_row else self.key, static_w=True, **self._weights(None))
 
     def _finalize(self):
-        """the token (arg-max, or the draw in sampled mode; from the penalised row with penalties) -> history, step++,
-        position++, next x; then the token's logprobs on the raw row when they are on"""
+        """the token (arg-max, or the draw in sampled mode; from the penalised and / or grammar-masked row when those
+        are on) -> history, step++, position++, next x; then the token's logprobs on the raw row when they are on"""
         emb = self.llm.model.embed_tokens.weight
+        row = self.logits
         if self.penalised:
-            ops.apply_penalties_row(self.logits, self.hist, self.step, self.presence, self.frequency,
-                                    out=self.pen_logits)
-        if self.sampled or self.penalised:
-            ops.sample_finalize(self.pen_logits if self.penalised else self.logits, self.inv_temperature, self.top_k,
-                                self.top_p, self.seed, self.step, self.token, self.hist, self.position, emb, self.x)
+            row = ops.apply_penalties_row(row, self.hist, self.step, self.presence, self.frequency, out=self.pen_logits)
+        if self.grammar is not None:
+            row = ops.apply_token_bitmask_row(row, self.mask, out=self.masked)
+        if self.sampled or self.penalised or self.grammar is not None:
+            ops.sample_finalize(row, self.inv_temperature, self.top_k, self.top_p, self.seed, self.step, self.token,
+                                self.hist, self.position, emb, self.x)
         else:
             ops.argmax_finalize(self.key, self.token, self.hist, self.step, self.position, emb, self.x)
         if self.top_n is not None:  # n = self.lp_n, a device scalar: one graph for every n
@@ -903,6 +963,11 @@ class GraphDecoder:
                                    n_used=self.lp_n)
 
     def _step(self):
+        self._body()
+        self._finalize()
+
+    def _body(self):
+        """the step up to the logits: the layers and lm_head"""
         llm, cfg, cache = self.llm, self.llm.config, self.cache
         Hq, Hkv, D = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
         for li, layer in enumerate(llm.model.layers):
@@ -924,24 +989,30 @@ class GraphDecoder:
                      norm_eps=cfg.rms_norm_eps, swiglu=True, out=self.act, static_w=True, **w_gu)
             ops.gemv(self.act, residual=self.x, out=self.x, static_w=True, **w_down)
         self._lm_head()
-        self._finalize()
 
     def start(self, last_hidden: torch.Tensor, cache: PagedKVCache, params: Optional[SamplingParams] = None, *,
-              logprobs: Optional[int] = None, penalties: Optional[PenaltyParams] = None) -> None:
+              logprobs: Optional[int] = None, penalties: Optional[PenaltyParams] = None, grammar=None) -> None:
         """Seed the loop from the prefill: first new token = argmax(lm_head(norm(last_hidden))), or with
         non-greedy `params` (seed set) the draw of token index 0 from those logits; the following steps
         run the matching graph.  params None or greedy: exactly the greedy path.
         logprobs: None, or n in 0..20: every token's log-probability and its n most likely alternatives under the raw
         row (vila_b200/logprobs.py), entry 0 from this first row (token_logprobs()).  penalties: a PenaltyParams,
         applied to every row before the choice (vila_b200/penalties.py; the first token's history is empty, so its row
-        is unchanged); None or both values 0 is the path without them.  Neither works with a sequence-parallel
-        cache (NotImplementedError)."""
+        is unchanged); None or both values 0 is the path without them.  grammar: a matcher with xgrammar's
+        GrammarMatcher interface (fill_next_token_bitmask, accept_token, is_terminated) whose token bitmask masks every
+        row before the choice (vila_b200/grammar.py); its bitmask width must be ceil(V / 32) for this model's V.  The
+        first token's mask is filled here, before the first row is computed; an all-zero mask is a ValueError and an id
+        the matcher does not accept a RuntimeError.  None of these works with a sequence-parallel cache
+        (NotImplementedError)."""
         assert cache is self.cache
         top_n = None if logprobs is None else check_top(logprobs)
         penalised = penalties is not None and not penalties.off
         if (top_n is not None or penalised) and getattr(self, "_order_key", None) is not None:
             raise NotImplementedError("sequence-parallel decode: logprobs and penalties are not implemented")
+        if grammar is not None and getattr(self, "_order_key", None) is not None:
+            raise NotImplementedError("sequence-parallel decode: grammar-constrained decoding is not implemented")
         self.top_n, self.penalised = top_n, penalised
+        self.grammar, self.grammar_ids, self.finished = grammar, [], False
         if top_n is not None:
             self._ensure_logprobs()
             self.lp_n.fill_(top_n)
@@ -950,8 +1021,8 @@ class GraphDecoder:
             self.presence.fill_(penalties.presence)
             self.frequency.fill_(penalties.frequency)
         self.sampled = params is not None and not params.greedy
-        if penalised and not self.sampled:
-            self.inv_temperature.fill_(0.0)  # vila_sample_finalize's greedy rule on the penalised row
+        if (penalised or grammar is not None) and not self.sampled:
+            self.inv_temperature.fill_(0.0)  # vila_sample_finalize's greedy rule on the penalised / masked row
         if self.sampled:
             if params.seed is None:
                 raise ValueError("GraphDecoder.start: sampling needs a seed (serving.sampling_for_requests draws one)")
@@ -963,8 +1034,14 @@ class GraphDecoder:
         self.key.zero_()
         self.position.fill_(cache.length - 1)  # finalize increments -> position of the new token
         self.x.copy_(last_hidden)
+        if grammar is not None:
+            self._ensure_grammar()
+            self._fill_mask()
         self._lm_head()
         self._finalize()
+        if grammar is not None:
+            self._copy_token()
+            self._wait_token()
         self._started = 1
 
     def run(self, n_tokens: int) -> None:
@@ -975,17 +1052,50 @@ class GraphDecoder:
             self._started = 2
         if n <= 0:
             return
-        key = self._graph_key()
+        if self.grammar is not None:
+            self._run_constrained(n)
+            return
+        g = self._graph(self._graph_key(), self._step)
+        for _ in range(n):
+            g.replay()
+        self.cache.length += n
+
+    def _graph(self, key, body):
         g = self.graphs.get(key)
         if g is None:
             # warm-up launch outside capture is not allowed to change state: capture directly
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                self._step()
+                body()
             self.graphs[key] = g
-        for _ in range(n):
-            g.replay()
-        self.cache.length += n
+        return g
+
+    def _run_constrained(self, n: int) -> None:
+        """up to n more tokens of a grammar-constrained request, one host round trip each (see the class docstring);
+        fewer when the matcher terminates, which sets `finished`.  Within the call, body(t + 1) is enqueued right after
+        choose(t) and before the host waits for token t: it reads only device state (the token's embedding that
+        choose(t) writes), so the device does not idle while the host wakes up, accepts the token and fills the next
+        mask.  The first body of each call is enqueued by the call itself."""
+        if self.finished:
+            return
+        key = self._graph_key()
+        body, choose = self._graph(key + ("body",), self._body), self._graph(key + ("choose",), self._finalize)
+        m = self.grammar
+        body.replay()
+        for i in range(n):
+            if not m.accept_token(self.grammar_ids[-1]):
+                raise RuntimeError(f"GraphDecoder: the grammar matcher rejected token {self.grammar_ids[-1]}, which "
+                                   "its own bitmask allowed")
+            if m.is_terminated():
+                self.finished = True
+                return
+            self._fill_mask()
+            choose.replay()
+            self._copy_token()
+            if i + 1 < n:
+                body.replay()
+            self._wait_token()
+            self.cache.length += 1
 
     def tokens(self, n: int) -> List[int]:
         return self.hist[:n].tolist()
@@ -1006,6 +1116,12 @@ class GraphDecoder:
         reads ahead, are copied by the function with a plain blocking copy."""
         n = self.top_n
         a, b = max(0, start), min(n_tokens, self.hist.numel())
+        if self.grammar is not None:  # the ids are on the host already, and there may be fewer than asked for
+            b = min(b, len(self.grammar_ids))
+            a = min(a, b)
+            if n is None:
+                ids = self.grammar_ids[a:b]
+                return lambda: (ids, None)
         if n is None:
             return lambda: (self.hist[a:b].tolist(), None)
         if a >= b:

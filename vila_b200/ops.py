@@ -871,6 +871,30 @@ def apply_penalties_row(logits: torch.Tensor, history: torch.Tensor, step: torch
     return out
 
 
+def apply_token_bitmask_row(logits: torch.Tensor, bitmask: torch.Tensor, *, out: torch.Tensor) -> torch.Tensor:
+    """The single-stream decoder's logits row masked by a grammar matcher's token bitmask (vila_apply_token_bitmask_row,
+    one launch; the rule of vila_b200/grammar.py): out[j] = logits[j] where bit j % 32 of bitmask[j // 32] is set,
+    -inf elsewhere.  logits: a contiguous bf16 row [V]; bitmask: contiguous int32 with at least ceil(V / 32) words
+    (xgrammar's layout; bits at or above V are ignored); out: a contiguous bf16 [V] buffer, logits itself for in
+    place.  -> out"""
+    _need(logits.dim() == 1 and logits.is_contiguous() and logits.numel() >= 1,
+          f"apply_token_bitmask_row: logits must be a contiguous [V] row, got {tuple(logits.shape)}")
+    V = logits.numel()
+    W = (V + 31) // 32
+    _need(bitmask.is_contiguous() and bitmask.numel() >= W,
+          f"apply_token_bitmask_row: bitmask must be contiguous with at least {W} words, got {tuple(bitmask.shape)}")
+    _need(out.shape == (V,) and out.is_contiguous(),
+          f"apply_token_bitmask_row: out must be a contiguous [{V}] buffer, got {tuple(out.shape)}")
+    arrays = [(logits, "logits", torch.bfloat16), (bitmask, "bitmask", torch.int32), (out, "out", torch.bfloat16)]
+    for t, name, dt in arrays:
+        _need(t.dtype == dt, f"apply_token_bitmask_row: {name} must be {dt}, got {t.dtype}")
+    for t, name, _ in arrays:
+        _chk(t, name, t.dtype)
+    check(_lib.load().vila_apply_token_bitmask_row(_p(logits), _p(bitmask), _p(out), V, _stream()),
+          "vila_apply_token_bitmask_row")
+    return out
+
+
 def prefix_block_hash(x: torch.Tensor, key0: int, key1: int) -> torch.Tensor:
     """The 128-bit digest of every full 128-row block of x [rows, cols] bf16 (unit column stride, any row stride that
     is a multiple of 4; cols a multiple of 4) under the 64-bit keys key0 / key1, by the rule of

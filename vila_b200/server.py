@@ -20,6 +20,12 @@ request with logprobs or a non-zero penalty is decoded by the single-stream grap
 `stream_content`, which computes both on the device as well: each SSE chunk carries `choices[0].logprobs.content` for
 the ids it was decoded from (every id once, in order, the stop token excluded), even when those ids decode to no text.
 With a model that has no `stream_content`, such streaming requests are refused.
+A request with a `response_format` of type `json_object` or `json_schema` (structured output), streamed or not, is
+decoded alone by the single-stream graph decoder through `stream_content(..., response_format=...)`, which masks every
+logits row with the grammar's token bitmask on the device (vila_b200/grammar.py); it never joins a batch, and it
+combines with --sample, logprobs and penalties.  A non-streaming one gets the chunks collected into one
+`chat.completion`.  `type: "text"` is no constraint, as in OpenAI's API.  A schema that is not JSON, or that the model's
+grammar compiler rejects, fails the request before anything is decoded or streamed.
 
     python -m vila_b200.server --model-path <dir> --port 8000
 """
@@ -37,6 +43,8 @@ from io import BytesIO
 from typing import Any, Dict, List, Literal, Optional, Union
 
 from pydantic import BaseModel
+
+from llava.model.configuration_llava import ResponseFormat
 
 IMAGE_B64 = re.compile(r"^data:image/(png|jpe?g);base64,(.*)$")
 VIDEO_B64 = re.compile(r"^data:video/(mp4);base64,(.*)$")
@@ -82,6 +90,7 @@ class ChatCompletionRequest(BaseModel):
     top_logprobs: Optional[int] = None
     presence_penalty: Optional[float] = 0.0
     frequency_penalty: Optional[float] = 0.0
+    response_format: Optional[ResponseFormat] = None
 
 
 def load_image(url: str):
@@ -185,6 +194,9 @@ class Engine:
             raise ValueError(f"The endpoint is configured to use the model {self.model_name}, "
                              f"but the request model is {req.model}")
         # checked before the request joins a batch: a bad value fails this request only
+        rf = self._response_format(req)
+        if rf is not None:
+            return await self._complete_constrained(req, rf)
         params = self._sampling(req) if self.sample else None
         top = self._top_logprobs(req)
         if top is not None and not hasattr(self.model, "generate_batch"):
@@ -212,11 +224,64 @@ class Engine:
                         if not b[1].done():
                             b[1].set_result(res)
         text, content = await fut
+        return self._completion(req, text, content)
+
+    @staticmethod
+    def _completion(req: ChatCompletionRequest, text: str, content) -> Dict[str, Any]:
         choice = {"message": {"role": "assistant", "content": text}}
         if content is not None:
             choice["logprobs"] = {"content": content}
         return {"id": uuid.uuid4().hex, "object": "chat.completion", "created": int(time.time()),
                 "model": req.model, "index": 0, "choices": [choice]}
+
+    def _response_format(self, req: ChatCompletionRequest):
+        """a request's ResponseFormat, None for none or type "text"; a json_schema without a schema or a schema that
+        is not a JSON document raises.  Cheap: the grammar is compiled in a worker thread (check_stream, or the
+        decode's own executor call for a non-streaming request)"""
+        rf = req.response_format
+        if rf is None or rf.type == "text":
+            return None
+        if not hasattr(self.model, "stream_content"):
+            raise ValueError("response_format needs a model with stream_content (the graph decoder applies the "
+                             "grammar)")
+        if rf.type == "json_schema":
+            if rf.json_schema is None:
+                raise ValueError("response_format of type json_schema needs json_schema.schema")
+            try:
+                json.loads(rf.json_schema.schema_)
+            except ValueError as e:
+                raise ValueError(f"response_format: the schema is not valid JSON: {e}") from None
+        return rf
+
+    async def check_stream(self, req: ChatCompletionRequest) -> None:
+        """a streaming request's values, checked before its stream starts: sampling, logprobs and penalties
+        (_stream_config), and its response_format, whose grammar is compiled here in a worker thread, so a schema the
+        model's grammar compiler rejects fails the request first and the event loop is not blocked while it compiles
+        (the compiler caches the result for the decode)"""
+        self._stream_config(req)
+        rf = self._response_format(req)
+        if rf is not None and hasattr(self.model, "compile_response_format"):
+            await asyncio.get_running_loop().run_in_executor(None, self.model.compile_response_format, rf)
+
+    async def _complete_constrained(self, req: ChatCompletionRequest, rf) -> Dict[str, Any]:
+        """a non-streaming request with a response_format: decoded alone under the lock by stream_content in a worker
+        thread, its chunks collected into one completion.  The grammar is compiled there too, before anything is
+        decoded, so a schema the compiler rejects fails the request without blocking the event loop"""
+        gc = self._stream_config(req)
+        top, pen = self._top_logprobs(req), self._penalties(req)
+
+        def run():
+            ids, entries = [], []
+            for chunk, chunk_entries in self.model.stream_content(build_prompt(req.messages), generation_config=gc,
+                                                                  logprobs=top, penalties=pen, response_format=rf):
+                ids += chunk
+                entries += chunk_entries or []
+            text = self.model.tokenizer.decode(ids, skip_special_tokens=True).strip()
+            return text, None if top is None else self._logprobs_content(ids, entries, top)
+
+        async with self.lock:
+            text, content = await asyncio.get_running_loop().run_in_executor(None, run)
+        return self._completion(req, text, content)
 
     @staticmethod
     def _top_logprobs(req: ChatCompletionRequest) -> Optional[int]:
@@ -332,11 +397,12 @@ class Engine:
             raise ValueError(f"The endpoint is configured to use the model {self.model_name}, "
                              f"but the request model is {req.model}")
         gc = self._stream_config(req)  # a bad value fails this request before it takes the lock
-        top, pen = self._top_logprobs(req), self._penalties(req)
-        if top is not None or pen is not None:
+        top, pen, rf = self._top_logprobs(req), self._penalties(req), self._response_format(req)
+        if top is not None or pen is not None or rf is not None:
+            kw = {} if rf is None else {"response_format": rf}  # as in _run_batch: only passed when asked for
             async with self.lock:
                 gen = self.model.stream_content(build_prompt(req.messages), generation_config=gc, logprobs=top,
-                                                penalties=pen)
+                                                penalties=pen, **kw)
                 for chunk_id, (ids, entries) in enumerate(gen):
                     text = self.model.tokenizer.decode(ids, skip_special_tokens=True)
                     content = None if top is None else self._logprobs_content(ids, entries, top)
@@ -371,7 +437,7 @@ def create_app(model, model_name: str, slots: int = 8, kv_cache: str = "bf16", s
     async def chat_completions(request: ChatCompletionRequest):
         try:
             if request.stream:
-                engine._stream_config(request)  # bad sampling values: this request's error, before streaming starts
+                await engine.check_stream(request)  # bad values or schemas fail this request before it streams
                 return StreamingResponse(engine.stream(request), media_type="text/event-stream")
             return await engine.complete(request)
         except Exception as e:  # the reference answers 500 with the message (server.py:302-306)
