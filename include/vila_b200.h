@@ -552,6 +552,29 @@ int vila_apply_token_bitmask_row(const void* logits, const int32_t* bitmask, voi
 int vila_prefix_block_hash(const void* x, int64_t ld, int64_t rows, int64_t cols, uint64_t key0, uint64_t key1,
                            uint64_t* out, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * test hooks (like vila_linear_cfg / vila_fmha_cfg): the programmatic-dependent-launch contract.  Every kernel
+ * above may become resident while its predecessor still runs; it must read nothing the predecessor produces, and
+ * write nothing the predecessor still reads, before its dependency wait.  These two entry points let a test place
+ * a late-finishing producer right before any of them.
+ *
+ * vila_test_pdl_late — 8 CTAs that let their dependents launch at once, spin on the global timer for delay_ns
+ * (0 .. 2,000,000; a bounded loop), then copy every snap[i] range and then every late[i] range (src -> dst, bytes).
+ * snap / late are DEVICE arrays of n_snap / n_late (0 .. 64) entries, 8-byte aligned.  A range that is both
+ * snapshotted and written late must be given with the same (dst or src, bytes) in both lists: each of its bytes is
+ * then read by the thread that later overwrites it.  The argument errors are reported before any device call. */
+typedef struct vila_pdl_copy {
+  const void* src;
+  void* dst;
+  int64_t bytes;
+} vila_pdl_copy;
+int vila_test_pdl_late(const vila_pdl_copy* snap, int n_snap, const vila_pdl_copy* late, int n_late, int64_t delay_ns,
+                       void* stream);
+/* vila_test_pdl_probe — one thread: seen[0] = *flag before its dependency wait, seen[1] = *flag after (int32, device).
+ * *pdl_enabled (a HOST int, may be NULL) is set to 1 when this process launches with PDL (VILA_B200_NO_PDL unset or
+ * not starting with '1'), else 0; with flag and seen both NULL nothing is launched and no device is needed. */
+int vila_test_pdl_probe(const int32_t* flag, int32_t* seen, int* pdl_enabled, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

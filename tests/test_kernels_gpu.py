@@ -148,24 +148,39 @@ def test_linear_qkv_rope_fused_equals_two_kernels(cuda, M):
 
 def test_linear_chain_under_pdl(cuda):
     """Back-to-back dependent kernels (programmatic dependent launch): every consumer must wait for
-    its producer; weights flagged static may be fetched early."""
+    its producer; weights flagged static may be fetched early.  The chained run must equal, bit for
+    bit, the same calls separated by synchronizes (and both must match the fp32 oracle)."""
     ops = _ops()
     g = torch.Generator(device="cuda").manual_seed(78)
     x = bf(torch.randn(300, 1024, device=cuda, generator=g))
     ws_ = [bf(torch.randn(1024, 1024, device=cuda, generator=g) / 32) for _ in range(6)]
     nw = bf(torch.ones(1024, device=cuda))
-    h = x
+
+    def chain(sync):
+        h = x
+        for w in ws_:
+            h = ops.linear(ops.rmsnorm(h.clone(), nw, 1e-6), w, static_w=True)
+            if sync:
+                torch.cuda.synchronize()
+        y = x.clone()
+        for w in ws_:
+            ops.linear(y.clone(), w, residual=y, out=y, static_w=True)
+            if sync:
+                torch.cuda.synchronize()
+        return h, y
+
+    torch.cuda.synchronize()
+    h_sync, y_sync = chain(True)
+    h, y = chain(False)
+    torch.cuda.synchronize()
+    assert torch.equal(h, h_sync) and torch.equal(y, y_sync)
     ref = x.float()
-    for w in ws_:
-        h = ops.linear(ops.rmsnorm(h.clone(), nw, 1e-6), w, static_w=True)
-        ref = rb(O.rms_norm(ref.to(torch.bfloat16), nw, 1e-6).float() @ w.float().t())
-    assert rel_err(h, ref) < 3e-2
-    # in-place residual chains (out aliases residual)
-    y = x.clone()
     r = x.float()
     for w in ws_:
-        ops.linear(y.clone(), w, residual=y, out=y, static_w=True)
+        ref = rb(O.rms_norm(ref.to(torch.bfloat16), nw, 1e-6).float() @ w.float().t())
         r = rb(rb(r @ w.float().t()) + r)
+    assert rel_err(h, ref) < 3e-2
+    # in-place residual chains (out aliases residual)
     assert rel_err(y, r) < 3e-2
 
 

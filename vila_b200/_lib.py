@@ -177,6 +177,8 @@ SIGNATURES = {
     "vila_apply_penalties_row": [C.POINTER(PenaltyRowParams), c_void_p],
     "vila_apply_token_bitmask_row": [c_void_p, c_void_p, c_void_p, C.c_int32, c_void_p],
     "vila_prefix_block_hash": [c_void_p, c_i64, c_i64, c_i64, C.c_uint64, C.c_uint64, c_void_p, c_void_p],
+    "vila_test_pdl_late": [c_void_p, c_int, c_void_p, c_int, c_i64, c_void_p],
+    "vila_test_pdl_probe": [c_void_p, c_void_p, C.POINTER(c_int), c_void_p],
 }
 _RESTYPES = {"vila_last_error": C.c_char_p}
 

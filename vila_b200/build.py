@@ -33,6 +33,7 @@ SOURCES = [
     "penalties.cu",
     "logprobs_row.cu",
     "token_bitmask.cu",
+    "pdl_test.cu",
 ]
 HEADERS = ["common.cuh", "wgmma.cuh", "kernels.h", "../../include/vila_b200.h"]
 

@@ -367,4 +367,20 @@ int vila_prefix_block_hash(const void* x, int64_t ld, int64_t rows, int64_t cols
   return vb::prefix_block_hash(x, ld, rows, cols, key0, key1, out, st(stream));
 }
 
+// test hooks: no reference seam (the reference launches without programmatic dependent launch)
+int vila_test_pdl_late(const vila_pdl_copy* snap, int n_snap, const vila_pdl_copy* late, int n_late, int64_t delay_ns,
+                       void* stream) {
+  if (int rc = vb::pdl_late_check(snap, n_snap, late, n_late, delay_ns)) return rc;
+  VB_REQUIRE_DEVICE();
+  return vb::pdl_late(snap, n_snap, late, n_late, delay_ns, st(stream));
+}
+
+int vila_test_pdl_probe(const int32_t* flag, int32_t* seen, int* pdl_enabled, void* stream) {
+  if (int rc = vb::pdl_probe_check(flag, seen)) return rc;
+  if (pdl_enabled != nullptr) *pdl_enabled = vb::pdl_enabled() ? 1 : 0;
+  if (flag == nullptr) return 0;
+  VB_REQUIRE_DEVICE();
+  return vb::pdl_probe(flag, seen, st(stream));
+}
+
 }  // extern "C"

@@ -10,6 +10,14 @@
 
 namespace vb {
 
+// PDL contract of every launcher below (tests/test_pdl_gpu.py holds one case per entry point): every argument is
+// PRODUCED (read, and every output written, only after griddep_wait) except these STATIC ones, which may be read
+// before it:
+//   gemm_bf16 / gemm_qkv_rope_bf16 / gemm_bf16_cfg   W when epi.static_w (its first stages, single-CTA tiles only)
+//   gemv_* / gemv_batch_*                            with flags bit 1: w, norm_w, w_scale, w_gscale / w_zero
+//   decode_attention (head kernel), decode_attention_batch, decode_attention_fp8_batch   the page table
+// Everything else (activations, positions, step counters, tokens, K/V pools, work buffers, counters) is produced.
+
 enum Act : int { ACT_NONE = 0, ACT_GELU_TANH = 1, ACT_GELU_ERF = 2, ACT_SILU = 3 };
 
 struct GemmEpilogue {
@@ -203,6 +211,14 @@ int apply_token_bitmask_row(const void* logits, const int32_t* bitmask, void* ou
 int prefix_block_hash_check(const void* x, int64_t ld, int64_t rows, int64_t cols, const uint64_t* out);
 int prefix_block_hash(const void* x, int64_t ld, int64_t rows, int64_t cols, uint64_t key0, uint64_t key1,
                       uint64_t* out, cudaStream_t stream);
+
+// ---- test hooks for the PDL contract (pdl_test.cu) ------------------------------------------------------------
+// a late producer (triggers at once, spins delay_ns, snapshots, then writes the late inputs) and the probe control
+int pdl_late_check(const vila_pdl_copy* snap, int n_snap, const vila_pdl_copy* late, int n_late, int64_t delay_ns);
+int pdl_late(const vila_pdl_copy* snap, int n_snap, const vila_pdl_copy* late, int n_late, int64_t delay_ns,
+             cudaStream_t stream);
+int pdl_probe_check(const int32_t* flag, const int32_t* seen);
+int pdl_probe(const int32_t* flag, int32_t* seen, cudaStream_t stream);
 
 
 }  // namespace vb

@@ -911,3 +911,32 @@ def prefix_block_hash(x: torch.Tensor, key0: int, key1: int) -> torch.Tensor:
     check(_lib.load().vila_prefix_block_hash(_p(x), ld, rows, cols, key0, key1, _p(out), _stream()),
           "vila_prefix_block_hash")
     return out
+
+
+def pdl_late(snap: torch.Tensor, late: torch.Tensor, delay_ns: int) -> None:
+    """Test hook (vila_test_pdl_late): a producer that lets the next launch start at once, spins delay_ns on the device,
+    then copies every snap row and then every late row.  snap / late: int64 [n, 3] device tensors of (src, dst, bytes)
+    rows (vila_pdl_copy)."""
+    for t, name in ((snap, "snap"), (late, "late")):
+        _need(t.dtype == torch.int64 and t.dim() == 2 and t.shape[1] == 3 and t.is_contiguous(),
+              f"pdl_late: {name} must be a contiguous int64 [n, 3] tensor of (src, dst, bytes), got {tuple(t.shape)}")
+        _chk(t, name, torch.int64)
+    check(_lib.load().vila_test_pdl_late(_p(snap), snap.shape[0], _p(late), late.shape[0], delay_ns, _stream()),
+          "vila_test_pdl_late")
+
+
+def pdl_probe(flag: torch.Tensor, seen: torch.Tensor) -> None:
+    """Test hook (vila_test_pdl_probe): seen[0] = flag[0] before the kernel's dependency wait, seen[1] = flag[0] after."""
+    for t, name in ((flag, "flag"), (seen, "seen")):
+        _need(t.dtype == torch.int32, f"pdl_probe: {name} must be int32, got {t.dtype}")
+        _chk(t, name, torch.int32)
+    _need(seen.numel() >= 2, "pdl_probe: seen needs two entries")
+    check(_lib.load().vila_test_pdl_probe(_p(flag), _p(seen), None, _stream()), "vila_test_pdl_probe")
+
+
+def pdl_enabled() -> bool:
+    """Whether this process launches its kernels with programmatic dependent launch (VILA_B200_NO_PDL unset or not
+    starting with '1'); read once per process.  Needs no device."""
+    on = C.c_int(-1)
+    check(_lib.load().vila_test_pdl_probe(None, None, C.byref(on), None), "vila_test_pdl_probe")
+    return on.value == 1
